@@ -2,13 +2,18 @@
 """Benchmark of the NES generation hot path (BASELINE.json: generations/s and policy-evals/s, pop 64k).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                    [--pop 65536] [--hidden 256] [--tape-len 256] [--precision fp32|f16|f16x3]
+                    [--pop 65536] [--hidden 256] [--tape-len 256] [--precision fp32|f16|f16x3] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...      (one rank per GPU, NCCL)
 
 A "step" is one NES generation (natural_es.py:62-96) over synthetic inputs: sample eps for the whole
 population, batched policy forward over population x tape, centered ranks, fitness x noise reduction,
 (1-wd)/Adam/step.  The population is fixed as GPUs are added (strong scaling, as BASELINE.json quotes
-the metric "at pop 64k, 1/2/4/8 B200").  Prints ONE JSON line on rank 0.
+the metric "at pop 64k, 1/2/4/8 GPUs").  Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR writes what the last timed generation of the headline workload handed to its caller (fitness_all,
+shaped, partial, update, theta) as DIR/<name>.npy in float32, at most 64 MB in all (a fixed seeded sample of an array
+too long for its share).  The inputs are seeded, so two builds run with the same arguments can be compared output for
+output.
 
   value        policy-evals/s of the headline workload with everything resident in HBM (generations/s = value / pop)
   e2e          same metric through the host-buffer API (tape H2D, theta+fitness D2H inside the timed region)
@@ -61,6 +66,8 @@ def parse():
     ap.add_argument('--cpu-sample', type=int, default=0, help='members per CPU-baseline step (0 = auto)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed generation of the headline workload as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -73,10 +80,27 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), float(d.get('bf16_tflops', 0.0)), float(d.get('bf16_tflops_sustained', 0.0)), 'measured'
-    return 6650.0, 1590.0, 1400.0, 'fallback'
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; no sustained figure without a measurement
+    return 3350.0, 989.0, 0.0, 'data sheet'
 
 
-FP32_FFMA_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12      # 148 SMs x 128 FFMA/clk x 1.965 GHz = 74.4 (nominal CUDA-core peak)
+FP32_FFMA_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12       # H100 SXM: 132 SMs x 128 FFMA/clk x 1.98 GHz = 66.9 (nominal CUDA-core peak)
+
+
+DUMP_NAMES = ('fitness_all', 'shaped', 'partial', 'update', 'theta')
+DUMP_MAX_ELEMS = (64 << 20) // (4 * len(DUMP_NAMES))     # 64 MB in all, float32
+
+
+def dump_outputs(eng, out_dir):
+    """The arrays a caller of NESEngine.generation() reads after a step, as float32 .npy files (1.4 MB for the headline
+    workload).  An array longer than DUMP_MAX_ELEMS is replaced by a fixed sample: the entries at the sorted indices
+    RandomState(0).choice(len, DUMP_MAX_ELEMS, replace=False), the same for every run of the same shape."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in DUMP_NAMES:
+        arr = getattr(eng, name).detach().float().cpu().numpy().ravel()
+        if arr.size > DUMP_MAX_ELEMS:
+            arr = arr[np.sort(np.random.RandomState(0).choice(arr.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), arr)
 
 
 # --------------------------------------------------------------------------------------------------------
@@ -234,7 +258,7 @@ class ClockSampler:
 
 
 def build_hash():
-    """Identity of the library the numbers were taken on (keys profiles/roofline_traffic.json)."""
+    """Identity of the library the numbers were taken on."""
     import hashlib
     try:
         from distributedes_b200 import _lib
@@ -265,7 +289,7 @@ def run_ours(a):
         print('bench.py: --gpus %d but WORLD_SIZE=%d; using WORLD_SIZE' % (a.gpus, world), file=sys.stderr)
 
     hbm_peak, bf16_peak, bf16_sustained, peak_kind = peaks()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2 (H100)
 
     def barrier():
         if world > 1:
@@ -293,14 +317,6 @@ def run_ours(a):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    traffic_table = {}
-    tp = os.path.join(REPO, 'profiles', 'roofline_traffic.json')
-    if os.path.exists(tp):
-        try:
-            traffic_table = json.load(open(tp))
-        except Exception:
-            traffic_table = {}
-
     def make_engine(d0, H, A, T, N, precision):
         env = TapeEnv(d0, A, T)
         theta0 = StandardFCNet(d0, A, H, seed=0).get_weight()
@@ -309,13 +325,15 @@ def run_ours(a):
                         device=dev, use_graph=not a.no_graph)
         return eng, env, theta0
 
-    def measure_nes(d0, H, A, T, N, precision, steps, warmup):
+    def measure_nes(d0, H, A, T, N, precision, steps, warmup, dump=None):
         """Device-resident generations of one configuration + its dominant kernel alone -> (dict, engine, env)."""
         eng, env, _ = make_engine(d0, H, A, T, N, precision)
         P = eng.P
         for _ in range(max(warmup, 3)):
             eng.generation()
         total_ms, _ = timed(eng.generation, steps)
+        if dump and rank == 0:
+            dump_outputs(eng, dump)
         ms_per_step = max_over_ranks(total_ms) / steps
 
         def eval_only():
@@ -349,27 +367,26 @@ def run_ours(a):
         fwd_flops = 2.0 * eng.n_local * T * (d0 * H + H * H + H * A)
         tf = fwd_flops / (ev_ms * 1e-3) / 1e12
         gbs = alg_bytes / (ev_ms * 1e-3) / 1e9
-        traffic = traffic_table.get('%s_H%d_n%d' % (precision, H, eng.n_local))
         tensor_path = precision in ('f16', 'f16x3')
         if tensor_path:
             roofline = {'kernel': 'des_nes_eval[%s]' % precision, 'bound': 'tensor', 'achieved': tf, 'peak': bf16_peak,
                         'unit': 'TFLOP/s', 'frac': tf / bf16_peak if bf16_peak else None,
-                        'peak_kind': 'of %s bf16 burst (cuBLAS)' % peak_kind,
+                        'peak_kind': 'of %s bf16 peak' % peak_kind,
                         'frac_of_sustained_peak': tf / bf16_sustained if bf16_sustained else None,
                         'algorithmic_flops_per_launch': fwd_flops,
                         'tensor_issued_frac': (3.0 if precision == 'f16x3' else 1.0) * tf / bf16_peak if bf16_peak else None}
         else:
             roofline = {'kernel': 'des_nes_eval[fp32]', 'bound': 'fp32 CUDA cores', 'achieved': tf, 'peak': FP32_FFMA_TFLOPS,
-                        'unit': 'TFLOP/s', 'frac': tf / FP32_FFMA_TFLOPS, 'peak_kind': 'nominal 148 x 128 FFMA/clk x 1.965 GHz',
+                        'unit': 'TFLOP/s', 'frac': tf / FP32_FFMA_TFLOPS, 'peak_kind': 'nominal 132 x 128 FFMA/clk x 1.98 GHz',
                         'algorithmic_flops_per_launch': fwd_flops}
         roofline.update({
-            'traffic': traffic, 'kernel_ms': ev_ms, 'kernel_share_of_step': ev_ms / ms_per_step,
+            'kernel_ms': ev_ms, 'kernel_share_of_step': ev_ms / ms_per_step,
             'hbm_contract': {'achieved': gbs, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': gbs / hbm_peak,
                              'algorithmic_bytes_per_launch': alg_bytes,
                              'note': 'SURVEY 8d materialised-noise contract (8 n P bytes per launch); eps is regenerated '
                                      'in the kernel, so this is an effective figure and may exceed the HBM peak'},
-            'note': 'binding roof = tensor pipe: measured DRAM traffic (`traffic`, ncu, profiles/) is ~1e-5 of the HBM '
-                    'contract bytes; the kernel is limited by instruction issue / XU(MUFU) / tensor hand-overs (profiles/README.md)'})
+            'note': 'binding roof = tensor pipe: eps is regenerated in the kernel, so its DRAM traffic is a small fraction '
+                    'of the HBM contract bytes; the kernel is limited by instruction issue / XU(MUFU) / tensor hand-overs'})
         res = {'workload': workload_name(d0, H, A, T, N), 'pop': N, 'hidden': H, 'param_count': P, 'precision': precision,
                'n_gpus': world, 'members_per_gpu': eng.n_local, 'ms_per_step': ms_per_step,
                'value': N / (ms_per_step * 1e-3), 'unit': 'policy-evals/s', 'generations_per_sec': 1e3 / ms_per_step,
@@ -379,7 +396,7 @@ def run_ours(a):
     # ================================ headline workload ================================
     d0, H, A, T, N = a.state_dim, a.hidden, a.action_dim, a.tape_len, a.pop
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    main, eng, env = measure_nes(d0, H, A, T, N, a.precision, a.steps, a.warmup)
+    main, eng, env = measure_nes(d0, H, A, T, N, a.precision, a.steps, a.warmup, dump=a.dump_outputs)
     clocks = sampler.stop() if sampler else None
     P = eng.P
     ms_per_step, value, roofline = main['ms_per_step'], main['value'], main['roofline']
@@ -561,7 +578,7 @@ def parity_check(torch, dist, eng, world, dev):
 
 def cma_roofline(n, lam, lam_local, world):
     """Roofline of the rank-mu update's two kernels, timed separately on this rank (CUDA events): the SYRK
-    (tensor pipe when ops picks the split-fp16 tcgen05 path, fp32 CUDA cores below ops.CMA_TC_MIN_N) and the
+    (tensor pipe when ops picks the split-fp16 wgmma path, fp32 CUDA cores below ops.CMA_TC_MIN_N) and the
     HBM-bound covariance blend.  Flops counted as 2 lambda n^2 (the full square; the kernels compute the upper triangle)."""
     import torch
     from distributedes_b200 import ops
@@ -586,13 +603,13 @@ def cma_roofline(n, lam, lam_local, world):
     tf = 2.0 * lam_local * n * n / (t_mu * 1e-3) / 1e12
     peak = bf16_peak if tc else FP32_FFMA_TFLOPS
     gbs = 12.0 * n * n / (t_cov * 1e-3) / 1e9
-    return {'kernel': 'des_cma_rank_mu_tc (split-fp16 tcgen05 SYRK, TMA-fed)' if tc else 'des_cma_rank_mu (fp32 FFMA)',
+    return {'kernel': 'des_cma_rank_mu_tc (split-fp16 wgmma SYRK, TMA-fed)' if tc else 'des_cma_rank_mu (fp32 FFMA)',
             'bound': 'tensor' if tc else 'fp32 CUDA cores', 'achieved': tf, 'peak': peak, 'unit': 'TFLOP/s',
             'frac': tf / peak if peak else None,
-            'peak_kind': ('of %s bf16 burst (cuBLAS)' % peak_kind) if tc else 'nominal 148 x 128 FFMA/clk x 1.965 GHz',
-            'tensor_issued_frac': (3.0 * 0.5 * (1 + 256.0 / n) * tf / peak) if (tc and peak) else None,
+            'peak_kind': ('of %s bf16 peak' % peak_kind) if tc else 'nominal 132 x 128 FFMA/clk x 1.98 GHz',
+            'tensor_issued_frac': (3.0 * 0.5 * (1 + 128.0 / n) * tf / peak) if (tc and peak) else None,
             'kernel_ms': t_mu, 'members_this_rank': lam_local, 'n_gpus': world,
-            'note': 'flops counted as 2 lambda n^2; the kernel issues three MMAs per k-step over the 128x256 tiles that touch the upper triangle',
+            'note': 'flops counted as 2 lambda n^2; the kernel issues three MMAs per k-step over the 128x128 tiles that touch the upper triangle',
             'cov_apply': {'bound': 'hbm', 'achieved': gbs, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': gbs / hbm_peak if hbm_peak else None,
                           'kernel_ms': t_cov, 'algorithmic_bytes': 12.0 * n * n}}
 

@@ -1,4 +1,4 @@
-"""B200-native Evolution-Strategies hot path (NES population-evaluate-update loop + CMA-ES rank-mu update).
+"""H100-native (sm_90a) Evolution-Strategies hot path (NES population-evaluate-update loop + CMA-ES rank-mu update).
 
 Product code = csrc/*.cu behind the C ABI of include/des_b200.h (libdes_b200.so) + this thin host layer that
 keeps the reference's Worker / train() / test() / Evaluator.eval() / fitness_shift / Adam surface.

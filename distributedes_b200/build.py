@@ -1,4 +1,4 @@
-"""Build libdes_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libdes_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m distributedes_b200.build            # build if stale
     python -m distributedes_b200.build --force
@@ -15,9 +15,10 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'build')
 LIB = os.path.join(PKG, 'libdes_b200.so')
-SOURCES = ['des_capi.cu', 'des_noise.cu', 'des_eval_ffma.cu', 'des_eval_tc.cu', 'des_eval_pair.cu', 'des_rank.cu', 'des_update.cu',
+SOURCES = ['des_capi.cu', 'des_noise.cu', 'des_eval_ffma.cu', 'des_eval_tc.cu', 'des_rank.cu', 'des_update.cu',
            'des_cma.cu', 'des_cma_tc.cu', 'des_envs.cu', 'des_comm.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden']
 
 
@@ -61,7 +62,7 @@ def build_library(force=False, verbose=False):
                 print(log)
     objs = [os.path.join(OBJ, src[:-3] + '.o') for src in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+        cmd = [nvcc, '-shared'] + ARCH + ['-o', LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -33,7 +33,7 @@ size_t eval_tc_workspace_bytes(des_dims dims, int precision);
 }  // namespace des
 
 extern "C" DES_API const char *des_last_error(void) { return des::g_err; }
-extern "C" DES_API const char *des_version(void) { return "distributedes_b200 0.1 (sm_100a)"; }
+extern "C" DES_API const char *des_version(void) { return "distributedes_b200 0.1 (sm_90a)"; }
 
 extern "C" DES_API int des_device_count(void) {
     int n = 0;

@@ -3,14 +3,14 @@
 //
 //   Z  = diag(sqrt|w|) Y           (so that dC = Zs^T Z with Zs = diag(sign w) Z; both operands are O(|y|): no scaling)
 //   pre-pass   Y [lambda][n] fp32 -> Zs_hi, Zs_lo, Z_hi, Z_lo  [n][lambda_pad] fp16, k contiguous (K-major), x = hi + lo
-//   main       per 128 x 256 output tile touching the upper triangle:  D += A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T
-//              (tcgen05.mma kind::f16, fp32 accumulation in TMEM; the dropped lo*lo term is 2^-22 relative), operand
-//              tiles brought in by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) through a two-stage mbarrier pipeline:
-//              warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM allocation), warps 2-5 = epilogue (tcgen05.ld -> global)
+//   main       per 128 x 128 output tile touching the upper triangle:  D += A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T
+//              (wgmma m64n128k16, fp32 accumulation in registers; the dropped lo*lo term is 2^-22 relative), operand
+//              tiles brought in by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) through a three-stage mbarrier pipeline:
+//              warps 0-7 = two consumer warpgroups (64 output rows each: wgmma, then registers -> global), warp 8 = TMA
 //   output     the full symmetric matrix (upper entry written to both sides: exactly symmetric), or the packed
 //              upper-triangular tiles of des_cma_rank_mu_packed (the payload of the cross-rank sum)
 //
-// The fp32 FFMA kernel of des_cma.cu (36 % of the CUDA-core peak in round 1) stays as the small-n / no-workspace path.
+// The fp32 FFMA kernel of des_cma.cu stays as the small-n / no-workspace path.
 // Accuracy: measured against the fp64 restatement in tests/test_gpu_cma.py at the same 1e-5 (both norms) bar.
 #include <cuda.h>
 #include <stddef.h>
@@ -22,11 +22,11 @@ namespace cmatc {
 
 using namespace tc;
 
-constexpr int kBM = 128, kBN = 256, kBK = 64;
-constexpr int kStages = 2;
+constexpr int kBM = 128, kBN = 128, kBK = 64;
+constexpr int kStages = 3;
 constexpr int kABytes = kBM * kBK * 2, kBBytes = kBN * kBK * 2;
-constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;             // A_hi | A_lo | B_hi | B_lo = 96 KB
-constexpr int kThreads = 6 * 32;
+constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;             // A_hi | A_lo | B_hi | B_lo = 64 KB
+constexpr int kThreads = 9 * 32;
 
 // ---- pre-pass: transpose + scale + split --------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) cma_split_kernel(__half *__restrict__ zs_hi, __half *__restrict__ zs_lo,
@@ -65,37 +65,30 @@ struct Args {
     float *out;
     int64_t n;
     int k_stages;            // lambda_pad / 64
-    int tiles_m, tiles_n;    // 128-row and 256-column blocks
+    int tiles;               // 128-row (and 128-column) blocks per side
     int packed, ptile, ptiles_per_side;
 };
 
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, int c0, int c1, uint32_t bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// one lane of a fully converged warp: the loop around it runs on the whole warp so that every operand of the TMA / MMA
-// instructions is warp-uniform (inside `if (lane == 0)` ptxas wraps each of them in an ELECT / R2UR.BROADCAST loop)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
 struct Bars {
-    uint64_t full[kStages], empty[kStages], acc_full;
-    uint32_t tmem_base;
+    uint64_t full[kStages], empty[kStages];
 };
+
+__device__ __forceinline__ void store_out(const Args &a, int64_t i, int64_t j, float x) {
+    const int64_t n = a.n;
+    if (a.packed) {
+        // packed upper tiles of side ptile: element (i, j) lives in tile (i / ptile, j / ptile), bi' <= bj'; the tiles are
+        // padded to a multiple of their side and the padding is written too (zeros from the TMA fill)
+        const int64_t lim = (int64_t)a.ptiles_per_side * a.ptile;
+        const int64_t pb_i = i / a.ptile, pb_j = j / a.ptile;
+        if (i < lim && j < lim && pb_i <= pb_j) {
+            const int64_t t = pb_i * a.ptiles_per_side - pb_i * (pb_i - 1) / 2 + (pb_j - pb_i);
+            a.out[t * a.ptile * a.ptile + (i % a.ptile) * a.ptile + (j % a.ptile)] = x;
+        }
+    } else if (i < n && j < n && j >= i) {
+        a.out[i * n + j] = x;
+        if (j > i) a.out[j * n + i] = x;                // mirrored: exactly symmetric
+    }
+}
 
 __global__ void __launch_bounds__(kThreads, 1) cma_syrk_kernel(Args a, const __grid_constant__ CUtensorMap map_a_hi,
                                                                const __grid_constant__ CUtensorMap map_a_lo,
@@ -105,29 +98,21 @@ __global__ void __launch_bounds__(kThreads, 1) cma_syrk_kernel(Args a, const __g
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     Bars *bars = reinterpret_cast<Bars *>(smem + kStages * kStageBytes);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // tile (bi, bj): 128-row block bi, 256-column block bj >= bi / 2 (the blocks that touch the upper triangle)
+    // tile (bi, bj): 128-row block bi, 128-column block bj >= bi (the blocks that touch the upper triangle)
     int bi = 0, rem = blockIdx.x;
-    while (rem >= a.tiles_n - (bi >> 1)) { rem -= a.tiles_n - (bi >> 1); ++bi; }
-    const int bj = (bi >> 1) + rem;
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < kStages; ++s) {
-                mbar_init(smem_u32(&bars->full[s]), 1);
-                mbar_init(smem_u32(&bars->empty[s]), 1);
-            }
-            mbar_init(smem_u32(&bars->acc_full), 1);
-            fence_barrier_init();
+    while (rem >= a.tiles - bi) { rem -= a.tiles - bi; ++bi; }
+    const int bj = bi + rem;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(smem_u32(&bars->full[s]), 1);
+            mbar_init(smem_u32(&bars->empty[s]), 2);          // one arrival per consumer warpgroup
         }
-        __syncwarp();
-        tmem_alloc(smem_u32(&bars->tmem_base), 512);
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = bars->tmem_base;
 
     const uint32_t smem_addr = smem_u32(smem), bars_addr = smem_u32(bars);
-    if (warp == 0) {
+    if (warp == 8) {
         // ---- TMA producer (whole warp converged, one elected lane issues)
         for (int ks = 0; ks < a.k_stages; ++ks) {
             const int s = ks % kStages, use = ks / kStages;
@@ -143,88 +128,50 @@ __global__ void __launch_bounds__(kThreads, 1) cma_syrk_kernel(Args a, const __g
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ---- MMA issuer (whole warp converged, one elected lane issues)
-        constexpr uint32_t idesc = idesc_f16(kBM, kBN);
-        const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0);
-        for (int ks = 0; ks < a.k_stages; ++ks) {
-            const int s = ks % kStages, use = ks / kStages;
-            mbar_wait(bars_addr + (uint32_t)offsetof(Bars, full) + 8u * s, use & 1);
-            tc_fence_after();
-            const uint32_t base = smem_addr + (uint32_t)(s * kStageBytes);
-            if (elect_one()) {
+    } else {
+        // ---- consumer warpgroup wg: output rows [64 wg, 64 wg + 64) of the tile
+        const int wg = warp >> 2;
+        // two accumulators, one per half of K, added with round-to-nearest in the epilogue: the tensor cores
+        // truncate when they align the fp32 accumulator, which biases long sums of same-sign terms (the diagonal)
+        float acc0[64], acc1[64];
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc0[e] = acc1[e] = 0.f;
+        // K stages [k0, k1) into acc: one loop per half of K, so that the accumulator each wgmma names is fixed per loop
+        auto run_stages = [&](float (&acc)[64], int k0, int k1) {
+            for (int ks = k0; ks < k1; ++ks) {
+                const int s = ks % kStages, use = ks / kStages;
+                mbar_wait(bars_addr + (uint32_t)offsetof(Bars, full) + 8u * s, use & 1);
+                const uint32_t base = smem_addr + (uint32_t)(s * kStageBytes);
+                const uint32_t a_hi = base + wg * (kABytes / 2), a_lo = a_hi + kABytes;
+                const uint32_t b_hi = base + 2 * kABytes, b_lo = b_hi + kBBytes;
+                wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < kBK / 16; ++k) {
-                    const uint64_t ah = smem_desc_sw128(base) + (uint64_t)(k * 2);
-                    const uint64_t al = smem_desc_sw128(base + kABytes) + (uint64_t)(k * 2);
-                    const uint64_t bh = smem_desc_sw128(base + 2 * kABytes) + (uint64_t)(k * 2);
-                    const uint64_t bl = smem_desc_sw128(base + 2 * kABytes + kBBytes) + (uint64_t)(k * 2);
-                    // two accumulators, one per half of K, added with round-to-nearest in the epilogue: the tensor cores
-                    // truncate when they align the fp32 accumulator, which biases long sums of same-sign terms (the
-                    // diagonal: -7e-6 relative at K = 1024 with one accumulator)
-                    const int half = ks >= (a.k_stages + 1) / 2 ? 1 : 0;
-                    const bool first = (k == 0) && (ks == 0 || ks == (a.k_stages + 1) / 2);
-                    const uint32_t d = tm + (uint32_t)(half * kBN);
-                    mma_ss(d, ah, bh, idesc, !first);
-                    mma_ss(d, al, bh, idesc, 1);
-                    mma_ss(d, ah, bl, idesc, 1);
+                    wgmma_ss_n128(acc, smem_desc_sw128(a_hi + k * 32), smem_desc_sw128(b_hi + k * 32), 1);
+                    wgmma_ss_n128(acc, smem_desc_sw128(a_lo + k * 32), smem_desc_sw128(b_hi + k * 32), 1);
+                    wgmma_ss_n128(acc, smem_desc_sw128(a_hi + k * 32), smem_desc_sw128(b_lo + k * 32), 1);
                 }
-                mma_commit(bars_addr + (uint32_t)offsetof(Bars, empty) + 8u * s);
-                if (ks == a.k_stages - 1) mma_commit(bars_addr + (uint32_t)offsetof(Bars, acc_full));
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(acc);
+                // every MMA of this warpgroup that read the stage has completed: one arrival frees it for the producer
+                if ((threadIdx.x & 127) == 0) mbar_arrive(bars_addr + (uint32_t)offsetof(Bars, empty) + 8u * s);
             }
-            __syncwarp();
-        }
-    } else {
-        // ---- epilogue: TMEM lane quadrant = warp id % 4; lane = output row
-        mbar_wait(smem_u32(&bars->acc_full), 0);
-        tc_fence_after();
-        const int q = warp & 3;
-        const int64_t i = (int64_t)bi * kBM + q * 32 + lane;
-        const int64_t n = a.n;
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);
-        // packed tiles are padded to a multiple of their side: the padding must be written too (zeros from the TMA fill)
-        const int64_t jlimit = a.packed ? (int64_t)a.ptiles_per_side * a.ptile : n;
-        for (int c0 = 0; c0 < kBN; c0 += 32) {
-            const int64_t j0 = (int64_t)bj * kBN + c0;
-            if (j0 >= jlimit) break;                                  // warp-uniform
-            if (!a.packed && j0 + 31 < (int64_t)bi * kBM + q * 32) continue;   // whole chunk below the diagonal for every lane
-            uint32_t v[32];
-            tmem_ld32(taddr + (uint32_t)c0, v);
-            tmem_wait_ld();
-            if (a.k_stages > 1) {                                     // second half of K (its own accumulator)
-                uint32_t v2[32];
-                tmem_ld32(taddr + (uint32_t)(kBN + c0), v2);
-                tmem_wait_ld();
+        };
+        const int k_half = (a.k_stages + 1) / 2;
+        run_stages(acc0, 0, k_half);
+        run_stages(acc1, k_half, a.k_stages);
+        const int64_t i0 = (int64_t)bi * kBM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int64_t j0 = (int64_t)bj * kBN + (lane & 3) * 2;
 #pragma unroll
-                for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(v2[e]));
-            }
-            if (a.packed) {
-                // packed upper tiles of side ptile: element (i, j) lives in tile (i / ptile, j / ptile), bi' <= bj'
-                const int64_t pb_i = i / a.ptile, pb_j = j0 / a.ptile;
-                if (i < (int64_t)a.ptiles_per_side * a.ptile && pb_i <= pb_j) {
-                    const int64_t t = pb_i * a.ptiles_per_side - pb_i * (pb_i - 1) / 2 + (pb_j - pb_i);
-                    float4 *dst = reinterpret_cast<float4 *>(a.out + t * a.ptile * a.ptile + (i % a.ptile) * a.ptile + (j0 % a.ptile));
+        for (int jb = 0; jb < kBN / 8; ++jb) {
 #pragma unroll
-                    for (int e = 0; e < 8; ++e)
-                        dst[e] = make_float4(__uint_as_float(v[4 * e]), __uint_as_float(v[4 * e + 1]),
-                                             __uint_as_float(v[4 * e + 2]), __uint_as_float(v[4 * e + 3]));
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const int64_t j = j0 + e;
-                    const float x = __uint_as_float(v[e]);
-                    if (i < n && j < n && j >= i) {
-                        a.out[i * n + j] = x;
-                        if (j > i) a.out[j * n + i] = x;                // mirrored: exactly symmetric
-                    }
-                }
+            for (int e = 0; e < 4; ++e) {
+                const int64_t i = i0 + 8 * (e >> 1), j = j0 + 8 * jb + (e & 1);
+                store_out(a, i, j, acc0[4 * jb + e] + acc1[4 * jb + e]);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -295,12 +242,11 @@ extern "C" DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, co
     }
     Args a;
     a.out = out_dev; a.n = n; a.k_stages = (int)(lp / kBK);
-    a.tiles_m = (int)((n + kBM - 1) / kBM); a.tiles_n = (int)((n + kBN - 1) / kBN);
+    a.tiles = (int)((n + kBM - 1) / kBM);
     a.packed = packed ? 1 : 0;
     a.ptile = n <= 2048 ? 64 : 128;
     a.ptiles_per_side = (int)((n + a.ptile - 1) / a.ptile);
-    int64_t tiles = 0;
-    for (int bi = 0; bi < a.tiles_m; ++bi) tiles += a.tiles_n - (bi >> 1);
+    const int64_t tiles = (int64_t)a.tiles * (a.tiles + 1) / 2;
     const size_t smem = 1024 + (size_t)kStages * kStageBytes + sizeof(Bars);
     DES_CUDA(cudaFuncSetAttribute(cma_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cma_syrk_kernel<<<(unsigned)tiles, kThreads, smem, st>>>(a, maps[0], maps[1], maps[2], maps[3]);

@@ -1,5 +1,5 @@
 // Shared device helpers: Philox4x32-10 counter RNG, Box-Muller, error plumbing.
-// Target: sm_100a only.
+// Target: sm_90a (H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

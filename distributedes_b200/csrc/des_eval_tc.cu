@@ -1,38 +1,32 @@
 // des_nes_eval, precision DES_FWD_F16 / DES_FWD_F16X3: fused sample + perturb + forward + fitness with the two
-// hidden-layer GEMMs on tcgen05 tensor cores.
+// hidden-layer GEMMs on Hopper tensor cores (wgmma).
 //
-// One persistent CTA per SM (or one CTA PAIR per two SMs, see TcCfg) walks its members (Worker.run
-// natural_es.py:27-32 per member).  For a member and a tile of 128 observations (M = 128 rows = TMEM lanes),
-// StandardFCNet.forward (model.py:34-39) is
+// One persistent CTA per SM (or one 2-CTA cluster per two SMs, see below) walks its members (Worker.run
+// natural_es.py:27-32 per member).  A CTA has two warpgroups; each owns 64 observation rows of a 128-row tile (one
+// "pass" over the tape is one such tile).  For a member, StandardFCNet.forward (model.py:34-39) is
 //
-//   D1 = X  W1'^T            tcgen05.mma kind::f16, SS: A = X tile (fp16, shared memory, resident for the whole
-//                            kernel), B = W1' tiles (shared-memory ring)
-//   H1 = tanh(D1 + b1')      epilogue warps: TMEM -> regs -> tanh -> fp16 -> TMEM (the A operand of layer 2)
-//   D2 = H1 W2'^T            tcgen05.mma, TS: A = H1 (TMEM), B = W2' tiles (shared-memory ring)
-//   H2 = tanh(D2 + b2')      epilogue warps, registers only
-//   a  = H2 W3'^T + b3'      A <= 8 outputs: exact fp32 FFMA2 in the same epilogue pass (no third MMA)
+//   D1 = X  W1'^T            wgmma m64n64k16, A = X (fp16 registers, loaded once per pass), B = W1' (shared memory)
+//   H1 = tanh(D1 + b1')      in registers; packed to fp16 the accumulator IS the A operand of layer 2 (des_tc.cuh)
+//   D2 = H1 W2'^T            wgmma, A = H1 (registers), B = W2' in 64-feature chunks (double-buffered shared memory)
+//   H2 = tanh(D2 + b2')      epilogue, registers only
+//   a  = H2 W3'^T + b3'      A <= 8 outputs: exact fp32 FFMA in the same epilogue (no third MMA)
 //   fitness += -|| clip(a) - a* ||^2                                              (utils.py:134-137)
 //
-// W' = fp32(theta + sigma*eps) (natural_es.py:28-30) is never stored in HBM: generator warps regenerate
-// eps from the counter RNG and write fp16 operand tiles straight into the 128B-swizzled K-major layout
-// tcgen05 reads, through a ring of [64 rows x 64 k] slots; biases / W3' go to small fp32 arrays.
+// W' = fp32(theta + sigma*eps) (natural_es.py:28-30) is never stored in HBM: every thread regenerates eps from the
+// counter RNG and writes fp16 operand tiles straight into the 128B-swizzled K-major layout wgmma reads.  The chunk
+// of W2' for the next MMA is generated while the current one runs on the tensor cores (wgmma is asynchronous).
+//
+// Clusters: when the tape has an even number of 128-row tiles, two CTAs of a cluster share a member.  Each evaluates
+// its own tiles and generates HALF of every weight tile, storing it into its own and its peer's shared memory
+// (distributed shared memory); one cluster barrier per chunk publishes both halves.  The flagship shape (T = 256)
+// is then one pass per CTA.  Other shapes loop over passes; with the optional workspace the W2' chunks generated in
+// pass 0 are mirrored to global memory (L2-resident) and copied back in the later passes, without it they are
+// regenerated (same bytes either way).
 //
 // Precision modes
 //   F16    operands rounded to fp16 (11 significant bits, as TF32), fp32 accumulate, MUFU tanh.approx.
 //   F16X3  every operand split x = hi + lo (fp16 each, ~22 bits); D += A_hi B_hi + A_lo B_hi + A_hi B_lo;
-//          tanh as 1 - 2/(1 + 2^(2x log2 e)) on packed f32x2 ops.  ~fp32 accuracy at 3 MMAs per k-step.
-//
-// Warp roles (aligned to warpgroups so setmaxnreg can move registers from generators to epilogue warps):
-// warps 0-7 = epilogue (NT == 2: warp w owns TMEM lane quadrant w%4 of tile slot w/4; NT == 1: two warps per
-// quadrant, each taking every other 32-column group), warps 8-23 = weight generators, warp 24 = TMEM allocator +
-// single-thread MMA issuer (+ three relay lanes in the follower CTA of a pair).  All hand-offs are mbarriers
-// (generator -> MMA: slot_full/empty; MMA -> epilogue: acc_full/empty; epilogue -> MMA: h_ready / h_free);
-// accumulators are double buffered in TMEM in chunks of NC columns.
-//
-// Measured (ncu, profiles/README.md): a latency-bound three-stage pipeline — ~26 useful instructions per normal
-// deviate in the generators, 2 MUFU + 4.5 other instructions per hidden activation in the f16x3 epilogue, tensor
-// pipe 25 % busy; DRAM traffic < 1 MB per launch.
-#include <stdlib.h>
+//          tanh as 1 - 2/(1 + 2^(2x log2 e)).  ~fp32 accuracy at 3 MMAs per k-step.
 #include "des_common.cuh"
 #include "des_tc.cuh"
 
@@ -40,25 +34,20 @@ namespace des {
 
 using namespace tc;
 
-constexpr int kGenWarps = 16;
-constexpr int kGenThreads = kGenWarps * 32;
 constexpr int kK1 = 32;        // layer-1 K (state_dim zero-padded): 2 k-steps of 16
 constexpr int kMaxA = 8;
+constexpr int kTcThreads = 256;
 
-// PAIR = two CTAs of a cluster share one member (cta_group::2): each keeps ONE 128-row tile in its TMEM and
-// generates half of every weight tile; the accumulator chunk is then 128 features wide (64 rows of B per CTA).
-template <int H, int MODE, bool PAIR = false>
+template <int H, bool X3>
 struct TcCfg {
-    static constexpr bool X3 = (MODE == DES_FWD_F16X3);
-    static constexpr int NC = PAIR ? 128 : 64;                // accumulator chunk = MMA N (output features)
-    static constexpr int NCH = H / NC;                        // output-feature chunks per layer
+    static constexpr int NCH = H / 64;                        // 64-feature output chunks per layer
     static constexpr int KAT = H / 64;                        // 64-wide k atoms of layer 2
-    static constexpr int ACOLS = X3 ? H : H / 2;              // TMEM columns of H1 per tile slot
-    static constexpr int SLOT_COLS = ACOLS + 2 * NC;          // + two accumulator stages
-    static constexpr int SLOT_BYTES = (X3 ? 2 : 1) * 64 * 128;   // this CTA's B tile: 64 rows x 128 B (hi [+ lo])
-    static constexpr int X_TILE_BYTES = (X3 ? 2 : 1) * 128 * 128;   // one X tile: 128 rows x 128 B (hi [+ lo])
+    static constexpr int KS2 = H / 16;                        // k16 steps of layer 2
+    static constexpr int PLANES = X3 ? 2 : 1;                 // hi [, lo]
+    static constexpr int CHUNK_BYTES = PLANES * KAT * 8192;   // W2' rows [64c, 64c + 64), every k: hi atoms | lo atoms
+    static constexpr int W1_BYTES = PLANES * H * 128;         // W1' rows of 128 B (k < 32 used): hi | lo
     static constexpr int SMALL_FLOATS = 2 * H + kMaxA * H + kMaxA;   // b1, b2, W3' [8][H], b3[8]
-    static constexpr int NT_MAX = 512 / SLOT_COLS >= 2 ? 2 : 1;     // tile slots resident in TMEM at once
+    static constexpr size_t SMEM = 1024 + 2 * (size_t)CHUNK_BYTES + W1_BYTES + SMALL_FLOATS * sizeof(float) + 8 * sizeof(float);
 };
 
 struct TcArgs {
@@ -66,38 +55,14 @@ struct TcArgs {
     const float *theta, *obs, *target;
     const des_state *state;
     Layout L;
-    int T, n_tiles, n_pass, n_slots;
+    int T, n_pass;
     float sigma, clip, neg2ln2_sigma2;
     PhiloxKey key;
     uint32_t gen;
     uint64_t member_offset;
     int64_t n_local;
-    uint8_t *cache;        // optional per-CTA image of one member's weight tiles (multi-pass shapes), else NULL
+    uint8_t *cache;        // optional per-CTA image of one member's W2' chunks (multi-pass shapes), else NULL
 };
-
-// barrier block in shared memory
-struct TcBars {
-    uint64_t slot_full[32], slot_empty[32];
-    uint64_t small_full[2], small_empty[2];
-    uint64_t acc_full[2][2], acc_empty[2][2];
-    uint64_t h_ready[2], h_free[2];
-    uint32_t tmem_base;
-    float fit_part[16];
-    float act_x[128][kMaxA];     // NT == 1: action partial sums handed from the half-1 warp to the half-0 warp
-};
-
-// eps for 8 consecutive flat parameters starting at j0 (multiple of 4): two quads.
-__device__ __forceinline__ void perturbed8(float (&w)[8], const float *__restrict__ theta, int j0, float sigma,
-                                           uint32_t member, uint32_t gen, const PhiloxKey &key) {
-    const float4 t0 = __ldg(reinterpret_cast<const float4 *>(theta + j0));
-    const float4 t1 = __ldg(reinterpret_cast<const float4 *>(theta + j0 + 4));
-    const float4 z0 = noise_quad((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, key);
-    const float4 z1 = noise_quad((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, key);
-    w[0] = __fmaf_rn(sigma, z0.x, t0.x); w[1] = __fmaf_rn(sigma, z0.y, t0.y);
-    w[2] = __fmaf_rn(sigma, z0.z, t0.z); w[3] = __fmaf_rn(sigma, z0.w, t0.w);
-    w[4] = __fmaf_rn(sigma, z1.x, t1.x); w[5] = __fmaf_rn(sigma, z1.y, t1.y);
-    w[6] = __fmaf_rn(sigma, z1.z, t1.z); w[7] = __fmaf_rn(sigma, z1.w, t1.w);
-}
 
 // one perturbed parameter at arbitrary flat index j (slow path: whole quad per element)
 __device__ __forceinline__ float perturbed1(const float *__restrict__ theta, int j, float sigma, uint32_t member,
@@ -109,649 +74,303 @@ __device__ __forceinline__ float perturbed1(const float *__restrict__ theta, int
 }
 
 template <bool X3>
-__device__ __forceinline__ void store_octet(uint8_t *slot, uint8_t *mirror, int r, int c8, const float (&w)[8]) {
-    uint4 hi, lo;
+__device__ __forceinline__ void octet(const float (&w)[8], uint4 &hi, uint4 &lo) {
     if (X3) {
         split_h2(w[0], w[1], hi.x, lo.x); split_h2(w[2], w[3], hi.y, lo.y);
         split_h2(w[4], w[5], hi.z, lo.z); split_h2(w[6], w[7], hi.w, lo.w);
     } else {
-        hi.x = pack_h2(w[0], w[1]); hi.y = pack_h2(w[2], w[3]); hi.z = pack_h2(w[4], w[5]); hi.w = pack_h2(w[6], w[7]);
-    }
-    const int off = r * 128 + ((c8 ^ (r & 7)) << 4);          // SWIZZLE_128B
-    *reinterpret_cast<uint4 *>(slot + off) = hi;
-    if (X3) *reinterpret_cast<uint4 *>(slot + 8192 + off) = lo;
-    if (mirror) {       // same thread re-reads exactly these bytes in the later passes (no cross-thread ordering needed)
-        *reinterpret_cast<uint4 *>(mirror + off) = hi;
-        if (X3) *reinterpret_cast<uint4 *>(mirror + 8192 + off) = lo;
+        hi = make_uint4(pack_h2(w[0], w[1]), pack_h2(w[2], w[3]), pack_h2(w[4], w[5]), pack_h2(w[6], w[7]));
+        lo = hi;
     }
 }
-// later passes over the same member: copy this thread's chunk(s) of the cached tile image back into the ring slot
+
+// A operand of the two layer-1 k-steps for rows ra, ra + 8 of the observation tape (zero beyond state_dim)
 template <bool X3>
-__device__ __forceinline__ void load_octet(uint4 &hi, uint4 &lo, const uint8_t *mirror, int r, int c8) {
-    const int off = r * 128 + ((c8 ^ (r & 7)) << 4);
-    hi = *reinterpret_cast<const uint4 *>(mirror + off);
-    if (X3) lo = *reinterpret_cast<const uint4 *>(mirror + 8192 + off);
-}
-template <bool X3>
-__device__ __forceinline__ void put_octet(uint8_t *slot, int r, int c8, const uint4 &hi, const uint4 &lo) {
-    const int off = r * 128 + ((c8 ^ (r & 7)) << 4);
-    *reinterpret_cast<uint4 *>(slot + off) = hi;
-    if (X3) *reinterpret_cast<uint4 *>(slot + 8192 + off) = lo;
-}
-
-// one lane of a fully converged warp (see the MMA issuer)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
+__device__ __forceinline__ void load_x(uint32_t (&xh)[2][4], uint32_t (&xl)[2][4], const float *__restrict__ obs, int d0,
+                                       int ra, int lane) {
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int row = ra + (i & 1) * 8, k = ks * 16 + (i >> 1) * 8 + (lane & 3) * 2;
+            const float v0 = k < d0 ? __ldg(obs + (int64_t)row * d0 + k) : 0.f;
+            const float v1 = k + 1 < d0 ? __ldg(obs + (int64_t)row * d0 + k + 1) : 0.f;
+            if (X3) split_h2(v0, v1, xh[ks][i], xl[ks][i]);
+            else xh[ks][i] = pack_h2(v0, v1);
+        }
+    }
 }
 
-template <int REGS>
-__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS>
-__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T (layer 1: A = X tile)
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-constexpr int kThetaStageBytes = 2 * 2 * kGenWarps * 32 * 16;   // two stages x two 16-byte halves per generator thread
-
-// Physical warp ids are assigned by priority (the SM's warp arbiter prefers the highest id among eligible warps, and the
-// epilogue chain is the critical path): physical warps 0-15 = generators, 16 = MMA issuer, 17-19 idle, 20-27 = epilogue.
-// The code below keeps the LOGICAL numbering of the comment at the top (epilogue 0-7, generators 8-23, MMA 24).
-constexpr int kTcThreads = (kGenWarps + 4 + 8) * 32;
-__device__ __forceinline__ int logical_warp(int p) { return p < kGenWarps ? 8 + p : (p < kGenWarps + 4 ? 24 + (p - kGenWarps) : p - (kGenWarps + 4)); }
-
-template <int H, int MODE, int NT, bool PAIR>
+// NA: compile-time bound on the action count (4 or 8) that sizes the per-thread action sums
+template <int H, bool X3, int CL, int NA>
 __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
-    static_assert(!PAIR || NT == 1, "a CTA pair keeps one tile per CTA");
-    using C = TcCfg<H, MODE, PAIR>;
-    constexpr bool X3 = C::X3;
-    constexpr int kNC = C::NC;
-    const uint32_t rank = PAIR ? cluster_ctarank() : 0u;          // 0 = leader (issues the MMAs)
-    constexpr int kEpiWarps = 8;              // NT == 2: four per tile slot; NT == 1: two per TMEM lane quadrant,
-                                              // each taking one 32-column half of every accumulator chunk
-    constexpr int kWarpsPerSlot = kEpiWarps / NT;
-    // Pairs with two H1 chunks signal each chunk's readiness separately (h_ready[chunk]; index 1 is otherwise the
-    // second tile slot's barrier, unused when NT == 1): the layer-2 MMAs over the first chunk's k-atoms then run
-    // while the epilogue warps are still producing the second chunk.
-    constexpr bool kChunkedH = PAIR && C::NCH == 2;
-    constexpr int kAtomsPerChunk = kNC / 64;
-    constexpr int kMmaWarp = kEpiWarps + kGenWarps;
+    using C = TcCfg<H, X3>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *xs = smem;                                                          // n_tiles * X_TILE_BYTES
-    uint8_t *ring = xs + (size_t)a.n_tiles * C::X_TILE_BYTES;                    // n_slots * SLOT_BYTES
-    float *small = reinterpret_cast<float *>(ring + (size_t)a.n_slots * C::SLOT_BYTES);   // [2][SMALL_FLOATS]
-    TcBars *bars = reinterpret_cast<TcBars *>(small + 2 * C::SMALL_FLOATS);
-    // theta of the NEXT layer-2 slot, staged per generator thread by cp.async: [stage][half][thread] x 16 bytes
-    float4 *th_stage = reinterpret_cast<float4 *>((reinterpret_cast<uintptr_t>(bars + 1) + 15) & ~(uintptr_t)15);
+    uint8_t *w2buf = smem;                                                  // [2][CHUNK_BYTES]
+    uint8_t *w1 = smem + 2 * C::CHUNK_BYTES;                                // [W1_BYTES]
+    float *small = reinterpret_cast<float *>(w1 + C::W1_BYTES);             // [SMALL_FLOATS]
+    float *fit_part = small + C::SMALL_FLOATS;                              // [8]
+    const float *b1 = small, *b2 = small + H, *w3 = small + 2 * H, *b3 = small + 2 * H + kMaxA * H;
 
-    const int warp = logical_warp(threadIdx.x >> 5), lane = threadIdx.x & 31;     // (warp & 3) is the same for both numberings
-    const int n_epi_warps = kEpiWarps;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
     const Layout L = a.L;
     const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
+    const int64_t first = blockIdx.x / CL, stride = gridDim.x / CL;
+    uint8_t *const cache = (a.cache && a.n_pass > 1) ? a.cache + (size_t)blockIdx.x * C::NCH * C::CHUNK_BYTES : nullptr;
 
-    // Pairs: barriers signalled by tcgen05.commit are multicast to both CTAs.  Barriers the leader's MMA thread waits
-    // on (slot_full, acc_empty, h_ready) need the arrivals of BOTH CTAs: every warp arrives on its OWN CTA's barrier,
-    // and three forwarder lanes of the follower's (otherwise idle) MMA warp relay each completed phase to the leader
-    // with ONE cluster-scope arrive.  (Arriving remotely from every warp put a MEMBAR.GPU + ERRBAR — the lowering of
-    // mbarrier.arrive.release.cluster — into each generator/epilogue warp per slot: 10% of all stall samples.)
-    auto arrive_leader = [&](uint64_t *bar) { mbar_arrive(smem_u32(bar)); };
-    auto commit = [&](uint64_t *bar) {
-        if (PAIR) mma2_commit(smem_u32(bar));
-        else mma_commit(smem_u32(bar));
+    auto sync_all = [&]() {
+        if (CL == 2) cluster_sync_all();
+        else __syncthreads();
     };
-    if (warp == kMmaWarp) {
-        if (lane == 0) {
-            for (int s = 0; s < a.n_slots; ++s) {
-                mbar_init(smem_u32(&bars->slot_full[s]), kGenWarps + ((PAIR && rank == 0) ? 1 : 0));
-                mbar_init(smem_u32(&bars->slot_empty[s]), 1);
-            }
-            for (int p = 0; p < 2; ++p) {
-                mbar_init(smem_u32(&bars->small_full[p]), kGenWarps);
-                mbar_init(smem_u32(&bars->small_empty[p]), n_epi_warps);
-                mbar_init(smem_u32(&bars->h_ready[p]), kWarpsPerSlot + ((PAIR && rank == 0) ? 1 : 0));
-                mbar_init(smem_u32(&bars->h_free[p]), 1);
-                for (int st = 0; st < 2; ++st) {
-                    mbar_init(smem_u32(&bars->acc_full[p][st]), 1);
-                    mbar_init(smem_u32(&bars->acc_empty[p][st]), kWarpsPerSlot + ((PAIR && rank == 0) ? 1 : 0));
+    // a 16-byte chunk of an operand tile (hi plane at `off`, lo plane `lo_off` further) into this CTA and its peer
+    auto put = [&](uint8_t *base, uint32_t off, uint32_t lo_off, const uint4 &hi, const uint4 &lo) {
+        *reinterpret_cast<uint4 *>(base + off) = hi;
+        if (X3) *reinterpret_cast<uint4 *>(base + lo_off + off) = lo;
+        if (CL == 2) {
+            st_cluster_v4(map_cluster(smem_u32(base + off), rank ^ 1u), hi);
+            if (X3) st_cluster_v4(map_cluster(smem_u32(base + lo_off + off), rank ^ 1u), lo);
+        }
+    };
+    // this CTA's share of W2' chunk c (rows [64c, 64c + 64)) into buffer `buf`; pass > 0 copies the cached image back
+    constexpr int kOct = H / 8;                                   // octets per row
+    constexpr int kRows = 64 / CL;                                // rows of a chunk generated here
+    auto gen_chunk = [&](uint32_t member, int c, int pass, int buf) {
+        uint8_t *dst = w2buf + buf * C::CHUNK_BYTES;
+        uint8_t *mirror = cache ? cache + (size_t)c * C::CHUNK_BYTES : nullptr;
+        for (int idx = tid; idx < kRows * kOct; idx += kTcThreads) {
+            const int rr = (int)rank * kRows + idx / kOct, o = idx % kOct;
+            const uint32_t off = (uint32_t)((o >> 3) * 8192 + rr * 128 + (((o & 7) ^ (rr & 7)) << 4));
+            uint4 hi, lo;
+            if (mirror && pass > 0) {
+                hi = *reinterpret_cast<const uint4 *>(mirror + off);
+                if (X3) lo = *reinterpret_cast<const uint4 *>(mirror + C::KAT * 8192 + off);
+                else lo = hi;
+            } else {
+                const int j0 = L.off_w2 + (c * 64 + rr) * H + o * 8;
+                const float4 p0 = perturbed_quad((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                                 __ldg(reinterpret_cast<const float4 *>(a.theta + j0)));
+                const float4 p1 = perturbed_quad((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                                 __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4)));
+                const float w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+                octet<X3>(w, hi, lo);
+                if (mirror) {       // the same thread reads exactly these bytes back in the later passes
+                    *reinterpret_cast<uint4 *>(mirror + off) = hi;
+                    if (X3) *reinterpret_cast<uint4 *>(mirror + C::KAT * 8192 + off) = lo;
                 }
             }
-            fence_barrier_init();
+            put(dst, off, C::KAT * 8192, hi, lo);
         }
-        __syncwarp();
-        if (PAIR) tmem_alloc2(smem_u32(&bars->tmem_base), 512);
-        else tmem_alloc(smem_u32(&bars->tmem_base), 512);
-    }
-    // X -> shared memory once: fp16 (hi [, lo]) K-major SWIZZLE_128B tiles of 128 observations, k < d0 (<= 32)
-    for (int idx = threadIdx.x; idx < a.n_tiles * 128 * 4; idx += blockDim.x) {
-        const int c8 = idx & 3, r = (idx >> 2) & 127, tt = idx >> 9;
-        const int gt = PAIR ? tt * 2 + (int)rank : tt;             // global tile of this CTA's local tile tt
-        const float *orow = a.obs + (int64_t)(gt * 128 + r) * L.d0;
-        float w[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) w[e] = (c8 * 8 + e < L.d0) ? __ldg(orow + c8 * 8 + e) : 0.f;
-        uint4 hi, lo;
-        if (X3) {
-            split_h2(w[0], w[1], hi.x, lo.x); split_h2(w[2], w[3], hi.y, lo.y);
-            split_h2(w[4], w[5], hi.z, lo.z); split_h2(w[6], w[7], hi.w, lo.w);
-        } else {
-            hi.x = pack_h2(w[0], w[1]); hi.y = pack_h2(w[2], w[3]); hi.z = pack_h2(w[4], w[5]); hi.w = pack_h2(w[6], w[7]);
-        }
-        const int off = r * 128 + ((c8 ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4 *>(xs + (size_t)tt * C::X_TILE_BYTES + off) = hi;
-        if (X3) *reinterpret_cast<uint4 *>(xs + (size_t)tt * C::X_TILE_BYTES + 16384 + off) = lo;
-    }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    if (PAIR) cluster_sync_all();          // the peer's barriers are initialised before anyone arrives on them
-    tc_fence_after();
-    const uint32_t tmem = bars->tmem_base;
-    // TMEM map: tile slot ts at ts*SLOT_COLS: H1 [0,ACOLS), accumulator stages at ACOLS + st*64
-    auto slot_base = [&](int ts) { return tmem + (uint32_t)(ts * C::SLOT_COLS); };
+    };
 
-    const int64_t first = PAIR ? blockIdx.x / 2 : blockIdx.x;
-    const int64_t stride = PAIR ? gridDim.x / 2 : gridDim.x;
+    // warpgroup wg owns rows [64 wg, 64 wg + 64) of the pass's tile; this thread rows ra and ra + 8 of them
+    const int wg = warp >> 2;
+    const int r_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = (lane & 3) * 2;                                // column pair inside every 8-column block
 
-    if (warp == kMmaWarp) {
-        // =================================== MMA issuer ===================================
-        // The whole warp runs the loop converged and one elected lane issues, so every tcgen05 operand is warp-uniform
-        // (inside `if (lane == 0)` ptxas wrapped each tcgen05.mma in an ELECT / R2UR.BROADCAST / BRA.U.ANY loop: ~160
-        // cycles per MMA, which made the issuing thread the bottleneck — round-2 trace of the pair kernel).
-        if (rank == 0) {
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem, 0);
-            auto slot_base_u = [&](int ts) { return tmem_u + (uint32_t)(ts * C::SLOT_COLS); };
-            constexpr uint32_t idesc = idesc_f16(PAIR ? 256 : 128, kNC);
-            uint32_t rs = 0, rph = 0;            // ring cursor: slot index and phase
-            uint32_t acc_u[2] = {0, 0};          // accumulator-stage use counters per tile slot
-            uint32_t hv[2] = {0, 0};             // (member, pass) counter per tile slot for h_ready
-            for (int64_t m = first; m < a.n_local; m += stride) {
-                for (int pass = 0; pass < a.n_pass; ++pass) {
-                    // ---- layer 1: D1 chunk nc = X W1'[64nc:64nc+64, :]^T
-                    for (int nc = 0; nc < C::NCH; ++nc) {
-                        const uint32_t s = rs, sph = rph;
-                        if (++rs == (uint32_t)a.n_slots) { rs = 0; rph ^= 1; }
-                        mbar_wait(smem_u32(&bars->slot_full[s]), sph);
-                        tc_fence_after();
-                        const uint32_t bbase = smem_u32(ring + (size_t)s * C::SLOT_BYTES);
-                        for (int ts = 0; ts < NT; ++ts) {
-                            const uint32_t u = acc_u[ts]++, st = u & 1, ph = (u >> 1) & 1;
-                            mbar_wait(smem_u32(&bars->acc_empty[ts][st]), ph ^ 1);
-                            tc_fence_after();
-                            const uint32_t d = slot_base_u(ts) + C::ACOLS + st * kNC;
-                            const uint32_t xaddr = smem_u32(xs + (size_t)(pass * NT + ts) * C::X_TILE_BYTES);
-                            if (elect_one()) {
+    // distributed shared memory may only be accessed once every CTA of the cluster is running
+    if (CL == 2) cluster_sync_all();
+    for (int64_t m = first; m < a.n_local; m += stride) {
+        const uint32_t member = (uint32_t)(a.member_offset + (uint64_t)m);
+        // ---- small fp32 arrays (whole, in every CTA): b1 | b2 | W3[8][H] | b3[8]
+        for (int i = tid; i < H / 4; i += kTcThreads) {
+            const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + i), member, gen, kStreamNesEps, a.key,
+                                             a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + i));
+            const float4 v2 = perturbed_quad((uint32_t)((L.off_b2 >> 2) + i), member, gen, kStreamNesEps, a.key,
+                                             a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + i));
+            // the f16x3 epilogue evaluates tanh(v + b) as 1 - 2/(1 + 2^(v*c + b*c)), c = 2 log2 e: store b*c
+            const float bsc = X3 ? kTwoLog2e : 1.0f;
+            reinterpret_cast<float4 *>(small)[i] = make_float4(v1.x * bsc, v1.y * bsc, v1.z * bsc, v1.w * bsc);
+            reinterpret_cast<float4 *>(small + H)[i] = make_float4(v2.x * bsc, v2.y * bsc, v2.z * bsc, v2.w * bsc);
+        }
+        for (int i = tid; i < L.A * H / 4; i += kTcThreads)                // W3' [q][n] row-major: aligned quads
+            reinterpret_cast<float4 *>(small + 2 * H)[i] =
+                perturbed_quad((uint32_t)((L.off_w3 >> 2) + i), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                               __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + i));
+        for (int i = L.A * H + tid; i < H * kMaxA; i += kTcThreads) small[2 * H + i] = 0.f;   // unused action rows
+        if (tid < kMaxA) small[2 * H + kMaxA * H + tid] = tid < L.A ? perturbed1(a.theta, L.off_b3 + tid, a.sigma, member, gen, a.key) : 0.f;
+        // ---- W1' (this CTA's half of the rows in a cluster): rows of 128 B, k < d0, zero padded to 32
+        for (int idx = tid; idx < (H / CL) * 4; idx += kTcThreads) {
+            const int n = (int)rank * (H / CL) + (idx >> 2), c8 = idx & 3;
+            float w[8];
+            if ((L.d0 & 3) == 0) {                                        // row starts are quad aligned
 #pragma unroll
-                            for (int ks = 0; ks < kK1 / 16; ++ks) {
-                                const uint64_t ah = smem_desc_sw128(xaddr) + (uint64_t)(ks * 2);
-                                const uint64_t bh = smem_desc_sw128(bbase) + (uint64_t)(ks * 2);
-                                if (PAIR) mma2_f16_ss(d, ah, bh, idesc, ks > 0); else mma_f16_ss(d, ah, bh, idesc, ks > 0);
-                                if (X3) {
-                                    const uint64_t al = smem_desc_sw128(xaddr + 16384) + (uint64_t)(ks * 2);
-                                    const uint64_t bl = smem_desc_sw128(bbase + 8192) + (uint64_t)(ks * 2);
-                                    if (PAIR) { mma2_f16_ss(d, al, bh, idesc, 1); mma2_f16_ss(d, ah, bl, idesc, 1); }
-                                    else { mma_f16_ss(d, al, bh, idesc, 1); mma_f16_ss(d, ah, bl, idesc, 1); }   // X_lo W_hi, X_hi W_lo
-                                }
-                            }
-                            commit(&bars->acc_full[ts][st]);
-                            }
-                            __syncwarp();
-                        }
-                        if (elect_one()) commit(&bars->slot_empty[s]);
-                        __syncwarp();
+                for (int hq = 0; hq < 2; ++hq) {
+                    const int k = c8 * 8 + hq * 4;
+                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (k < L.d0) {
+                        const int j = L.off_w1 + n * L.d0 + k;
+                        v = perturbed_quad((uint32_t)(j >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                           __ldg(reinterpret_cast<const float4 *>(a.theta + j)));
                     }
-                    // ---- layer 2: D2 chunk nc = H1 W2'[64nc:64nc+64, :]^T, k in atoms of 64
-                    for (int nc = 0; nc < C::NCH; ++nc) {
-                        uint32_t st_[2], d_[2];
-                        for (int ts = 0; ts < NT; ++ts) {
-                            const uint32_t u = acc_u[ts]++, st = u & 1, ph = (u >> 1) & 1;
-                            mbar_wait(smem_u32(&bars->acc_empty[ts][st]), ph ^ 1);
-                            st_[ts] = st;
-                            d_[ts] = slot_base_u(ts) + C::ACOLS + st * kNC;
-                            if (nc == 0 && !kChunkedH) mbar_wait(smem_u32(&bars->h_ready[ts]), hv[ts] & 1);
-                        }
-                        tc_fence_after();
-                        for (int ka = 0; ka < C::KAT; ++ka) {
-                            const uint32_t s = rs, sph = rph;
-                            if (++rs == (uint32_t)a.n_slots) { rs = 0; rph ^= 1; }
-                            if (kChunkedH && nc == 0 && ka % kAtomsPerChunk == 0)
-                                mbar_wait(smem_u32(&bars->h_ready[ka / kAtomsPerChunk]), hv[0] & 1);
-                            mbar_wait(smem_u32(&bars->slot_full[s]), sph);
-                            tc_fence_after();
-                            const uint32_t bbase = smem_u32(ring + (size_t)s * C::SLOT_BYTES);
-                            if (elect_one()) {
-                            for (int ts = 0; ts < NT; ++ts) {
-                                const uint32_t ah = slot_base_u(ts) + ka * 32;
+                    w[4 * hq] = v.x; w[4 * hq + 1] = v.y; w[4 * hq + 2] = v.z; w[4 * hq + 3] = v.w;
+                }
+            } else {
 #pragma unroll
-                                for (int ks = 0; ks < 4; ++ks) {
-                                    const uint64_t bh = smem_desc_sw128(bbase) + (uint64_t)(ks * 2);
-                                    if (PAIR) mma2_f16_ts(d_[ts], ah + ks * 8, bh, idesc, (ka | ks) != 0);
-                                    else mma_f16_ts(d_[ts], ah + ks * 8, bh, idesc, (ka | ks) != 0);
-                                    if (X3) {
-                                        const uint64_t bl = smem_desc_sw128(bbase + 8192) + (uint64_t)(ks * 2);
-                                        if (PAIR) { mma2_f16_ts(d_[ts], ah + H / 2 + ks * 8, bh, idesc, 1); mma2_f16_ts(d_[ts], ah + ks * 8, bl, idesc, 1); }
-                                        else { mma_f16_ts(d_[ts], ah + H / 2 + ks * 8, bh, idesc, 1); mma_f16_ts(d_[ts], ah + ks * 8, bl, idesc, 1); }   // H1_lo W_hi, H1_hi W_lo
-                                    }
-                                }
-                            }
-                            commit(&bars->slot_empty[s]);
-                            }
-                            __syncwarp();
+                for (int e = 0; e < 8; ++e) {
+                    const int k = c8 * 8 + e;
+                    w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, a.sigma, member, gen, a.key) : 0.f;
+                }
+            }
+            uint4 hi, lo;
+            octet<X3>(w, hi, lo);
+            put(w1, (uint32_t)(n * 128 + ((c8 ^ (n & 7)) << 4)), H * 128, hi, lo);
+        }
+        gen_chunk(member, 0, 0, 0);
+        fence_proxy_async_cluster();
+        sync_all();
+
+        float sq = 0.f;
+        for (int pass = 0; pass < a.n_pass; ++pass) {
+            const int tile = pass * CL + (int)rank;
+            const int ra = tile * 128 + r_in_tile;
+            // ---------------- layer 1: H1 = tanh(X W1'^T + b1), kept as the fp16 A operand of layer 2
+            uint32_t h1h[C::KS2][4], h1l[X3 ? C::KS2 : 1][4];
+            {
+                uint32_t xh[2][4], xl[2][4];
+                load_x<X3>(xh, xl, a.obs, L.d0, ra, lane);
+#pragma unroll
+                for (int c = 0; c < C::NCH; ++c) {
+                    float d[32];
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 2; ++ks) {
+                        const uint32_t bh = smem_u32(w1) + c * 8192 + ks * 32;
+                        wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh), ks > 0);
+                        if (X3) {
+                            wgmma_rs_n64(d, xl[ks], smem_desc_sw128(bh), 1);                   // X_lo W_hi
+                            wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh + H * 128), 1);         // X_hi W_lo
                         }
-                        const bool issuer = elect_one();
-                        for (int ts = 0; ts < NT; ++ts) {
-                            if (issuer) commit(&bars->acc_full[ts][st_[ts]]);
-                            if (nc == C::NCH - 1) {
-                                if (issuer) commit(&bars->h_free[ts]);
-                                ++hv[ts];
-                            }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float2 b = *reinterpret_cast<const float2 *>(b1 + c * 64 + j * 8 + cq);
+                        const int s = c * 4 + (j >> 1), e = (j & 1) * 2;
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const float v0 = d[4 * j + 2 * r], v1 = d[4 * j + 2 * r + 1];
+                            if (X3) split_h2(tanh_acc_b(v0, b.x), tanh_acc_b(v1, b.y), h1h[s][e + r], h1l[s][e + r]);
+                            else h1h[s][e + r] = pack_h2(tanh_fast(v0 + b.x), tanh_fast(v1 + b.y));
                         }
-                        __syncwarp();
                     }
                 }
             }
-        }
-        if (PAIR && rank == 1 && lane < 3) {
-            // ---- follower CTA: relay completed local phases to the leader's barriers, in the leader's wait order
-            const int64_t rounds = (a.n_local - first + stride - 1) / stride * a.n_pass;     // (member, pass) pairs
-            if (lane == 0) {                      // slot_full: one relay per ring slot
-                uint32_t rs = 0, rph = 0;
-                for (int64_t i = 0; i < rounds * (C::NCH + C::NCH * C::KAT); ++i) {
-                    mbar_wait(smem_u32(&bars->slot_full[rs]), rph);
-                    mbar_arrive_cluster(smem_u32(&bars->slot_full[rs]), 0);
-                    if (++rs == (uint32_t)a.n_slots) { rs = 0; rph ^= 1; }
-                }
-            } else if (lane == 1) {               // acc_empty: one relay per accumulator-stage use
-                for (int64_t u = 0; u < rounds * 2 * C::NCH; ++u) {
-                    const uint32_t st = (uint32_t)u & 1, ph = (uint32_t)(u >> 1) & 1;
-                    mbar_wait(smem_u32(&bars->acc_empty[0][st]), ph);
-                    mbar_arrive_cluster(smem_u32(&bars->acc_empty[0][st]), 0);
-                }
-            } else {                              // h_ready: one relay per (member, pass)
-                for (int64_t v = 0; v < rounds; ++v) {
-                    mbar_wait(smem_u32(&bars->h_ready[0]), (uint32_t)v & 1);
-                    mbar_arrive_cluster(smem_u32(&bars->h_ready[0]), 0);
-                    if (kChunkedH) {
-                        mbar_wait(smem_u32(&bars->h_ready[1]), (uint32_t)v & 1);
-                        mbar_arrive_cluster(smem_u32(&bars->h_ready[1]), 0);
+            // ---------------- layer 2 + 3: per 64-feature chunk, H2 = tanh(H1 W2'^T + b2); a += H2 W3'^T
+            float act[NA][2];
+#pragma unroll
+            for (int q = 0; q < NA; ++q) act[q][0] = act[q][1] = 0.f;
+            for (int c = 0; c < C::NCH; ++c) {
+                const int qi = pass * C::NCH + c;
+                const uint32_t bbase = smem_u32(w2buf + (qi & 1) * C::CHUNK_BYTES);
+                float d[32];
+#pragma unroll
+                for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                wgmma_fence();
+#pragma unroll
+                for (int s = 0; s < C::KS2; ++s) {
+                    const uint32_t bh = bbase + (s >> 2) * 8192 + (s & 3) * 32;
+                    wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh), s > 0);
+                    if (X3) {
+                        wgmma_rs_n64(d, h1l[s], smem_desc_sw128(bh), 1);                          // H1_lo W_hi
+                        wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh + C::KAT * 8192), 1);          // H1_hi W_lo
                     }
                 }
-            }
-        }
-    } else if (warp < kEpiWarps) {
-        // =================================== epilogue warps ============================================
-        reg_alloc<96>();
-        const int ts = (NT == 2) ? (warp >> 2) : 0;                   // tile slot
-        const int my_half = warp >> 2;                                // NT == 1: this warp owns the 32-column groups g with (g & 1) == my_half
-        constexpr int kGroups = kNC / 32;                             // 32-column groups per accumulator chunk
-        // this warp's share of an accumulator chunk as 16-column steps: group g = (NT == 2 ? s/2 : 2*(s/2) + my_half)
-        constexpr int kSteps = 2 * ((NT == 2) ? kGroups : kGroups / 2);
-        auto step_col = [&](int s) { return ((NT == 2) ? (s >> 1) : 2 * (s >> 1) + my_half) * 32 + (s & 1) * 16; };
-        const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;  // TMEM lane quadrant of this warp
-        const int row = (warp & 3) * 32 + lane;                       // observation row inside the tile
-        uint32_t acc_u = 0, hv = 0, mi = 0;
-        const uint32_t sbase = slot_base(ts) + lane_off;
-        for (int64_t m = first; m < a.n_local; m += stride, ++mi) {
-            const uint32_t p = mi & 1;
-            const float *sm = small + p * C::SMALL_FLOATS;
-            const float *b1 = sm, *b2 = sm + H, *w3 = sm + 2 * H, *b3 = sm + 2 * H + kMaxA * H;
-            mbar_wait(smem_u32(&bars->small_full[p]), (mi >> 1) & 1);
-            float sq = 0.f;
-            for (int pass = 0; pass < a.n_pass; ++pass) {
-                // ---------------- epilogue 1: H1 = tanh(D1 + b1) -> fp16 -> TMEM A buffer
-                for (int nc = 0; nc < C::NCH; ++nc) {
-                    const uint32_t u = acc_u++, st = u & 1, ph = (u >> 1) & 1;
-                    mbar_wait(smem_u32(&bars->acc_full[ts][st]), ph);
-                    tc_fence_after();
-                    // 16-column steps, software pipelined: the tcgen05.ld of step s+1 is in flight while step s is
-                    // computed (the TMEM read latency was 14 % of the epilogue warps' busy time)
-                    const uint32_t acc_base = sbase + C::ACOLS + st * kNC;
-                    uint32_t vbuf[2][16];
-                    tmem_ld16(acc_base + step_col(0), vbuf[0]);
+                wgmma_commit();
+                // the next chunk (of this pass or the next) is generated while the tensor cores run this one
+                if (c + 1 < C::NCH) gen_chunk(member, c + 1, pass, (qi + 1) & 1);
+                else if (pass + 1 < a.n_pass) gen_chunk(member, 0, pass + 1, (qi + 1) & 1);
+                wgmma_wait<0>();
+                fence_regs(d);
 #pragma unroll
-                    for (int s = 0; s < kSteps; ++s) {
-                        uint32_t (&v)[16] = vbuf[s & 1];
-                        tmem_wait_ld16(v);
-                        if (s + 1 < kSteps) {
-                            tmem_ld16(acc_base + step_col(s + 1), vbuf[(s + 1) & 1]);
-                        } else {                                   // every load of this accumulator stage has landed
-                            tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0) arrive_leader(&bars->acc_empty[ts][st]);
-                        }
-                        if (nc == 0 && s == 0) {
-                            // the previous (member, pass) must have finished reading H1 before we overwrite it
-                            mbar_wait(smem_u32(&bars->h_free[ts]), (hv & 1) ^ 1);
-                            tc_fence_after();
-                        }
-                        const int col = step_col(s);
-                        const float4 *bq = reinterpret_cast<const float4 *>(b1 + nc * kNC + col);
-                        uint32_t hi[8], lo[8];
+                for (int j = 0; j < 8; ++j) {
+                    const int n = c * 64 + j * 8 + cq;
+                    const float2 b = *reinterpret_cast<const float2 *>(b2 + n);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float4 b = bq[i];
-                            const float2 v01 = make_float2(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]));
-                            const float2 v23 = make_float2(__uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-                            if (X3) {       // b1 holds b * 2log2(e) in this mode (see the generator)
-                                split_h2p(tanh_acc2(v01, make_float2(b.x, b.y)), hi[2 * i], lo[2 * i]);
-                                split_h2p(tanh_acc2(v23, make_float2(b.z, b.w)), hi[2 * i + 1], lo[2 * i + 1]);
-                            } else {
-                                // (tanh.approx.f16x2 was tried here: SASS issues one MUFU.TANH.F16 per half plus a PRMT,
-                                //  so it saves nothing over fp32 MUFU.TANH and costs precision)
-                                const float2 x01 = fadd2(v01, make_float2(b.x, b.y)), x23 = fadd2(v23, make_float2(b.z, b.w));
-                                hi[2 * i] = pack_h2(tanh_fast(x01.x), tanh_fast(x01.y));
-                                hi[2 * i + 1] = pack_h2(tanh_fast(x23.x), tanh_fast(x23.y));
-                            }
-                        }
-                        tmem_st8(sbase + nc * (kNC / 2) + col / 2, hi);
-                        if (X3) tmem_st8(sbase + H / 2 + nc * (kNC / 2) + col / 2, lo);
-                    }
-                    if (kChunkedH) {              // this chunk of H1 is complete: its k-atoms may be consumed
-                        tmem_wait_st();
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) arrive_leader(&bars->h_ready[nc]);
-                    }
-                }
-                if (!kChunkedH) {
-                    tmem_wait_st();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) arrive_leader(&bars->h_ready[ts]);
-                }
-                ++hv;
-                // ---------------- epilogue 2+3: H2 = tanh(D2 + b2); a = H2 W3^T + b3 in fp32 registers
-                float2 actp[kMaxA];                          // (even-n, odd-n) partial sums of action q
-#pragma unroll
-                for (int q = 0; q < kMaxA; ++q) actp[q] = make_float2(0.f, 0.f);
-                for (int nc = 0; nc < C::NCH; ++nc) {
-                    const uint32_t u = acc_u++, st = u & 1, ph = (u >> 1) & 1;
-                    mbar_wait(smem_u32(&bars->acc_full[ts][st]), ph);
-                    tc_fence_after();
-                    const uint32_t acc_base = sbase + C::ACOLS + st * kNC;
-                    uint32_t vbuf[2][16];
-                    tmem_ld16(acc_base + step_col(0), vbuf[0]);
-#pragma unroll
-                    for (int s = 0; s < kSteps; ++s) {
-                        uint32_t (&v)[16] = vbuf[s & 1];
-                        tmem_wait_ld16(v);
-                        if (s + 1 < kSteps) {
-                            tmem_ld16(acc_base + step_col(s + 1), vbuf[(s + 1) & 1]);
+                    for (int r = 0; r < 2; ++r) {
+                        float h0, h1;
+                        if (X3) {          // b2 holds b * 2log2(e)
+                            h0 = tanh_acc_b(d[4 * j + 2 * r], b.x);
+                            h1 = tanh_acc_b(d[4 * j + 2 * r + 1], b.y);
                         } else {
-                            tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0) arrive_leader(&bars->acc_empty[ts][st]);
+                            h0 = tanh_fast(d[4 * j + 2 * r] + b.x);
+                            h1 = tanh_fast(d[4 * j + 2 * r + 1] + b.y);
                         }
-                        const int n0 = nc * kNC + step_col(s);
-                        const float4 *bq = reinterpret_cast<const float4 *>(b2 + n0);
+                        // layer 3 (model.py:38) in fp32: W3' row-major [q][n]
 #pragma unroll
-                        for (int i4 = 0; i4 < 4; ++i4) {
-                            const float4 b = bq[i4];
-                            const float2 v01 = make_float2(__uint_as_float(v[4 * i4]), __uint_as_float(v[4 * i4 + 1]));
-                            const float2 v23 = make_float2(__uint_as_float(v[4 * i4 + 2]), __uint_as_float(v[4 * i4 + 3]));
-                            float2 h01, h23;
-                            if (X3) {           // b2 holds b * 2log2(e)
-                                h01 = tanh_acc2(v01, make_float2(b.x, b.y));
-                                h23 = tanh_acc2(v23, make_float2(b.z, b.w));
-                            } else {
-                                const float2 x01 = fadd2(v01, make_float2(b.x, b.y)), x23 = fadd2(v23, make_float2(b.z, b.w));
-                                h01 = make_float2(tanh_fast(x01.x), tanh_fast(x01.y));
-                                h23 = make_float2(tanh_fast(x23.x), tanh_fast(x23.y));
-                            }
-                            // layer 3 (model.py:38) in fp32 on packed FFMA2: W3' row-major [q][n], 4 consecutive n per LDS.128
-#pragma unroll
-                            for (int q = 0; q < kMaxA; ++q) {
-                                if (q < 4 || L.A > 4) {
-                                    const float4 w = *reinterpret_cast<const float4 *>(w3 + q * H + n0 + 4 * i4);
-                                    actp[q] = ffma2(h01, make_float2(w.x, w.y), actp[q]);
-                                    actp[q] = ffma2(h23, make_float2(w.z, w.w), actp[q]);
-                                }
+                        for (int q = 0; q < NA; ++q) {
+                            if (q < L.A) {
+                                const float2 w = *reinterpret_cast<const float2 *>(w3 + q * H + n);
+                                act[q][r] = __fmaf_rn(h1, w.y, __fmaf_rn(h0, w.x, act[q][r]));
                             }
                         }
                     }
                 }
-                float act[kMaxA];
+                fence_proxy_async_cluster();
+                sync_all();          // the next chunk is in both CTAs; every MMA that read this buffer has completed
+            }
+            // ---- the four lanes of a quad hold the action sums over disjoint columns of the same two rows
 #pragma unroll
-                for (int q = 0; q < kMaxA; ++q) act[q] = actp[q].x + actp[q].y;
-                if (NT == 1) {
-                    // the two warps of a lane quadrant each hold the action sums over their half of the features:
-                    // combine (fixed order: half 0 + half 1) before the nonlinear clip
-                    if (my_half == 1) {
+            for (int q = 0; q < NA; ++q) {
 #pragma unroll
-                        for (int q = 0; q < kMaxA; ++q) bars->act_x[row][q] = act[q];
-                    }
-                    asm volatile("bar.sync 2, 256;" ::: "memory");
-                    if (my_half == 0) {
-#pragma unroll
-                        for (int q = 0; q < kMaxA; ++q) act[q] += bars->act_x[row][q];
-                    }
-                    asm volatile("bar.sync 2, 256;" ::: "memory");
-                }
-                const int t = (PAIR ? pass * 2 + (int)rank : pass * NT + ts) * 128 + row;
-#pragma unroll
-                for (int q = 0; q < kMaxA; ++q) {
-                    if (q < L.A && (NT == 2 || my_half == 0)) {
-                        float v = act[q] + b3[q];
-                        v = fminf(fmaxf(v, -a.clip), a.clip);
-                        const float d = v - __ldg(a.target + (int64_t)t * L.A + q);
-                        sq = __fmaf_rn(d, d, sq);
-                    }
+                for (int r = 0; r < 2; ++r) {
+                    act[q][r] += __shfl_xor_sync(0xffffffffu, act[q][r], 1);
+                    act[q][r] += __shfl_xor_sync(0xffffffffu, act[q][r], 2);
                 }
             }
-            // ---- member done: reduce squared error over all rows / tile slots (fixed order -> deterministic)
+            if ((lane & 3) == 0) {
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-            if (lane == 0) bars->fit_part[warp] = sq;
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bars->small_empty[p]));     // done with this member's b/W3
-            asm volatile("bar.sync 1, %0;" ::"r"(n_epi_warps * 32) : "memory");
-            if (warp == 0 && lane == 0) {
-                double f = 0.0;
-                for (int w = 0; w < n_epi_warps; ++w) f += (double)bars->fit_part[w];
-                // a pair adds its two halves into the (pre-zeroed) output: two commutative fp32 adds -> deterministic
-                if (PAIR) atomicAdd(a.fitness + m, (float)(-f));
-                else a.fitness[m] = (float)(-f);
-            }
-            asm volatile("bar.sync 1, %0;" ::"r"(n_epi_warps * 32) : "memory");
-        }
-    } else if (warp < kMmaWarp) {
-        // =================================== weight generators =========================================
-        reg_dealloc<56>();
-        // producer-side waits: tight polling in f16x3 mode, polling with back-off in f16 mode (measured: the back-off
-        // gains 1.6 % in f16 mode, where the generators are the bottleneck and share issue slots with their own
-        // waiters, and loses 0.6 % in f16x3 mode, where wake-up latency matters more)
-        auto gen_wait = [](uint32_t bar, uint32_t parity) {
-            if (X3) mbar_wait(bar, parity);
-            else mbar_wait_relaxed(bar, parity);
-        };
-        const int gtid = (warp - kEpiWarps) * 32 + lane;                // 0..511
-        uint32_t rs = 0, rph = 0, mi = 0;     // ring cursor: slot index and phase
-        constexpr int kSlotsPerMember = C::NCH + C::NCH * C::KAT;
-        uint8_t *const cache = (a.cache && a.n_pass > 1)
-                                   ? a.cache + (size_t)blockIdx.x * kSlotsPerMember * C::SLOT_BYTES : nullptr;
-        const int r2 = gtid >> 3, c82 = gtid & 7;
-        const int row_base = PAIR ? 64 * (int)rank : 0;                  // this CTA's 64 rows of every kNC-row chunk
-        auto w2_index = [&](int nc, int ka) { return L.off_w2 + (nc * kNC + row_base + r2) * H + ka * 64 + c82 * 8; };
-        // theta of a layer-2 octet does not depend on the member: it is copied one slot ahead into this thread's own
-        // staging cells with cp.async (no registers, no scoreboard), so its L2 latency never reaches the FFMAs
-        uint32_t tq = 0;                                                 // generated layer-2 slots so far (stage = tq & 1)
-        auto stage_cell = [&](uint32_t st, int half) { return th_stage + (st * 2 + half) * kGenThreads + gtid; };
-        auto stage_fetch = [&](uint32_t st, int nc, int ka) {
-            const float *src = a.theta + w2_index(nc, ka);
-            cp_async16(smem_u32(stage_cell(st, 0)), src);
-            cp_async16(smem_u32(stage_cell(st, 1)), src + 4);
-            cp_async_commit();
-        };
-        constexpr bool kStageTheta = X3;      // measured: +1 % in f16x3 mode, -1 % in f16 mode (one ring slot fewer)
-        if (kStageTheta) stage_fetch(0, 0, 0);
-        for (int64_t m = first; m < a.n_local; m += stride, ++mi) {
-            const uint32_t member = (uint32_t)(a.member_offset + (uint64_t)m);
-            // ---- small fp32 arrays: b1 | b2 | W3[8][H] | b3[8]
-            const uint32_t p = mi & 1;
-            float *sm = small + p * C::SMALL_FLOATS;
-            gen_wait(smem_u32(&bars->small_empty[p]), ((mi >> 1) & 1) ^ 1);
-            for (int i = gtid; i < H / 4; i += kGenThreads) {                // b1, b2: aligned quads
-                const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + i), member, gen, kStreamNesEps, a.key,
-                                                 a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + i));
-                const float4 v2 =
-                    perturbed_quad((uint32_t)((L.off_b2 >> 2) + i), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                   __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + i));
-                // f16x3 epilogue evaluates tanh(v + b) as 1 - 2/(1 + 2^(v*c + b*c)), c = 2 log2 e: store b*c
-                const float bsc = X3 ? kTwoLog2e : 1.0f;
-                reinterpret_cast<float4 *>(sm)[i] = make_float4(v1.x * bsc, v1.y * bsc, v1.z * bsc, v1.w * bsc);
-                reinterpret_cast<float4 *>(sm + H)[i] = make_float4(v2.x * bsc, v2.y * bsc, v2.z * bsc, v2.w * bsc);
-            }
-            for (int i = gtid; i < L.A * H / 4; i += kGenThreads)            // W3' [q][n] row-major: aligned quads
-                reinterpret_cast<float4 *>(sm + 2 * H)[i] =
-                    perturbed_quad((uint32_t)((L.off_w3 >> 2) + i), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                   __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + i));
-            if (mi < 2)                                                       // unused action rows stay zero (finite)
-                for (int i = L.A * H + gtid; i < H * kMaxA; i += kGenThreads) sm[2 * H + i] = 0.f;
-            if (gtid < L.A) sm[2 * H + kMaxA * H + gtid] = perturbed1(a.theta, L.off_b3 + gtid, a.sigma, member, gen, a.key);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bars->small_full[p]));
-
-            for (int pass = 0; pass < a.n_pass; ++pass) {
-                // ---- layer-1 tiles: rows [64nc, 64nc+64) of W1', k < d0 (zero padded to 32)
-                for (int nc = 0; nc < C::NCH; ++nc) {
-                    const uint32_t s = rs, sph = rph;
-                    if (++rs == (uint32_t)a.n_slots) { rs = 0; rph ^= 1; }
-                    gen_wait(smem_u32(&bars->slot_empty[s]), sph ^ 1);
-                    uint8_t *slot = ring + (size_t)s * C::SLOT_BYTES;
-                    uint8_t *mirror = cache ? cache + (size_t)nc * C::SLOT_BYTES : nullptr;
-                    if (gtid < 256 && pass > 0 && cache) {
-                        uint4 hi, lo;
-                        load_octet<X3>(hi, lo, mirror, gtid >> 2, gtid & 3);
-                        put_octet<X3>(slot, gtid >> 2, gtid & 3, hi, lo);
-                    } else if (gtid < 256) {   // 64 rows x 4 octets = 256 items
-                        const int r = gtid >> 2, c8 = gtid & 3;
-                        const int n = nc * kNC + row_base + r;
-                        float w[8];
-                        if ((L.d0 & 3) == 0) {                                // row starts are quad aligned
+                for (int r = 0; r < 2; ++r) {
+                    const int t = ra + 8 * r;
 #pragma unroll
-                            for (int hq = 0; hq < 2; ++hq) {
-                                const int k = c8 * 8 + hq * 4;
-                                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                                if (k < L.d0) {
-                                    const int j = L.off_w1 + n * L.d0 + k;
-                                    v = perturbed_quad((uint32_t)(j >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                                       __ldg(reinterpret_cast<const float4 *>(a.theta + j)));
-                                }
-                                w[4 * hq] = v.x; w[4 * hq + 1] = v.y; w[4 * hq + 2] = v.z; w[4 * hq + 3] = v.w;
-                            }
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) {
-                                const int k = c8 * 8 + e;
-                                w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, a.sigma, member, gen, a.key) : 0.f;
-                            }
+                    for (int q = 0; q < NA; ++q) {
+                        if (q < L.A) {
+                            float v = act[q][r] + b3[q];
+                            v = fminf(fmaxf(v, -a.clip), a.clip);
+                            const float dd = v - __ldg(a.target + (int64_t)t * L.A + q);
+                            sq = __fmaf_rn(dd, dd, sq);
                         }
-                        store_octet<X3>(slot, mirror, r, c8, w);
-                    }
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) arrive_leader(&bars->slot_full[s]);
-                }
-                // ---- layer-2 tiles: rows [64nc, +64) x k [64ka, +64) of W2'
-                for (int nc = 0; nc < C::NCH; ++nc) {
-                    for (int ka = 0; ka < C::KAT; ++ka) {
-                        const uint32_t s = rs, sph = rph;
-                        if (++rs == (uint32_t)a.n_slots) { rs = 0; rph ^= 1; }
-                        uint8_t *slot = ring + (size_t)s * C::SLOT_BYTES;
-                        uint8_t *mirror = cache ? cache + (size_t)(C::NCH + nc * C::KAT + ka) * C::SLOT_BYTES : nullptr;
-                        if (pass > 0 && cache) {
-                            uint4 hi, lo;                                     // issued before the ring wait: L2 latency overlaps it
-                            load_octet<X3>(hi, lo, mirror, r2, c82);
-                            gen_wait(smem_u32(&bars->slot_empty[s]), sph ^ 1);
-                            put_octet<X3>(slot, r2, c82, hi, lo);
-                        } else {   // 64 rows x 8 octets = 512 items: one per thread
-                            const uint32_t stg = tq & 1;
-                            ++tq;
-                            int nnc = nc, nka = ka + 1;                       // next generated slot (wraps to the next member)
-                            if (nka == C::KAT) { nka = 0; if (++nnc == C::NCH) nnc = 0; }
-                            if (kStageTheta) stage_fetch(stg ^ 1, nnc, nka);
-                            const int j0 = w2_index(nc, ka);
-                            float4 t0, t1;
-                            if (!kStageTheta) {
-                                t0 = __ldg(reinterpret_cast<const float4 *>(a.theta + j0));
-                                t1 = __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4));
-                            }
-                            const uint4 x0 = philox4x32((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, a.key);
-                            const uint4 x1 = philox4x32((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, a.key);
-                            const BmParts pa = box_muller_parts(x0.x, x0.y, a.neg2ln2_sigma2, a.key.one_bits);
-                            const BmParts pb = box_muller_parts(x0.z, x0.w, a.neg2ln2_sigma2, a.key.one_bits);
-                            const BmParts pc = box_muller_parts(x1.x, x1.y, a.neg2ln2_sigma2, a.key.one_bits);
-                            const BmParts pd = box_muller_parts(x1.z, x1.w, a.neg2ln2_sigma2, a.key.one_bits);
-                            if (kStageTheta) {
-                                cp_async_wait<1>();                           // this slot's theta has landed
-                                t0 = *stage_cell(stg, 0);
-                                t1 = *stage_cell(stg, 1);
-                            }
-                            const float4 w0 = make_float4(__fmaf_rn(pa.nr, pa.c, t0.x), __fmaf_rn(pa.nr, pa.s, t0.y),
-                                                          __fmaf_rn(pb.nr, pb.c, t0.z), __fmaf_rn(pb.nr, pb.s, t0.w));
-                            const float4 w1 = make_float4(__fmaf_rn(pc.nr, pc.c, t1.x), __fmaf_rn(pc.nr, pc.s, t1.y),
-                                                          __fmaf_rn(pd.nr, pd.c, t1.z), __fmaf_rn(pd.nr, pd.s, t1.w));
-                            const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-                            gen_wait(smem_u32(&bars->slot_empty[s]), sph ^ 1);
-                            store_octet<X3>(slot, mirror, r2, c82, w);
-                        }
-                        fence_proxy_async_smem();
-                        __syncwarp();
-                        if (lane == 0) arrive_leader(&bars->slot_full[s]);
                     }
                 }
             }
         }
+        // ---- member done: reduce squared error over all rows (fixed order -> deterministic)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+        if (lane == 0) fit_part[warp] = sq;
+        __syncthreads();
+        if (tid == 0) {
+            double f = 0.0;
+            for (int w = 0; w < kTcThreads / 32; ++w) f += (double)fit_part[w];
+            // a cluster adds its two halves into the (pre-zeroed) output: two commutative fp32 adds -> deterministic
+            if (CL == 2) atomicAdd(a.fitness + m, (float)(-f));
+            else a.fitness[m] = (float)(-f);
+        }
     }
-    cp_async_wait<0>();                    // the generators' last (unused) theta prefetch
-    tc_fence_before();
-    __syncthreads();
-    if (PAIR) cluster_sync_all();          // no CTA leaves (or frees TMEM) while its peer may still signal or read it
-    if (warp == kMmaWarp) {
-        if (PAIR) tmem_dealloc2(tmem, 512);
-        else tmem_dealloc(tmem, 512);
-    }
+    if (CL == 2) cluster_sync_all();          // no CTA leaves while its peer may still write into its shared memory
 }
 
-template <int H, int MODE, int NT, bool PAIR>
-static int launch_tc_nt(TcArgs &a, cudaStream_t st) {
-    using C = TcCfg<H, MODE, PAIR>;
-    const int tiles_total = a.T / 128;
-    a.n_pass = tiles_total / (PAIR ? 2 : NT);
-    a.n_tiles = PAIR ? a.n_pass : tiles_total;                 // X tiles held by ONE CTA
-    const size_t fixed = 2 * C::SMALL_FLOATS * sizeof(float) + sizeof(TcBars) + 1024 + (C::X3 ? kThetaStageBytes + 16 : 0);
-    const size_t xbytes = (size_t)a.n_tiles * C::X_TILE_BYTES;
-    const int per_member = C::NCH + C::NCH * C::KAT;
-    int n_slots = xbytes + fixed >= 227 * 1024 ? 0 : (int)((227 * 1024 - fixed - xbytes) / C::SLOT_BYTES);
-    if (n_slots > 32) n_slots = 32;
-    if (n_slots > 2 * per_member) n_slots = 2 * per_member;
-    if (n_slots < 4) {
-        set_error("des_nes_eval(tensor): tape_len %d leaves no shared memory for the weight ring (H=%d)", a.T, H);
-        return DES_ERR_UNSUPPORTED;
-    }
-    a.n_slots = n_slots;
-    const size_t smem = xbytes + (size_t)n_slots * C::SLOT_BYTES + fixed;
-    int dev = 0, sms = 148;
+template <int H, bool X3, int CL, int NA>
+static int launch_tc(TcArgs &a, cudaStream_t st) {
+    using C = TcCfg<H, X3>;
+    a.n_pass = a.T / 128 / CL;
+    int dev = 0, sms = 132;
     DES_CUDA(cudaGetDevice(&dev));
     DES_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    DES_CUDA(cudaFuncSetAttribute(eval_tc_kernel<H, MODE, NT, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int threads = kTcThreads;
-    if (PAIR) {
-        // each pair accumulates its two halves into the output with atomicAdd: zero it first
+    DES_CUDA(cudaFuncSetAttribute(eval_tc_kernel<H, X3, CL, NA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    if (CL == 2) {
+        // each cluster accumulates its two halves into the output with atomicAdd: zero it first
         DES_CUDA(cudaMemsetAsync(a.fitness, 0, (size_t)a.n_local * sizeof(float), st));
-        const int64_t pairs = a.n_local < sms / 2 ? a.n_local : sms / 2;
+        const int64_t clusters = a.n_local < sms / 2 ? a.n_local : sms / 2;
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(2 * pairs));
-        cfg.blockDim = dim3(threads);
-        cfg.dynamicSmemBytes = smem;
+        cfg.gridDim = dim3((unsigned)(2 * clusters));
+        cfg.blockDim = dim3(kTcThreads);
+        cfg.dynamicSmemBytes = C::SMEM;
         cfg.stream = st;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -760,80 +379,41 @@ static int launch_tc_nt(TcArgs &a, cudaStream_t st) {
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        DES_CUDA(cudaLaunchKernelEx(&cfg, eval_tc_kernel<H, MODE, NT, PAIR>, a));
+        DES_CUDA(cudaLaunchKernelEx(&cfg, eval_tc_kernel<H, X3, CL, NA>, a));
     } else {
         const int64_t grid = a.n_local < sms ? a.n_local : sms;
-        eval_tc_kernel<H, MODE, NT, PAIR><<<(unsigned)grid, threads, smem, st>>>(a);
+        eval_tc_kernel<H, X3, CL, NA><<<(unsigned)grid, kTcThreads, C::SMEM, st>>>(a);
     }
     DES_LAUNCH_CHECK("eval_tc_kernel");
     return DES_OK;
 }
 
-// CTA pairs (cta_group::2): each CTA of a 2-cluster keeps one tile and generates half of every weight tile.
-//   DES_TC_PAIR=1 (default)  pairs where two tiles do not fit one CTA's tensor memory (f16x3 at H = 256)
-//   DES_TC_PAIR=2            pairs wherever the shape allows it (H a multiple of 128, even number of tiles);
-//                            measured slower than two tile slots per CTA for f16 at H = 256 (10.3 vs 9.7 ms)
-//   DES_TC_PAIR=0            never (multi-pass with the L2 tile cache instead)
-static int pair_mode() {
-    const char *e = getenv("DES_TC_PAIR");
-    if (!e) return 1;
-    return e[0] == '0' ? 0 : (e[0] == '2' ? 2 : 1);
-}
-static bool pair_enabled() { return pair_mode() != 0; }
-
-template <int H, int MODE>
-static int launch_tc(TcArgs &a, cudaStream_t st) {
-    using C = TcCfg<H, MODE, false>;
-    const int tiles = a.T / 128;
-    if constexpr (H % 128 == 0) {
-        const bool want = (C::NT_MAX < 2 && pair_mode() >= 1) || pair_mode() == 2;
-        if (tiles % 2 == 0 && want) return launch_tc_nt<H, MODE, 1, true>(a, st);
-    }
-    if (C::NT_MAX >= 2 && tiles % 2 == 0) return launch_tc_nt<H, MODE, (C::NT_MAX >= 2 ? 2 : 1), false>(a, st);
-    return launch_tc_nt<H, MODE, 1, false>(a, st);
+template <int H, bool X3>
+static int launch_tc_h(TcArgs &a, cudaStream_t st) {
+    const bool even = (a.T / 128) % 2 == 0;
+    if (a.L.A <= 4) return even ? launch_tc<H, X3, 2, 4>(a, st) : launch_tc<H, X3, 1, 4>(a, st);
+    return even ? launch_tc<H, X3, 2, kMaxA>(a, st) : launch_tc<H, X3, 1, kMaxA>(a, st);
 }
 
-static void tc_shape(int H, bool x3, int T, int &n_pass, size_t &slot_bytes, int &slots_per_member) {
-    const int acols = x3 ? H : H / 2;
-    const int nt_max = 512 / (acols + 2 * 64) >= 2 ? 2 : 1;
-    const int n_tiles = T / 128;
-    const bool pair = H % 128 == 0 && n_tiles % 2 == 0 && ((nt_max < 2 && pair_mode() >= 1) || pair_mode() == 2);
-    const bool two_per_pass = pair || (n_tiles % 2 == 0 && nt_max >= 2);
-    n_pass = two_per_pass ? n_tiles / 2 : n_tiles;
-    const int nc = pair ? 128 : 64;
-    slot_bytes = (size_t)(x3 ? 2 : 1) * 64 * 128;
-    slots_per_member = H / nc + (H / nc) * (H / 64);
-}
+static int tc_passes(int T) { const int tiles = T / 128; return tiles % 2 == 0 ? tiles / 2 : tiles; }
 
 size_t eval_tc_workspace_bytes(des_dims dims, int precision) {
     const int H = dims.hidden;
-    if (!(H == 64 || H == 128 || H == 256) || dims.tape_len % 128 != 0) return 0;
-    int n_pass, spm;
-    size_t sb;
-    tc_shape(H, precision == DES_FWD_F16X3, dims.tape_len, n_pass, sb, spm);
-    if (n_pass <= 1) return 0;
-    int dev = 0, sms = 148;
+    if (!(H == 64 || H == 128 || H == 256) || dims.tape_len % 128 != 0 || tc_passes(dims.tape_len) <= 1) return 0;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
         cudaGetLastError();
-        sms = 148;
+        sms = 132;
     }
-    return (size_t)sms * spm * sb;
+    // one image of a member's W2' chunks per CTA: H/64 chunks of (hi [+ lo]) 64 x H fp16
+    return (size_t)sms * (size_t)H * H * 2 * (precision == DES_FWD_F16X3 ? 2 : 1);
 }
-
-bool eval_pair_supported(des_dims dims, int precision);
-int eval_pair_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims, double sigma,
-                     double clip, uint64_t seed, uint64_t generation, const des_state *state, int64_t member_offset,
-                     int64_t n_local, int precision, cudaStream_t st);
 
 int eval_tc_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                    double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
                    int64_t member_offset, int64_t n_local, int precision, void *workspace, size_t workspace_bytes,
                    cudaStream_t st) {
     const int H = dims.hidden;
-    // tape of 256 observations on CTA pairs: the pipelined pair kernel (des_eval_pair.cu)
-    if (pair_enabled() && eval_pair_supported(dims, precision))
-        return eval_pair_launch(fitness, theta, obs, target, dims, sigma, clip, seed, generation, state, member_offset,
-                                n_local, precision, st);
     if (!(H == 64 || H == 128 || H == 256) || dims.state_dim > kK1 || dims.action_dim > kMaxA || dims.tape_len % 128 != 0) {
         set_error("des_nes_eval(tensor): needs hidden in {64,128,256}, state_dim <= %d, action_dim <= %d, tape_len %% 128 == 0 "
                   "(got d0=%d H=%d A=%d T=%d); use DES_FWD_FP32 for other shapes", kK1, kMaxA, dims.state_dim, H,
@@ -853,14 +433,12 @@ int eval_tc_launch(float *fitness, const float *theta, const float *obs, const f
     a.key = make_philox_key(seed); a.gen = (uint32_t)generation;
     a.member_offset = (uint64_t)member_offset; a.n_local = n_local;
     const bool x3 = precision == DES_FWD_F16X3;
-    // multi-pass shapes: with a workspace, the tiles generated in pass 0 are mirrored to it and copied back in the
-    // later passes (L2-resident, 148 x ~320 KB); without one they are regenerated per pass (slower, same results)
     const size_t need = eval_tc_workspace_bytes(dims, precision);
     a.cache = (need > 0 && workspace && workspace_bytes >= need && ((uintptr_t)workspace & 15) == 0) ? (uint8_t *)workspace : nullptr;
     switch (H) {
-        case 64: return x3 ? launch_tc<64, DES_FWD_F16X3>(a, st) : launch_tc<64, DES_FWD_F16>(a, st);
-        case 128: return x3 ? launch_tc<128, DES_FWD_F16X3>(a, st) : launch_tc<128, DES_FWD_F16>(a, st);
-        default: return x3 ? launch_tc<256, DES_FWD_F16X3>(a, st) : launch_tc<256, DES_FWD_F16>(a, st);
+        case 64: return x3 ? launch_tc_h<64, true>(a, st) : launch_tc_h<64, false>(a, st);
+        case 128: return x3 ? launch_tc_h<128, true>(a, st) : launch_tc_h<128, false>(a, st);
+        default: return x3 ? launch_tc_h<256, true>(a, st) : launch_tc_h<256, false>(a, st);
     }
 }
 

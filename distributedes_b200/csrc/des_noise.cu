@@ -33,7 +33,7 @@ static int launch_rows(bool perturb, float *out, const float *theta, int64_t n, 
     const int64_t total = n * ((P + 3) / 4);
     const int threads = 256;
     int64_t blocks = (total + threads - 1) / threads;
-    if (blocks > 148 * 64) blocks = 148 * 64;
+    if (blocks > 132 * 64) blocks = 132 * 64;      // 132 SMs (H100 SXM)
     const PhiloxKey key = make_philox_key(seed);
     if (perturb)
         noise_rows_kernel<true><<<(unsigned)blocks, threads, 0, st>>>(out, theta, n, P, (float)sigma, key,

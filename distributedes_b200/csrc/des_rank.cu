@@ -354,7 +354,7 @@ extern "C" DES_API int des_centered_rank(float *shaped_out_dev, int32_t *rank_ou
     DES_CUDA(cudaMemsetAsync(counts, 0, (size_t)n_local * sizeof(int32_t), st));
     const unsigned bx = (unsigned)((n_local + kRankThreads - 1) / kRankThreads);
     // enough j-slices to fill the machine a few times over, each a multiple of the smem tile
-    int64_t want_blocks = 148 * 8;
+    int64_t want_blocks = 132 * 8;                 // 132 SMs (H100 SXM)
     int64_t by = (want_blocks + bx - 1) / bx;
     int64_t max_by = (N + kRankTile - 1) / kRankTile;
     if (by > max_by) by = max_by;

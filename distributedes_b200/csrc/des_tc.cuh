@@ -1,10 +1,14 @@
-// tcgen05 / TMEM / mbarrier primitives (inline PTX, sm_100a).  Layout facts used here were checked on
-// hardware with scripts/probe/umma_probe.cu:
-//   * kind::f16 MMA, M=128: accumulator D[m][n] lives at TMEM lane m, column n (fp32);
-//     an A operand read from TMEM has row m at lane m, fp16 elements packed two per 32-bit column;
-//   * B operand in shared memory, K-major, SWIZZLE_128B: rows of 64 fp16 (128 B), 16-byte chunk c of
-//     row r stored at chunk (c ^ (r & 7)); 8-row groups 1024 B apart; K-advance of 16 elements = +32 B
+// Hopper tensor-core primitives (inline PTX, sm_90a): wgmma, mbarrier, TMA, cluster shared memory.
+//
+// Operand layouts used by the kernels:
+//   * shared-memory operands are K-major SWIZZLE_128B: rows of 64 fp16 (128 B), 16-byte chunk c of row r stored at chunk
+//     (c ^ (r & 7)); 8-row groups 1024 B apart (the descriptor's stride byte offset); a K-advance of 16 elements is +32 B
 //     on the descriptor start address; the atom base must be 1024-byte aligned.
+//   * wgmma m64nNk16 with fp32 accumulators: warp w of the warpgroup owns rows 16w + lane/4 and 16w + lane/4 + 8; for
+//     every 8-column block j it holds d[4j + 0..1] = (row lane/4, columns 8j + 2(lane%4) + 0..1) and d[4j + 2..3] = the
+//     same columns of row lane/4 + 8.  An fp16 A operand in registers (k16 step) has the same per-warp layout: a[0] =
+//     row lane/4, k = 2(lane%4) + 0..1; a[1] = row lane/4 + 8; a[2], a[3] = the same rows at k + 8.  So the accumulator
+//     columns [16s, 16s + 16) of one layer, packed to fp16, are the A operand of k-step s of the next layer.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -19,9 +23,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// try_wait suspends the warp in hardware until the phase completes or the time hint (ns) expires, so a
-// long hint keeps waiting warps out of the issue slots (ncu: 23% of issued instructions were spin loops
-// with the default hint).
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -35,63 +36,30 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {
     }
 }
-// For waits that are long when they happen at all (a producer that ran ahead of its consumer): back off between polls
-// so the waiting warps stay out of the issue slots of the warps they are waiting for (ncu: half of the instructions the
-// generator warps executed were try_wait/NANOSLEEP/BRA of the tight loop above).
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {
-        asm volatile("nanosleep.u32 %0;" ::"r"(64u));
-    }
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// generic-proxy writes (st.shared) -> visible to the async proxy (tcgen05.mma operand fetch)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// generic-proxy writes (st.shared, st.shared::cluster) -> visible to the async proxy (wgmma operand fetch)
+__device__ __forceinline__ void fence_proxy_async_cluster() { asm volatile("fence.proxy.async.shared::cluster;" ::: "memory"); }
 
-// ---- TMEM allocation -------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {    // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors -----------------------------------------------------------------------------------
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B) |
-// [46,48) version=1 | [61,64) layout=2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// Instruction descriptor, kind::f16: fp16 A/B (format 0), fp32 accumulate (c_format 1 at [4,6)),
-// both operands K-major, N>>3 at [17,23), M>>4 at [24,29)   (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]^T, issued by ONE thread.
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// ---- TMA ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void *map, int c0, int c1, uint32_t bar) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// mbarrier arrives once every tcgen05 op issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
 }
 
-// ---- CTA pairs (cluster of 2, cta_group::2): checked on hardware with scripts/probe/umma2_probe.cu ---------------
-// M = 256 = 2 x 128 rows: each CTA keeps its 128 rows of A and D in its own TMEM; B is split by N, CTA r holding rows
-// [N/2*r, N/2*(r+1)) in ITS shared memory at the same offset; the leader (rank 0) issues, commits multicast.
+// one lane of a fully converged warp
+__device__ __forceinline__ bool elect_one() {
+    uint32_t pred;
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
+    return pred != 0;
+}
+
+// ---- clusters ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -100,93 +68,63 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+// address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t map_cluster(uint32_t saddr, uint32_t rank) {
     uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(bar), "r"(rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(saddr), "r"(rank));
+    return ra;
 }
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {   // same warp of BOTH CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma2_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma2_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrives on the barrier at this offset in BOTH CTAs once every tcgen05 op issued so far has completed
-__device__ __forceinline__ void mma2_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
+__device__ __forceinline__ void st_cluster_v4(uint32_t caddr, const uint4 &v) {
+    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(caddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+                 : "memory");
 }
 
-// ---- TMEM <-> registers: this thread's lane, 32 / 16 consecutive 32-bit columns ---------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
-        "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
+// ---- wgmma --------------------------------------------------------------------------------------------
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor):
+// [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B) | [62,64) layout=1 (128B)
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&w)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-        "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-        ::"r"(taddr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]),
-          "r"(w[9]), "r"(w[10]), "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15]), "r"(w[16]), "r"(w[17]),
-          "r"(w[18]), "r"(w[19]), "r"(w[20]), "r"(w[21]), "r"(w[22]), "r"(w[23]), "r"(w[24]), "r"(w[25]), "r"(w[26]),
-          "r"(w[27]), "r"(w[28]), "r"(w[29]), "r"(w[30]), "r"(w[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&w)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-        ::"r"(taddr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]),
-          "r"(w[9]), "r"(w[10]), "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15]) : "memory");
-}
-
-// 16-column variants for the software-pipelined epilogue.  tmem_wait_ld16 carries the destination registers of the
-// outstanding load as in/out operands, so no use of them can be scheduled above the wait.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld16(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :: "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&w)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 ::"r"(taddr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
-
-// ---- per-thread asynchronous global->shared copies (LDGSTS): no destination registers, no scoreboard held ---------
-__device__ __forceinline__ void cp_async16(uint32_t saddr, const void *gptr) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across an asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define DES_F8(d, o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+                     "+f"(d[o + 6]), "+f"(d[o + 7])
+
+// D[64 x 64] (+)= A[64 x 16] (registers, fp16) * B[64 x 16]^T (shared memory, K-major), fp32 accumulate
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : DES_F8(d, 0), DES_F8(d, 8), DES_F8(d, 16), DES_F8(d, 24)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(acc));
+}
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both in shared memory (K-major), fp32 accumulate
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : DES_F8(d, 0), DES_F8(d, 8), DES_F8(d, 16), DES_F8(d, 24), DES_F8(d, 32), DES_F8(d, 40), DES_F8(d, 48),
+          DES_F8(d, 56)
+        : "l"(a_desc), "l"(b_desc), "r"(acc));
+}
+#undef DES_F8
 
 // ---- fp16 packing -------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {       // element k (even) low half, k+1 high half
@@ -202,84 +140,20 @@ __device__ __forceinline__ void split_h2(float a, float b, uint32_t &hi, uint32_
     lo = *reinterpret_cast<const uint32_t *>(&l);
 }
 
-// packed pairs ----------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t tanh_h2(uint32_t x) {   // MUFU.TANH on both fp16 halves
-    uint32_t y;
-    asm("tanh.approx.f16x2 %0, %1;" : "=r"(y) : "r"(x));
-    return y;
-}
-__device__ __forceinline__ uint32_t add_h2(uint32_t a, uint32_t b) {
-    uint32_t y;
-    asm("add.rn.f16x2 %0, %1, %2;" : "=r"(y) : "r"(a), "r"(b));
-    return y;
-}
-// d = a*b + c on two packed fp32 lanes (Blackwell FFMA2): one issue slot for two FMAs
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    uint64_t ra, rb, rc, rd;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-    return d;
-}
-
-__device__ __forceinline__ uint64_t pk2(float2 a) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y));
-    return r;
-}
-__device__ __forceinline__ float2 upk2(uint64_t r) {
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(r));
-    return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {          // two fp32 adds in one issue slot
-    uint64_t rd;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(pk2(a)), "l"(pk2(b)));
-    return upk2(rd);
-}
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-    uint64_t rd;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(pk2(a)), "l"(pk2(b)));
-    return upk2(rd);
-}
-// tanh(v + b) for two lanes with the bias pre-scaled: bs = b * 2 log2(e).
-//   e = 2^(v * 2log2e + bs);  tanh = 1 - 2/(1 + e)      abs err ~2e-7; 2 MUFU + 1.5 packed FP32 ops per element
-// (Replacing the MUFU reciprocal by a bit-trick seed + Halley + Newton step on packed FFMA2 — 7 instead of 3.5 issue
-//  slots per element, half the MUFU work — was measured SLOWER: eval 13.9 -> 15.1 ms.  The epilogue warps are bound
-//  by issue slots, not by the XU pipe.)
+// tanh(v + b) with the bias pre-scaled: bs = b * 2 log2(e).
+//   e = 2^(v * 2log2e + bs);  tanh = 1 - 2/(1 + e)      abs err ~2e-7; 2 MUFU + 3 FP32 ops
 constexpr float kTwoLog2e = 2.8853900817779268f;
-__device__ __forceinline__ float2 tanh_acc2(float2 v, float2 bs) {
-    const float2 arg = ffma2(v, make_float2(kTwoLog2e, kTwoLog2e), bs);
-    float2 e, r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(arg.x));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(arg.y));
-    const float2 d = fadd2(e, make_float2(1.0f, 1.0f));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.x) : "f"(d.x));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.y) : "f"(d.y));
-    return ffma2(make_float2(-2.0f, -2.0f), r, make_float2(1.0f, 1.0f));
-}
-// hi = fp16(x), lo = fp16(x - hi) for a pair, the subtraction packed
-__device__ __forceinline__ void split_h2p(float2 x, uint32_t &hi, uint32_t &lo) {
-    const __half2 h = __floats2half2_rn(x.x, x.y);
-    const float2 d = fsub2(x, __half22float2(h));
-    const __half2 l = __floats2half2_rn(d.x, d.y);
-    hi = *reinterpret_cast<const uint32_t *>(&h);
-    lo = *reinterpret_cast<const uint32_t *>(&l);
+__device__ __forceinline__ float tanh_acc_b(float v, float bs) {
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__fmaf_rn(v, kTwoLog2e, bs)));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+    return __fmaf_rn(-2.0f, r, 1.0f);
 }
 
 __device__ __forceinline__ float tanh_fast(float x) {       // MUFU.TANH, max rel err 2^-11
     float y;
     asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-__device__ __forceinline__ float tanh_acc(float x) {        // 1 - 2/(1+e^{2x}), abs err ~2e-7
-    float e, r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.8853900817779268f));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-    return __fmaf_rn(-2.0f, r, 1.0f);
 }
 
 }  // namespace tc

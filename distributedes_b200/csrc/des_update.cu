@@ -38,7 +38,7 @@ __host__ inline GradPlan grad_plan(int64_t n_local, int64_t P) {
     const int64_t bx = (p.nq + kGradThreads - 1) / kGradThreads;
     // ~16 resident CTAs of 128 threads per SM, a few waves; keep slices >= 32 members so that the
     // per-thread fp32 running sum stays short (<= 1024 terms) and the setup cost is amortised.
-    int64_t want = (148 * 16 * 2 + bx - 1) / bx;
+    int64_t want = (132 * 16 * 2 + bx - 1) / bx;     // 132 SMs (H100 SXM)
     int64_t max_chunks = (n_local + 31) / 32;
     int64_t min_chunks = (n_local + 1023) / 1024;
     if (want > max_chunks) want = max_chunks;

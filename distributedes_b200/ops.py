@@ -1,7 +1,7 @@
 """Thin torch-tensor front ends for the C-ABI kernels (include/des_b200.h).
 
 PyTorch is plumbing here: it owns device memory and the stream; every op below passes raw
-pointers to libdes_b200.so, which enqueues hand-written sm_100a kernels on the current stream.
+pointers to libdes_b200.so, which enqueues hand-written sm_90a kernels on the current stream.
 CPU tensors are an error (there is no CPU fallback).
 """
 from __future__ import annotations
@@ -298,7 +298,7 @@ def _cma_rank_mu(Y, w, out, packed, path):
 
 def cma_rank_mu(Y, w, out=None, path=None):
     """dC[n,n] = sum_i w_i y_i y_i^T for Y[lambda_local, n] (rank-mu term of es.tell, cma_es.py:90).
-    path: None = tensor cores (split-fp16 tcgen05 SYRK) for n >= 256, fp32 FFMA below; 'tc' / 'ffma' force one."""
+    path: None = tensor cores (split-fp16 wgmma SYRK) for n >= 256, fp32 FFMA below; 'tc' / 'ffma' force one."""
     lam, n = Y.shape
     if w.numel() != lam:
         raise RuntimeError('w has %d entries, Y has %d rows' % (w.numel(), lam))

@@ -1,5 +1,5 @@
 /*
- * des_b200.h — C ABI of the B200-native Evolution-Strategies hot path.
+ * des_b200.h — C ABI of the H100-native (sm_90a) Evolution-Strategies hot path.
  *
  * Drop-in boundary for the per-generation hot path of ShangtongZhang/DistributedES
  * (reference @ c4de970; the reference is pure Python and has no FFI of its own — each entry point
@@ -55,9 +55,9 @@ typedef enum des_status {
 /* Policy-forward arithmetic (StandardFCNet.forward model.py:34-39). */
 typedef enum des_precision {
     DES_FWD_FP32 = 0,     /* CUDA-core FFMA, fp32 everywhere: the parity-grade path              */
-    DES_FWD_F16 = 1,      /* tcgen05 kind::f16: operands rounded to fp16 (11 significant bits,     */
-                          /* like TF32), fp32 accumulate in TMEM, MUFU tanh                        */
-    DES_FWD_F16X3 = 2     /* tcgen05 kind::f16 with hi/lo split operands (3 MMAs), ~fp32 accuracy */
+    DES_FWD_F16 = 1,      /* wgmma f16: operands rounded to fp16 (11 significant bits,             */
+                          /* like TF32), fp32 accumulate, MUFU tanh                                */
+    DES_FWD_F16X3 = 2     /* wgmma f16 with hi/lo split operands (3 MMAs), ~fp32 accuracy         */
 } des_precision;
 
 /* MLP shape (config.py:10-13: state_dim, action_dim, hidden_size) + the tape length. */
@@ -238,7 +238,7 @@ DES_API int des_cma_cov_apply_packed(float *C_dev, const float *tiles_dev, const
                                      double c1, double cmu, void *stream);
 
 /* The rank-mu term on the tensor cores (csrc/des_cma_tc.cu): dC = Zs^T Z with Z = diag(sqrt|w|) Y, operands split into
- * fp16 hi + lo (three tcgen05 MMAs per k-step, fp32 accumulation, TMA-fed) — same result contract as des_cma_rank_mu
+ * fp16 hi + lo (three wgmma MMAs per k-step, fp32 accumulation, TMA-fed) — same result contract as des_cma_rank_mu
  * (packed == 0: full symmetric [n][n]) / des_cma_rank_mu_packed (packed != 0), within 1e-5 of the fp64 restatement in both
  * norms.  Needs des_cma_tc_workspace_bytes(n, lambda_local) bytes of workspace; |sqrt|w_k| * y| must stay below 65504. */
 DES_API size_t des_cma_tc_workspace_bytes(int64_t n, int64_t lambda_local);

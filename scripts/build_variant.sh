@@ -7,10 +7,10 @@ cd "$(dirname "$0")/.."
 python -m distributedes_b200.build > /dev/null
 mkdir -p distributedes_b200/build/variants
 obj=distributedes_b200/build/variants/${src%.cu}_$name.o
-nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden "$@" -c distributedes_b200/csrc/$src -o $obj
+nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden "$@" -c distributedes_b200/csrc/$src -o $obj
 others=""
 for o in distributedes_b200/build/des_*.o; do
   [ "$(basename $o .o)" != "${src%.cu}" ] && others="$others $o"
 done
-nvcc -shared -gencode arch=compute_100a,code=sm_100a -o distributedes_b200/libdes_b200_$name.so $others $obj
+nvcc -shared -gencode arch=compute_90a,code=sm_90a -o distributedes_b200/libdes_b200_$name.so $others $obj
 echo distributedes_b200/libdes_b200_$name.so

@@ -1,4 +1,4 @@
-"""Run a few eager NES generations (for ncu).  python scripts/profile_gen.py [pop] [hidden] [precision] [gens]"""
+"""Run a few eager NES generations (for a profiler: torch.profiler or CUDA events around the kernels).  python scripts/profile_gen.py [pop] [hidden] [precision] [gens]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Two closed-loop generations at the given population for ncu (argv: pop hidden)."""
+"""Two closed-loop generations at the given population for a profiler (argv: pop hidden)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""One rank's kernels of an 8-way sharded generation on ONE GPU (for an ncu launch list): members [0, 8192) of N = 65536.
+"""One rank's kernels of an 8-way sharded generation on ONE GPU (for a profiler launch list): members [0, 8192) of N = 65536.
 python scripts/profile_shard.py [N] [n_local] [hidden] [gens]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

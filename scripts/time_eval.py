@@ -18,7 +18,7 @@ obs, target = orc.synthetic_tape(T, d0, A)
 th = torch.from_numpy(orc.synthetic_theta(d0, H, A)).to(dev)
 o, t = torch.from_numpy(obs).to(dev), torch.from_numpy(target).to(dev)
 kw = dict(hidden=H, sigma=0.1, clip=1.0, seed=9, generation=2, member_offset=0)
-out = {'pop': pop, 'H': H, 'precision': prec, 'v2': os.environ.get('DES_TC_PAIR_V2', '1')}
+out = {'pop': pop, 'H': H, 'precision': prec}
 if ncheck:
     a = ops.nes_eval(th, o, t, precision='fp32', n_local=ncheck, **kw)
     b = ops.nes_eval(th, o, t, precision=prec, n_local=ncheck, **kw)

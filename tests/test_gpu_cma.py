@@ -156,7 +156,7 @@ def test_packed_rank_mu_and_apply_equal_the_full_matrix_path(n, lam):
 
 @pytest.mark.parametrize('n,lam', [(256, 64), (1000, 130), (2048, 8), (4096, 128)])
 def test_tensor_core_rank_mu_agrees_with_the_ffma_kernel(n, lam):
-    """des_cma_rank_mu_tc (split-fp16 tcgen05 SYRK, TMA-fed) against des_cma_rank_mu (fp32 FFMA) and the fp64 restatement,
+    """des_cma_rank_mu_tc (split-fp16 wgmma SYRK, TMA-fed) against des_cma_rank_mu (fp32 FFMA) and the fp64 restatement,
     signed weights, ragged sizes; full and packed outputs carry the same numbers."""
     from distributedes_b200 import ops
     rs = np.random.RandomState(n * 7 + lam)

@@ -87,10 +87,10 @@ def test_eval_fp32_matches_oracle(d0, H, A, T, clip, n, off):
 
 
 TC_CASES = [  # d0, H, A, T, clip, n_local, offset
-    (24, 64, 4, 256, 1.0, 40, 4000),     # two 128-row tiles resident in TMEM
+    (24, 64, 4, 256, 1.0, 40, 4000),     # two 128-row tiles on a 2-CTA cluster
     (24, 64, 4, 128, 1.0, 7, 0),
     (24, 128, 4, 256, 1.0, 9, 123),
-    (24, 256, 4, 256, 1.0, 10, 65000),   # BASELINE configs[3] shape: two passes over the ring
+    (24, 256, 4, 256, 1.0, 10, 65000),   # BASELINE configs[3] shape: one pass on a 2-CTA cluster
     (24, 256, 4, 512, 1.0, 3, 1),
     (8, 64, 2, 128, 2.0, 5, 0),
     (3, 64, 1, 128, 2.0, 6, 0),          # state_dim not a multiple of 4 (generic W1 path)
@@ -101,7 +101,7 @@ TC_CASES = [  # d0, H, A, T, clip, n_local, offset
 @pytest.mark.parametrize('precision,tol', [('f16', 4e-3), ('f16x3', 3e-5)])
 @pytest.mark.parametrize('d0,H,A,T,clip,n,off', TC_CASES)
 def test_eval_tensor_core_matches_oracle(d0, H, A, T, clip, n, off, precision, tol):
-    """tcgen05 forward.  f16: operands rounded to fp16 (2^-11 relative, like TF32) + MUFU tanh.approx (2^-11):
+    """wgmma forward.  f16: operands rounded to fp16 (2^-11 relative, like TF32) + MUFU tanh.approx (2^-11):
     fitness within 4e-3 relative.  f16x3: hi/lo split operands (~2^-22) + accurate tanh: within 3e-5."""
     obs, target = orc.synthetic_tape(T, d0, A)
     theta = orc.synthetic_theta(d0, H, A)
@@ -115,7 +115,7 @@ def test_eval_tensor_core_matches_oracle(d0, H, A, T, clip, n, off, precision, t
 
 
 def test_eval_tensor_core_many_members_equals_fp32_path():
-    """More members than SMs (persistent loop, ring wrap-around, small-array double buffering): the f16x3
+    """More members than SMs (persistent loop, W2' chunk buffers reused across members): the f16x3
     kernel must agree with the fp32 FFMA kernel member by member."""
     d0, H, A, T, n = 24, 64, 4, 256, 1000
     obs, target = orc.synthetic_tape(T, d0, A)
@@ -148,7 +148,7 @@ def test_eval_multi_pass_tile_cache_is_transparent(H, T, precision):
     ref = orc.evaluate_population(th.cpu().numpy(), obs, target, 0.1, 1.0, 4, 1, 5, 8, d0, H, A)
     assert np.max(np.abs(b[:8].cpu().numpy() - ref) / np.abs(ref)) < (3e-5 if precision == 'f16x3' else 4e-3)
     assert ops().eval_workspace(d0, 64, A, 256, 'f16', DEV) is None          # single-pass shape: no scratch needed
-    assert ops().eval_workspace(d0, 256, A, 256, 'f16x3', DEV) is None       # one pass on a CTA pair
+    assert ops().eval_workspace(d0, 256, A, 256, 'f16x3', DEV) is None       # one pass on a 2-CTA cluster
 
 
 def test_eval_state_generation_overrides_argument():
