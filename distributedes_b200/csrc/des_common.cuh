@@ -111,6 +111,13 @@ __device__ __forceinline__ float lg2_approx(float x) {
     asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
+// np.clip(v, -c, c): NaN stays NaN (fminf/fmaxf would return the bound); max/min.NaN cost the same as fmaxf/fminf
+__device__ __forceinline__ float clip_keep_nan(float v, float c) {
+    float y;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(y) : "f"(v), "f"(-c));
+    asm("min.NaN.f32 %0, %0, %1;" : "+f"(y) : "f"(c));
+    return y;
+}
 __device__ __forceinline__ float sqrt_approx(float x) {
     float y;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
                         const int tt = t0 + warp * kObsPerWarp + t;
                         if (tt < a.T) {
                             float v = acc[t] + b;
-                            v = fminf(fmaxf(v, -a.clip), a.clip);          // np.clip, config.py:29,37
+                            v = clip_keep_nan(v, a.clip);          // np.clip, config.py:29,37
                             const float d = v - __ldg(a.target + (int64_t)tt * L.A + n);
                             sq = __fmaf_rn(d, d, sq);
                         }

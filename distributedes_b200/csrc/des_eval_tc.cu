@@ -331,7 +331,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                     for (int q = 0; q < NA; ++q) {
                         if (q < L.A) {
                             float v = act[q][r] + b3[q];
-                            v = fminf(fmaxf(v, -a.clip), a.clip);
+                            v = clip_keep_nan(v, a.clip);
                             const float dd = v - __ldg(a.target + (int64_t)t * L.A + q);
                             sq = __fmaf_rn(dd, dd, sq);
                         }

@@ -162,7 +162,10 @@ def eval_workspace(state_dim, hidden, action_dim, tape_len, precision, device):
 
 def nes_eval(theta, obs, target, *, hidden, sigma, clip, seed, generation=0, state=None, member_offset=0,
              n_local, precision='fp32', out=None, workspace=None):
-    """Fused sample+forward+fitness for members [member_offset, member_offset+n_local) -> fitness[n_local]."""
+    """Fused sample+forward+fitness for members [member_offset, member_offset+n_local) -> fitness[n_local].
+
+    precision 'f16' / 'f16x3' run the hidden layers on tensor cores with fp16 operands: |obs| and |theta'| must stay
+    below 65520, or they overflow to inf.  A NaN action gives a NaN fitness on every path (np.clip keeps NaN)."""
     T, d0 = obs.shape
     A = target.shape[1]
     if target.shape[0] != T:

@@ -153,7 +153,9 @@ DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_total
  * model.py:34-39 over the synthetic tape env (obs_dev [T][d0], target_dev [T][A], both fp32).
  * `state_dev` may be NULL (then `generation` is used); if non-NULL, state_dev->generation wins
  * (graph replay).  precision: see des_precision; DES_FWD_F16 / F16X3 need H in {64,128,256},
- * d0 <= 32, A <= 8, T a multiple of 128 and |values| < 65504 — otherwise DES_ERR_UNSUPPORTED (never a silent fallback).
+ * d0 <= 32, A <= 8, T a multiple of 128 — otherwise DES_ERR_UNSUPPORTED (never a silent fallback).  Their operands
+ * are fp16: |obs| and |theta'| must stay below 65520 or they overflow to inf (the call cannot check values).
+ * A NaN action (from theta, obs or target) makes that member's fitness NaN in every precision, as np.clip does.
  * workspace (optional, may be NULL): des_nes_eval_workspace_bytes() bytes, 16-byte aligned; shapes whose tape does not
  * fit the tensor memory in one pass use it to keep a member's generated weight tiles between passes instead of
  * regenerating them (same results either way). */
