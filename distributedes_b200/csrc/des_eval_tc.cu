@@ -2,26 +2,35 @@
 // hidden-layer GEMMs on Hopper tensor cores (wgmma).
 //
 // One persistent CTA per SM (or one 2-CTA cluster per two SMs, see below) walks its members (Worker.run
-// natural_es.py:27-32 per member).  A CTA has two warpgroups; each owns 64 observation rows of a 128-row tile (one
-// "pass" over the tape is one such tile).  For a member, StandardFCNet.forward (model.py:34-39) is
+// natural_es.py:27-32 per member).  A CTA has two consumer warpgroups; each owns 64 observation rows of a 128-row
+// tile (one "pass" over the tape is one such tile).  For a member, StandardFCNet.forward (model.py:34-39) is
 //
 //   D1 = X  W1'^T            wgmma m64n64k16, A = X (fp16 registers, loaded once per pass), B = W1' (shared memory)
 //   H1 = tanh(D1 + b1')      in registers; packed to fp16 the accumulator IS the A operand of layer 2 (des_tc.cuh)
-//   D2 = H1 W2'^T            wgmma, A = H1 (registers), B = W2' in 64-feature chunks (double-buffered shared memory)
+//   D2 = H1 W2'^T            wgmma, A = H1 (registers), B = W2' in 64-feature chunks (two-stage shared-memory ring)
 //   H2 = tanh(D2 + b2')      epilogue, registers only
 //   a  = H2 W3'^T + b3'      A <= 8 outputs: exact fp32 FFMA in the same epilogue (no third MMA)
 //   fitness += -|| clip(a) - a* ||^2                                              (utils.py:134-137)
 //
-// W' = fp32(theta + sigma*eps) (natural_es.py:28-30) is never stored in HBM: every thread regenerates eps from the
-// counter RNG and writes fp16 operand tiles straight into the 128B-swizzled K-major layout wgmma reads.  The chunk
-// of W2' for the next MMA is generated while the current one runs on the tensor cores (wgmma is asynchronous).
+// W' = fp32(theta + sigma*eps) (natural_es.py:28-30) is never stored in HBM: two producer warpgroups regenerate eps
+// from the counter RNG and write fp16 operand tiles straight into the 128B-swizzled K-major layout wgmma reads.
+// Warp specialisation (512 threads, setmaxnreg: producers 56 registers, consumers 200; 40 / 216 for f16x3, H = 256, NA = 8):
+//   producers  per member: b1 | b2 | W3' | b3 into one of two small-array buffers, W1' into its single buffer once
+//              every consumer of the cluster has run the previous member's layer 1, then the W2' chunks of every
+//              pass into the ring.  They run ahead across member boundaries, bounded only by the buffers.
+//   consumers  layer 1, the layer-2 chunks, the epilogues and the fitness reduction; they never generate weights.
+// Every buffer has full / empty mbarriers: full takes one arrival per producer thread of the cluster (after its
+// stores and a fence.proxy.async), empty one per consumer warp of the cluster, right after the wgmma_wait of the
+// MMAs that read it, so a W2' stage is refilled while the consumers run its epilogue.  Stage and phase come from one
+// running chunk counter that both roles advance alike.  The two consumer warpgroups are not kept in step: fitness
+// partials are double-buffered by member parity and the last consumer warp to finish a member adds them in warp order.
 //
 // Clusters: when the tape has an even number of 128-row tiles, two CTAs of a cluster share a member.  Each evaluates
 // its own tiles and generates HALF of every weight tile, storing it into its own and its peer's shared memory
-// (distributed shared memory); one cluster barrier per chunk publishes both halves.  The flagship shape (T = 256)
-// is then one pass per CTA.  Other shapes loop over passes; with the optional workspace the W2' chunks generated in
-// pass 0 are mirrored to global memory (L2-resident) and copied back in the later passes, without it they are
-// regenerated (same bytes either way).
+// (distributed shared memory) and arriving on both CTAs' barriers.  The flagship shape (T = 256) is then one pass per
+// CTA.  Other shapes loop over passes; with the optional workspace the W2' chunks generated in pass 0 are mirrored
+// to global memory (L2-resident) and copied back in the later passes, without it they are regenerated (same bytes
+// either way).
 //
 // Precision modes
 //   F16    operands rounded to fp16 (11 significant bits, as TF32), fp32 accumulate, MUFU tanh.approx.
@@ -36,7 +45,21 @@ using namespace tc;
 
 constexpr int kK1 = 32;        // layer-1 K (state_dim zero-padded): 2 k-steps of 16
 constexpr int kMaxA = 8;
-constexpr int kTcThreads = 256;
+// Roles: warpgroups 0-1 generate the perturbed weights (one producer warpgroup cannot keep up: a Philox +
+// Box-Muller chain per thread at one warp per scheduler is latency bound), warpgroups 2-3 run the MMAs and epilogues.
+constexpr int kProdWGs = 2;
+constexpr int kProdThreads = 128 * kProdWGs;
+constexpr int kTcThreads = kProdThreads + 256;
+constexpr int kConsWarps = 8;
+// register budgets: the launch gives every thread 65536 / 512 = 128; the producers hand theirs to the consumers.  The
+// producers get 56 (measured on the headline shape: 40 make the kernel 1.2 ms slower, 48 are no faster than 56);
+// only f16x3 at H = 256 with 8 action sums needs more than 200 consumer registers (128 of them layer-1 activations)
+// and gets 256 x 40 + 256 x 216 = 65536.
+template <int H, bool X3, int NA>
+__host__ __device__ constexpr uint32_t prod_regs() { return (H == 256 && X3 && NA == 8) ? 40u : 56u; }
+template <int H, bool X3, int NA>
+__host__ __device__ constexpr uint32_t cons_regs() { return (((65536u / kTcThreads) & ~7u) * kTcThreads - kProdThreads * prod_regs<H, X3, NA>()) / 256u & ~7u; }
+static_assert(cons_regs<256, true, 4>() == 200 && cons_regs<256, true, 8>() == 216, "register split");
 
 template <int H, bool X3>
 struct TcCfg {
@@ -47,7 +70,17 @@ struct TcCfg {
     static constexpr int CHUNK_BYTES = PLANES * KAT * 8192;   // W2' rows [64c, 64c + 64), every k: hi atoms | lo atoms
     static constexpr int W1_BYTES = PLANES * H * 128;         // W1' rows of 128 B (k < 32 used): hi | lo
     static constexpr int SMALL_FLOATS = 2 * H + kMaxA * H + kMaxA;   // b1, b2, W3' [8][H], b3[8]
-    static constexpr size_t SMEM = 1024 + 2 * (size_t)CHUNK_BYTES + W1_BYTES + SMALL_FLOATS * sizeof(float) + 8 * sizeof(float);
+    // mbarriers: W2' stage s full / empty, W1' full / empty, small-array buffer b empty
+    enum { BAR_W2_FULL = 0, BAR_W2_EMPTY = 2, BAR_W1_FULL = 4, BAR_W1_EMPTY = 5, BAR_SMALL_EMPTY = 6, NBARS = 8 };
+    // W2' ring [2][CHUNK_BYTES] | W1' | small [2][SMALL_FLOATS] | fitness partials [2][8] | arrival counters [2] | mbarriers
+    static constexpr size_t OFF_W1 = 2 * (size_t)CHUNK_BYTES;
+    static constexpr size_t OFF_SMALL = OFF_W1 + W1_BYTES;
+    static constexpr size_t OFF_FIT = OFF_SMALL + 2 * (size_t)SMALL_FLOATS * sizeof(float);
+    static constexpr size_t OFF_CNT = OFF_FIT + 2 * kConsWarps * sizeof(float);
+    static constexpr size_t OFF_BAR = (OFF_CNT + 2 * sizeof(uint32_t) + 7) & ~(size_t)7;
+    static constexpr size_t SMEM = 1024 + OFF_BAR + NBARS * sizeof(uint64_t);
+    static_assert(SMEM <= 227 * 1024, "eval_tc_kernel: shared memory over the 227 KB per-block limit");
+    static_assert(SMALL_FLOATS * sizeof(float) % 16 == 0, "small-array buffers must stay float4 aligned");
 };
 
 struct TcArgs {
@@ -108,248 +141,308 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t *w2buf = smem;                                                  // [2][CHUNK_BYTES]
-    uint8_t *w1 = smem + 2 * C::CHUNK_BYTES;                                // [W1_BYTES]
-    float *small = reinterpret_cast<float *>(w1 + C::W1_BYTES);             // [SMALL_FLOATS]
-    float *fit_part = small + C::SMALL_FLOATS;                              // [8]
-    const float *b1 = small, *b2 = small + H, *w3 = small + 2 * H, *b3 = small + 2 * H + kMaxA * H;
+    uint8_t *w1 = smem + C::OFF_W1;                                         // [W1_BYTES]
+    float *small_buf = reinterpret_cast<float *>(smem + C::OFF_SMALL);      // [2][SMALL_FLOATS]
+    float *fit_part = reinterpret_cast<float *>(smem + C::OFF_FIT);         // [2][kConsWarps]
+    uint32_t *fit_cnt = reinterpret_cast<uint32_t *>(smem + C::OFF_CNT);    // [2]
+    const uint32_t bars = smem_u32(smem + C::OFF_BAR);
+    auto bar = [&](int k) { return bars + 8u * (uint32_t)k; };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
     const Layout L = a.L;
     const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
     const int64_t first = blockIdx.x / CL, stride = gridDim.x / CL;
-    uint8_t *const cache = (a.cache && a.n_pass > 1) ? a.cache + (size_t)blockIdx.x * C::NCH * C::CHUNK_BYTES : nullptr;
 
-    auto sync_all = [&]() {
-        if (CL == 2) cluster_sync_all();
-        else __syncthreads();
-    };
-    // a 16-byte chunk of an operand tile (hi plane at `off`, lo plane `lo_off` further) into this CTA and its peer
-    auto put = [&](uint8_t *base, uint32_t off, uint32_t lo_off, const uint4 &hi, const uint4 &lo) {
-        *reinterpret_cast<uint4 *>(base + off) = hi;
-        if (X3) *reinterpret_cast<uint4 *>(base + lo_off + off) = lo;
-        if (CL == 2) {
-            st_cluster_v4(map_cluster(smem_u32(base + off), rank ^ 1u), hi);
-            if (X3) st_cluster_v4(map_cluster(smem_u32(base + lo_off + off), rank ^ 1u), lo);
+    // full: one arrival per producer thread of the cluster (each stores into both CTAs); empty: one per consumer warp
+    // of the cluster (each reads its own CTA's copy, which both producers write); small arrays are per CTA
+    if (tid == 0) {
+        for (int s = 0; s < 2; ++s) {
+            mbar_init(bar(C::BAR_W2_FULL + s), kProdThreads * CL);
+            mbar_init(bar(C::BAR_W2_EMPTY + s), kConsWarps * CL);
+            mbar_init(bar(C::BAR_SMALL_EMPTY + s), kTcThreads - kProdThreads);
         }
-    };
-    // this CTA's share of W2' chunk c (rows [64c, 64c + 64)) into buffer `buf`; pass > 0 copies the cached image back
-    constexpr int kOct = H / 8;                                   // octets per row
-    constexpr int kRows = 64 / CL;                                // rows of a chunk generated here
-    auto gen_chunk = [&](uint32_t member, int c, int pass, int buf) {
-        uint8_t *dst = w2buf + buf * C::CHUNK_BYTES;
-        uint8_t *mirror = cache ? cache + (size_t)c * C::CHUNK_BYTES : nullptr;
-        for (int idx = tid; idx < kRows * kOct; idx += kTcThreads) {
-            const int rr = (int)rank * kRows + idx / kOct, o = idx % kOct;
-            const uint32_t off = (uint32_t)((o >> 3) * 8192 + rr * 128 + (((o & 7) ^ (rr & 7)) << 4));
-            uint4 hi, lo;
-            if (mirror && pass > 0) {
-                hi = *reinterpret_cast<const uint4 *>(mirror + off);
-                if (X3) lo = *reinterpret_cast<const uint4 *>(mirror + C::KAT * 8192 + off);
-                else lo = hi;
-            } else {
-                const int j0 = L.off_w2 + (c * 64 + rr) * H + o * 8;
-                const float4 p0 = perturbed_quad((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                                 __ldg(reinterpret_cast<const float4 *>(a.theta + j0)));
-                const float4 p1 = perturbed_quad((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                                 __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4)));
-                const float w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
-                octet<X3>(w, hi, lo);
-                if (mirror) {       // the same thread reads exactly these bytes back in the later passes
-                    *reinterpret_cast<uint4 *>(mirror + off) = hi;
-                    if (X3) *reinterpret_cast<uint4 *>(mirror + C::KAT * 8192 + off) = lo;
-                }
-            }
-            put(dst, off, C::KAT * 8192, hi, lo);
-        }
-    };
-
-    // warpgroup wg owns rows [64 wg, 64 wg + 64) of the pass's tile; this thread rows ra and ra + 8 of them
-    const int wg = warp >> 2;
-    const int r_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int cq = (lane & 3) * 2;                                // column pair inside every 8-column block
-
-    // distributed shared memory may only be accessed once every CTA of the cluster is running
+        mbar_init(bar(C::BAR_W1_FULL), kProdThreads * CL);
+        mbar_init(bar(C::BAR_W1_EMPTY), kConsWarps * CL);
+        fit_cnt[0] = fit_cnt[1] = 0u;
+        fence_barrier_init();
+    }
+    // distributed shared memory and the peer's barriers may only be used once every CTA of the cluster runs and has
+    // initialised them
     if (CL == 2) cluster_sync_all();
-    for (int64_t m = first; m < a.n_local; m += stride) {
-        const uint32_t member = (uint32_t)(a.member_offset + (uint64_t)m);
-        // ---- small fp32 arrays (whole, in every CTA): b1 | b2 | W3[8][H] | b3[8]
-        for (int i = tid; i < H / 4; i += kTcThreads) {
-            const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + i), member, gen, kStreamNesEps, a.key,
-                                             a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + i));
-            const float4 v2 = perturbed_quad((uint32_t)((L.off_b2 >> 2) + i), member, gen, kStreamNesEps, a.key,
-                                             a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + i));
-            // the f16x3 epilogue evaluates tanh(v + b) as 1 - 2/(1 + 2^(v*c + b*c)), c = 2 log2 e: store b*c
-            const float bsc = X3 ? kTwoLog2e : 1.0f;
-            reinterpret_cast<float4 *>(small)[i] = make_float4(v1.x * bsc, v1.y * bsc, v1.z * bsc, v1.w * bsc);
-            reinterpret_cast<float4 *>(small + H)[i] = make_float4(v2.x * bsc, v2.y * bsc, v2.z * bsc, v2.w * bsc);
+    else __syncthreads();
+    // one arrival on barrier k of every CTA of the cluster; the release orders this thread's earlier stores before it
+    auto arrive_all = [&](int k) {
+        if (CL == 2) {
+            mbar_arrive_cluster(map_cluster(bar(k), 0u));
+            mbar_arrive_cluster(map_cluster(bar(k), 1u));
+        } else {
+            mbar_arrive(bar(k));
         }
-        for (int i = tid; i < L.A * H / 4; i += kTcThreads)                // W3' [q][n] row-major: aligned quads
-            reinterpret_cast<float4 *>(small + 2 * H)[i] =
-                perturbed_quad((uint32_t)((L.off_w3 >> 2) + i), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                               __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + i));
-        for (int i = L.A * H + tid; i < H * kMaxA; i += kTcThreads) small[2 * H + i] = 0.f;   // unused action rows
-        if (tid < kMaxA) small[2 * H + kMaxA * H + tid] = tid < L.A ? perturbed1(a.theta, L.off_b3 + tid, a.sigma, member, gen, a.key) : 0.f;
-        // ---- W1' (this CTA's half of the rows in a cluster): rows of 128 B, k < d0, zero padded to 32
-        for (int idx = tid; idx < (H / CL) * 4; idx += kTcThreads) {
-            const int n = (int)rank * (H / CL) + (idx >> 2), c8 = idx & 3;
-            float w[8];
-            if ((L.d0 & 3) == 0) {                                        // row starts are quad aligned
-#pragma unroll
-                for (int hq = 0; hq < 2; ++hq) {
-                    const int k = c8 * 8 + hq * 4;
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (k < L.d0) {
-                        const int j = L.off_w1 + n * L.d0 + k;
-                        v = perturbed_quad((uint32_t)(j >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                           __ldg(reinterpret_cast<const float4 *>(a.theta + j)));
+    };
+
+    if (warp < 4 * kProdWGs) {
+        // ================= producer warpgroups: perturbed weights for the consumers, running ahead across members
+        setmaxnreg_dec<prod_regs<H, X3, NA>()>();
+        const int ptid = tid;
+        uint8_t *const cache = (a.cache && a.n_pass > 1) ? a.cache + (size_t)blockIdx.x * C::NCH * C::CHUNK_BYTES : nullptr;
+        // a 16-byte chunk of an operand tile (hi plane at `off`, lo plane `lo_off` further) into this CTA and its peer
+        auto put = [&](uint8_t *base, uint32_t off, uint32_t lo_off, const uint4 &hi, const uint4 &lo) {
+            *reinterpret_cast<uint4 *>(base + off) = hi;
+            if (X3) *reinterpret_cast<uint4 *>(base + lo_off + off) = lo;
+            if (CL == 2) {
+                st_cluster_v4(map_cluster(smem_u32(base + off), rank ^ 1u), hi);
+                if (X3) st_cluster_v4(map_cluster(smem_u32(base + lo_off + off), rank ^ 1u), lo);
+            }
+        };
+        // this CTA's share of W2' chunk c (rows [64c, 64c + 64)) into stage `buf`; pass > 0 copies the cached image back
+        constexpr int kOct = H / 8;                               // octets per row
+        constexpr int kRows = 64 / CL;                            // rows of a chunk generated here
+        auto gen_chunk = [&](uint32_t member, int c, int pass, int buf) {
+            uint8_t *dst = w2buf + buf * C::CHUNK_BYTES;
+            uint8_t *mirror = cache ? cache + (size_t)c * C::CHUNK_BYTES : nullptr;
+            for (int idx = ptid; idx < kRows * kOct; idx += kProdThreads) {
+                const int rr = (int)rank * kRows + idx / kOct, o = idx % kOct;
+                const uint32_t off = (uint32_t)((o >> 3) * 8192 + rr * 128 + (((o & 7) ^ (rr & 7)) << 4));
+                uint4 hi, lo;
+                if (mirror && pass > 0) {
+                    hi = *reinterpret_cast<const uint4 *>(mirror + off);
+                    if (X3) lo = *reinterpret_cast<const uint4 *>(mirror + C::KAT * 8192 + off);
+                    else lo = hi;
+                } else {
+                    const int j0 = L.off_w2 + (c * 64 + rr) * H + o * 8;
+                    const float4 p0 = perturbed_quad((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                                     __ldg(reinterpret_cast<const float4 *>(a.theta + j0)));
+                    const float4 p1 = perturbed_quad((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                                     __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4)));
+                    const float w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+                    octet<X3>(w, hi, lo);
+                    if (mirror) {       // the same thread reads exactly these bytes back in the later passes
+                        *reinterpret_cast<uint4 *>(mirror + off) = hi;
+                        if (X3) *reinterpret_cast<uint4 *>(mirror + C::KAT * 8192 + off) = lo;
                     }
-                    w[4 * hq] = v.x; w[4 * hq + 1] = v.y; w[4 * hq + 2] = v.z; w[4 * hq + 3] = v.w;
                 }
-            } else {
+                put(dst, off, C::KAT * 8192, hi, lo);
+            }
+        };
+
+        uint32_t q = 0;                                           // running W2' chunk counter, as in the consumers
+        int i = 0;
+        for (int64_t m = first; m < a.n_local; m += stride, ++i) {
+            const uint32_t member = (uint32_t)(a.member_offset + (uint64_t)m);
+            // ---- small fp32 arrays (whole, in every CTA) into buffer i & 1: b1 | b2 | W3[8][H] | b3[8]
+            float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
+            if (i >= 2) mbar_wait(bar(C::BAR_SMALL_EMPTY + (i & 1)), ((i >> 1) - 1) & 1);
+            for (int k = ptid; k < H / 4; k += kProdThreads) {
+                const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + k), member, gen, kStreamNesEps, a.key,
+                                                 a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + k));
+                const float4 v2 = perturbed_quad((uint32_t)((L.off_b2 >> 2) + k), member, gen, kStreamNesEps, a.key,
+                                                 a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + k));
+                // the f16x3 epilogue evaluates tanh(v + b) as 1 - 2/(1 + 2^(v*c + b*c)), c = 2 log2 e: store b*c
+                const float bsc = X3 ? kTwoLog2e : 1.0f;
+                reinterpret_cast<float4 *>(small)[k] = make_float4(v1.x * bsc, v1.y * bsc, v1.z * bsc, v1.w * bsc);
+                reinterpret_cast<float4 *>(small + H)[k] = make_float4(v2.x * bsc, v2.y * bsc, v2.z * bsc, v2.w * bsc);
+            }
+            for (int k = ptid; k < L.A * H / 4; k += kProdThreads)             // W3' [q][n] row-major: aligned quads
+                reinterpret_cast<float4 *>(small + 2 * H)[k] =
+                    perturbed_quad((uint32_t)((L.off_w3 >> 2) + k), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                   __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + k));
+            for (int k = L.A * H + ptid; k < H * kMaxA; k += kProdThreads) small[2 * H + k] = 0.f;   // unused action rows
+            if (ptid < kMaxA)
+                small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, a.sigma, member, gen, a.key) : 0.f;
+            // ---- W1' (this CTA's half of the rows in a cluster), once every consumer has run member i-1's layer 1
+            if (i >= 1) mbar_wait_cluster(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
+            for (int idx = ptid; idx < (H / CL) * 4; idx += kProdThreads) {
+                const int n = (int)rank * (H / CL) + (idx >> 2), c8 = idx & 3;
+                float w[8];
+                if ((L.d0 & 3) == 0) {                                        // row starts are quad aligned
 #pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const int k = c8 * 8 + e;
-                    w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, a.sigma, member, gen, a.key) : 0.f;
+                    for (int hq = 0; hq < 2; ++hq) {
+                        const int k = c8 * 8 + hq * 4;
+                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (k < L.d0) {
+                            const int j = L.off_w1 + n * L.d0 + k;
+                            v = perturbed_quad((uint32_t)(j >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
+                                               __ldg(reinterpret_cast<const float4 *>(a.theta + j)));
+                        }
+                        w[4 * hq] = v.x; w[4 * hq + 1] = v.y; w[4 * hq + 2] = v.z; w[4 * hq + 3] = v.w;
+                    }
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                        const int k = c8 * 8 + e;
+                        w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, a.sigma, member, gen, a.key) : 0.f;
+                    }
+                }
+                uint4 hi, lo;
+                octet<X3>(w, hi, lo);
+                put(w1, (uint32_t)(n * 128 + ((c8 ^ (n & 7)) << 4)), H * 128, hi, lo);
+            }
+            fence_proxy_async_cluster();                          // generic-proxy stores -> wgmma operand fetch
+            arrive_all(C::BAR_W1_FULL);                           // publishes the small arrays too
+            // ---- W2' chunks of every pass through the two-stage ring
+            for (int pass = 0; pass < a.n_pass; ++pass) {
+                for (int c = 0; c < C::NCH; ++c, ++q) {
+                    const int s = (int)(q & 1u);
+                    if (q >= 2) mbar_wait_cluster(bar(C::BAR_W2_EMPTY + s), ((q >> 1) - 1) & 1u);
+                    gen_chunk(member, c, pass, s);
+                    fence_proxy_async_cluster();
+                    arrive_all(C::BAR_W2_FULL + s);
                 }
             }
-            uint4 hi, lo;
-            octet<X3>(w, hi, lo);
-            put(w1, (uint32_t)(n * 128 + ((c8 ^ (n & 7)) << 4)), H * 128, hi, lo);
         }
-        gen_chunk(member, 0, 0, 0);
-        fence_proxy_async_cluster();
-        sync_all();
+    } else {
+        // ================= consumer warpgroups cw = 0, 1: rows [64 cw, 64 cw + 64) of the pass's tile
+        setmaxnreg_inc<cons_regs<H, X3, NA>()>();
+        const int cwarp = warp - 4 * kProdWGs, cw = cwarp >> 2;
+        const int r_in_tile = cw * 64 + (cwarp & 3) * 16 + (lane >> 2);   // this thread: rows ra and ra + 8
+        const int cq = (lane & 3) * 2;                            // column pair inside every 8-column block
+        uint32_t q = 0;
+        int i = 0;
+        for (int64_t m = first; m < a.n_local; m += stride, ++i) {
+            const float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
+            const float *b1 = small, *b2 = small + H, *w3 = small + 2 * H, *b3 = small + 2 * H + kMaxA * H;
+            mbar_wait_cluster(bar(C::BAR_W1_FULL), (uint32_t)i & 1u);
 
-        float sq = 0.f;
-        for (int pass = 0; pass < a.n_pass; ++pass) {
-            const int tile = pass * CL + (int)rank;
-            const int ra = tile * 128 + r_in_tile;
-            // ---------------- layer 1: H1 = tanh(X W1'^T + b1), kept as the fp16 A operand of layer 2
-            uint32_t h1h[C::KS2][4], h1l[X3 ? C::KS2 : 1][4];
-            {
-                uint32_t xh[2][4], xl[2][4];
-                load_x<X3>(xh, xl, a.obs, L.d0, ra, lane);
+            float sq = 0.f;
+            for (int pass = 0; pass < a.n_pass; ++pass) {
+                const int tile = pass * CL + (int)rank;
+                const int ra = tile * 128 + r_in_tile;
+                // ---------------- layer 1: H1 = tanh(X W1'^T + b1), kept as the fp16 A operand of layer 2
+                uint32_t h1h[C::KS2][4], h1l[X3 ? C::KS2 : 1][4];
+                {
+                    uint32_t xh[2][4], xl[2][4];
+                    load_x<X3>(xh, xl, a.obs, L.d0, ra, lane);
 #pragma unroll
-                for (int c = 0; c < C::NCH; ++c) {
+                    for (int c = 0; c < C::NCH; ++c) {
+                        float d[32];
+#pragma unroll
+                        for (int k = 0; k < 32; ++k) d[k] = 0.f;
+                        wgmma_fence();
+#pragma unroll
+                        for (int ks = 0; ks < 2; ++ks) {
+                            const uint32_t bh = smem_u32(w1) + c * 8192 + ks * 32;
+                            wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh), ks > 0);
+                            if (X3) {
+                                wgmma_rs_n64(d, xl[ks], smem_desc_sw128(bh), 1);                   // X_lo W_hi
+                                wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh + H * 128), 1);         // X_hi W_lo
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        fence_regs(d);
+                        // the last layer-1 MMA of the member has read W1': the producer may write the next member's
+                        if (c == C::NCH - 1 && pass == a.n_pass - 1 && lane == 0) arrive_all(C::BAR_W1_EMPTY);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const float2 b = *reinterpret_cast<const float2 *>(b1 + c * 64 + j * 8 + cq);
+                            const int s = c * 4 + (j >> 1), e = (j & 1) * 2;
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) {
+                                const float v0 = d[4 * j + 2 * r], v1 = d[4 * j + 2 * r + 1];
+                                if (X3) split_h2(tanh_acc_b(v0, b.x), tanh_acc_b(v1, b.y), h1h[s][e + r], h1l[s][e + r]);
+                                else h1h[s][e + r] = pack_h2(tanh_fast(v0 + b.x), tanh_fast(v1 + b.y));
+                            }
+                        }
+                    }
+                }
+                // ---------------- layer 2 + 3: per 64-feature chunk, H2 = tanh(H1 W2'^T + b2); a += H2 W3'^T
+                float act[NA][2];
+#pragma unroll
+                for (int k = 0; k < NA; ++k) act[k][0] = act[k][1] = 0.f;
+                for (int c = 0; c < C::NCH; ++c, ++q) {
+                    const int st = (int)(q & 1u);
+                    mbar_wait_cluster(bar(C::BAR_W2_FULL + st), (q >> 1) & 1u);
+                    const uint32_t bbase = smem_u32(w2buf + st * C::CHUNK_BYTES);
                     float d[32];
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                    for (int k = 0; k < 32; ++k) d[k] = 0.f;
                     wgmma_fence();
 #pragma unroll
-                    for (int ks = 0; ks < 2; ++ks) {
-                        const uint32_t bh = smem_u32(w1) + c * 8192 + ks * 32;
-                        wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh), ks > 0);
+                    for (int s = 0; s < C::KS2; ++s) {
+                        const uint32_t bh = bbase + (s >> 2) * 8192 + (s & 3) * 32;
+                        wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh), s > 0);
                         if (X3) {
-                            wgmma_rs_n64(d, xl[ks], smem_desc_sw128(bh), 1);                   // X_lo W_hi
-                            wgmma_rs_n64(d, xh[ks], smem_desc_sw128(bh + H * 128), 1);         // X_hi W_lo
+                            wgmma_rs_n64(d, h1l[s], smem_desc_sw128(bh), 1);                          // H1_lo W_hi
+                            wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh + C::KAT * 8192), 1);          // H1_hi W_lo
                         }
                     }
                     wgmma_commit();
                     wgmma_wait<0>();
                     fence_regs(d);
+                    // every MMA of this warp that read the stage has completed: the producer may refill it during the epilogue
+                    if (lane == 0) arrive_all(C::BAR_W2_EMPTY + st);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        const float2 b = *reinterpret_cast<const float2 *>(b1 + c * 64 + j * 8 + cq);
-                        const int s = c * 4 + (j >> 1), e = (j & 1) * 2;
+                        const int n = c * 64 + j * 8 + cq;
+                        const float2 b = *reinterpret_cast<const float2 *>(b2 + n);
 #pragma unroll
                         for (int r = 0; r < 2; ++r) {
-                            const float v0 = d[4 * j + 2 * r], v1 = d[4 * j + 2 * r + 1];
-                            if (X3) split_h2(tanh_acc_b(v0, b.x), tanh_acc_b(v1, b.y), h1h[s][e + r], h1l[s][e + r]);
-                            else h1h[s][e + r] = pack_h2(tanh_fast(v0 + b.x), tanh_fast(v1 + b.y));
-                        }
-                    }
-                }
-            }
-            // ---------------- layer 2 + 3: per 64-feature chunk, H2 = tanh(H1 W2'^T + b2); a += H2 W3'^T
-            float act[NA][2];
+                            float h0, h1;
+                            if (X3) {          // b2 holds b * 2log2(e)
+                                h0 = tanh_acc_b(d[4 * j + 2 * r], b.x);
+                                h1 = tanh_acc_b(d[4 * j + 2 * r + 1], b.y);
+                            } else {
+                                h0 = tanh_fast(d[4 * j + 2 * r] + b.x);
+                                h1 = tanh_fast(d[4 * j + 2 * r + 1] + b.y);
+                            }
+                            // layer 3 (model.py:38) in fp32: W3' row-major [q][n]
 #pragma unroll
-            for (int q = 0; q < NA; ++q) act[q][0] = act[q][1] = 0.f;
-            for (int c = 0; c < C::NCH; ++c) {
-                const int qi = pass * C::NCH + c;
-                const uint32_t bbase = smem_u32(w2buf + (qi & 1) * C::CHUNK_BYTES);
-                float d[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) d[i] = 0.f;
-                wgmma_fence();
-#pragma unroll
-                for (int s = 0; s < C::KS2; ++s) {
-                    const uint32_t bh = bbase + (s >> 2) * 8192 + (s & 3) * 32;
-                    wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh), s > 0);
-                    if (X3) {
-                        wgmma_rs_n64(d, h1l[s], smem_desc_sw128(bh), 1);                          // H1_lo W_hi
-                        wgmma_rs_n64(d, h1h[s], smem_desc_sw128(bh + C::KAT * 8192), 1);          // H1_hi W_lo
-                    }
-                }
-                wgmma_commit();
-                // the next chunk (of this pass or the next) is generated while the tensor cores run this one
-                if (c + 1 < C::NCH) gen_chunk(member, c + 1, pass, (qi + 1) & 1);
-                else if (pass + 1 < a.n_pass) gen_chunk(member, 0, pass + 1, (qi + 1) & 1);
-                wgmma_wait<0>();
-                fence_regs(d);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int n = c * 64 + j * 8 + cq;
-                    const float2 b = *reinterpret_cast<const float2 *>(b2 + n);
-#pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        float h0, h1;
-                        if (X3) {          // b2 holds b * 2log2(e)
-                            h0 = tanh_acc_b(d[4 * j + 2 * r], b.x);
-                            h1 = tanh_acc_b(d[4 * j + 2 * r + 1], b.y);
-                        } else {
-                            h0 = tanh_fast(d[4 * j + 2 * r] + b.x);
-                            h1 = tanh_fast(d[4 * j + 2 * r + 1] + b.y);
-                        }
-                        // layer 3 (model.py:38) in fp32: W3' row-major [q][n]
-#pragma unroll
-                        for (int q = 0; q < NA; ++q) {
-                            if (q < L.A) {
-                                const float2 w = *reinterpret_cast<const float2 *>(w3 + q * H + n);
-                                act[q][r] = __fmaf_rn(h1, w.y, __fmaf_rn(h0, w.x, act[q][r]));
+                            for (int k = 0; k < NA; ++k) {
+                                if (k < L.A) {
+                                    const float2 w = *reinterpret_cast<const float2 *>(w3 + k * H + n);
+                                    act[k][r] = __fmaf_rn(h1, w.y, __fmaf_rn(h0, w.x, act[k][r]));
+                                }
                             }
                         }
                     }
                 }
-                fence_proxy_async_cluster();
-                sync_all();          // the next chunk is in both CTAs; every MMA that read this buffer has completed
-            }
-            // ---- the four lanes of a quad hold the action sums over disjoint columns of the same two rows
+                // ---- the four lanes of a quad hold the action sums over disjoint columns of the same two rows
 #pragma unroll
-            for (int q = 0; q < NA; ++q) {
+                for (int k = 0; k < NA; ++k) {
 #pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    act[q][r] += __shfl_xor_sync(0xffffffffu, act[q][r], 1);
-                    act[q][r] += __shfl_xor_sync(0xffffffffu, act[q][r], 2);
+                    for (int r = 0; r < 2; ++r) {
+                        act[k][r] += __shfl_xor_sync(0xffffffffu, act[k][r], 1);
+                        act[k][r] += __shfl_xor_sync(0xffffffffu, act[k][r], 2);
+                    }
                 }
-            }
-            if ((lane & 3) == 0) {
+                if ((lane & 3) == 0) {
 #pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const int t = ra + 8 * r;
+                    for (int r = 0; r < 2; ++r) {
+                        const int t = ra + 8 * r;
 #pragma unroll
-                    for (int q = 0; q < NA; ++q) {
-                        if (q < L.A) {
-                            float v = act[q][r] + b3[q];
-                            v = clip_keep_nan(v, a.clip);
-                            const float dd = v - __ldg(a.target + (int64_t)t * L.A + q);
-                            sq = __fmaf_rn(dd, dd, sq);
+                        for (int k = 0; k < NA; ++k) {
+                            if (k < L.A) {
+                                float v = act[k][r] + b3[k];
+                                v = clip_keep_nan(v, a.clip);
+                                const float dd = v - __ldg(a.target + (int64_t)t * L.A + k);
+                                sq = __fmaf_rn(dd, dd, sq);
+                            }
                         }
                     }
                 }
             }
-        }
-        // ---- member done: reduce squared error over all rows (fixed order -> deterministic)
+            // ---- member done: reduce squared error over all rows (fixed order -> deterministic)
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-        if (lane == 0) fit_part[warp] = sq;
-        __syncthreads();
-        if (tid == 0) {
-            double f = 0.0;
-            for (int w = 0; w < kTcThreads / 32; ++w) f += (double)fit_part[w];
-            // a cluster adds its two halves into the (pre-zeroed) output: two commutative fp32 adds -> deterministic
-            if (CL == 2) atomicAdd(a.fitness + m, (float)(-f));
-            else a.fitness[m] = (float)(-f);
+            for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+            if (lane == 0) {
+                // the two consumer warpgroups need not be on the same member: partials and counter are double-buffered
+                // by member parity, and the last consumer warp to arrive adds the partials in warp order
+                float *part = fit_part + (i & 1) * kConsWarps;
+                part[cwarp] = sq;
+                __threadfence_block();
+                if (atomicAdd(fit_cnt + (i & 1), 1u) == kConsWarps - 1) {
+                    __threadfence_block();
+                    double f = 0.0;
+                    for (int w = 0; w < kConsWarps; ++w) f += (double)reinterpret_cast<volatile float *>(part)[w];
+                    fit_cnt[i & 1] = 0u;
+                    // a cluster adds its two halves into the (pre-zeroed) output: two commutative fp32 adds -> deterministic
+                    if (CL == 2) atomicAdd(a.fitness + m, (float)(-f));
+                    else a.fitness[m] = (float)(-f);
+                }
+            }
+            // every thread's reads of this member's small arrays (and its fitness bookkeeping) are done
+            mbar_arrive(bar(C::BAR_SMALL_EMPTY + (i & 1)));
         }
     }
     if (CL == 2) cluster_sync_all();          // no CTA leaves while its peer may still write into its shared memory

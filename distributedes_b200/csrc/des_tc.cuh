@@ -39,6 +39,24 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// cluster-scope acquire: also orders the stores a peer CTA released with mbar_arrive_cluster (st.shared::cluster included)
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2, %3;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok) : "r"(bar), "r"(parity), "r"(1000000u) : "memory");
+    return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
+    while (!mbar_try_wait_cluster(bar, parity)) {
+    }
+}
+// one arrival on the mbarrier at cluster address `cbar` (this CTA's or a peer's, from map_cluster), cluster-scope release
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cbar) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cbar) : "memory");
+}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -78,6 +96,12 @@ __device__ __forceinline__ void st_cluster_v4(uint32_t caddr, const uint4 &v) {
     asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(caddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
                  : "memory");
 }
+
+// ---- warp specialisation: per-warpgroup register budgets (every warp of the warpgroup executes it) ----------------
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---- wgmma --------------------------------------------------------------------------------------------
 // K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor):
