@@ -19,18 +19,22 @@
 //              every consumer of the cluster has run the previous member's layer 1, then the W2' chunks of every
 //              pass into the ring.  They run ahead across member boundaries, bounded only by the buffers.
 //   consumers  layer 1, the layer-2 chunks, the epilogues and the fitness reduction; they never generate weights.
-// Every buffer has full / empty mbarriers: full takes one arrival per producer thread of the cluster (after its
-// stores and a fence.proxy.async), empty one per consumer warp of the cluster, right after the wgmma_wait of the
-// MMAs that read it, so a W2' stage is refilled while the consumers run its epilogue.  Stage and phase come from one
-// running chunk counter that both roles advance alike.  The two consumer warpgroups are not kept in step: fitness
-// partials are double-buffered by member parity and the last consumer warp to finish a member adds them in warp order.
+// Every buffer has full / empty mbarriers, and all synchronisation is CTA-scope (no GPU-scope fence, no L1
+// invalidation in the loop).  The producers store into their own CTA only, each runs fence.proxy.async.shared::cta,
+// and they meet on a named barrier; then one thread arrives on the full barrier.  Empty takes one arrival per consumer
+// warp of the cluster, right after the wgmma_wait of the MMAs that read the buffer, so a W2' stage is refilled while
+// the consumers run its epilogue.  Stage and phase come from one running chunk counter that both roles advance alike.
+// The two consumer warpgroups are not kept in step: fitness partials are double-buffered by member parity and the last
+// consumer warp to finish a member adds them in warp order.
 //
 // Clusters: when the tape has an even number of 128-row tiles, two CTAs of a cluster share a member.  Each evaluates
-// its own tiles and generates HALF of every weight tile, storing it into its own and its peer's shared memory
-// (distributed shared memory) and arriving on both CTAs' barriers.  The flagship shape (T = 256) is then one pass per
-// CTA.  Other shapes loop over passes; with the optional workspace the W2' chunks generated in pass 0 are mirrored
-// to global memory (L2-resident) and copied back in the later passes, without it they are regenerated (same bytes
-// either way).
+// its own tiles and generates HALF of every weight tile into its own shared memory; the thread that arrives on its
+// full barrier (arrive.expect_tx for the peer's half) pushes that half to the peer with cp.async.bulk (4 KB per 8 KB
+// atom of a W2' chunk, H/2 rows per W1' plane), which completes on the peer's full barrier.  Consumers release a
+// buffer on both CTAs' empty barriers (a plain remote mbarrier.arrive).  The flagship shape (T = 256) is then one pass
+// per CTA.  Other shapes loop over passes; with the optional workspace the W2' chunks generated in pass 0 are
+// mirrored to global memory (L2-resident) and copied back in the later passes, without it they are regenerated (same
+// bytes either way).
 //
 // Precision modes
 //   F16    operands rounded to fp16 (11 significant bits, as TF32), fp32 accumulate, MUFU tanh.approx.
@@ -60,6 +64,24 @@ __host__ __device__ constexpr uint32_t prod_regs() { return (H == 256 && X3 && N
 template <int H, bool X3, int NA>
 __host__ __device__ constexpr uint32_t cons_regs() { return (((65536u / kTcThreads) & ~7u) * kTcThreads - kProdThreads * prod_regs<H, X3, NA>()) / 256u & ~7u; }
 static_assert(cons_regs<256, true, 4>() == 200 && cons_regs<256, true, 8>() == 216, "register split");
+
+// Phase trace (build with -DDES_EVAL_TRACE, scripts/trace_eval.py): every thread charges the clock64() time since its
+// previous mark to the phase it has just finished; lane 0 of every warp of CTAs 0 and 1 prints its totals at the end.
+// Without the macro the marks compile to nothing.
+#ifdef DES_EVAL_TRACE
+enum { TR_WAIT, TR_MMA, TR_SYNC, TR_EPI, TR_GEN, TR_OTHER, TR_N };
+#define DES_TRACE_INIT uint32_t tr_[TR_N] = {}; long long tr_t = clock64(), tr_0 = tr_t;
+#define DES_TRACE(k) do { const long long t_ = clock64(); tr_[k] += (uint32_t)(t_ - tr_t); tr_t = t_; } while (0)
+#define DES_TRACE_PRINT(role, members)                                                                                \
+    if (blockIdx.x < 2 && lane == 0)                                                                                  \
+        printf("DES_TRACE cta=%d warp=%d role=%s members=%d wait=%u mma=%u sync=%u epi=%u gen=%u other=%u total=%u\n", \
+               (int)blockIdx.x, warp, role, members, tr_[TR_WAIT], tr_[TR_MMA], tr_[TR_SYNC], tr_[TR_EPI], tr_[TR_GEN],  \
+               tr_[TR_OTHER], (uint32_t)(clock64() - tr_0))
+#else
+#define DES_TRACE_INIT
+#define DES_TRACE(k)
+#define DES_TRACE_PRINT(role, members)
+#endif
 
 template <int H, bool X3>
 struct TcCfg {
@@ -154,45 +176,69 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
     const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
     const int64_t first = blockIdx.x / CL, stride = gridDim.x / CL;
 
-    // full: one arrival per producer thread of the cluster (each stores into both CTAs); empty: one per consumer warp
-    // of the cluster (each reads its own CTA's copy, which both producers write); small arrays are per CTA
+    // A CTA's half of a weight tile in a cluster: rows [32 rank, 32 rank + 32) of every 8 KB atom of a W2' chunk, rows
+    // [H/2 rank, H/2 rank + H/2) of each W1' plane.  Its producers store it locally; one thread then pushes it to the
+    // peer with one bulk copy per atom (per plane for W1'), which completes on the peer's full barrier.
+    constexpr uint32_t kW2Copy = (64 / CL) * 128, kW2Copies = C::PLANES * C::KAT;
+    constexpr uint32_t kW1Copy = (H / CL) * 128, kW1Copies = C::PLANES;
+    static_assert(CL * kW2Copies * kW2Copy == C::CHUNK_BYTES && CL * kW1Copies * kW1Copy == C::W1_BYTES,
+                  "the two halves must make up the whole tile, or a full barrier never completes");
+    static_assert(kW2Copy % 16 == 0 && kW1Copy % 16 == 0, "bulk copies move multiples of 16 bytes");
+    static_assert(kW2Copies * kW2Copy < (1u << 20) && kW1Copies * kW1Copy < (1u << 20), "mbarrier tx-count range");
+
+    // full: one arrival, by the elected producer thread after its CTA's producers have stored their half, plus in a
+    // cluster the bytes of the peer's half (complete_tx of its bulk copies); empty: one arrival per consumer warp of the
+    // cluster (each reads its own CTA's copy, which both producers fill); small arrays are per CTA
     if (tid == 0) {
         for (int s = 0; s < 2; ++s) {
-            mbar_init(bar(C::BAR_W2_FULL + s), kProdThreads * CL);
+            mbar_init(bar(C::BAR_W2_FULL + s), 1);
             mbar_init(bar(C::BAR_W2_EMPTY + s), kConsWarps * CL);
             mbar_init(bar(C::BAR_SMALL_EMPTY + s), kTcThreads - kProdThreads);
         }
-        mbar_init(bar(C::BAR_W1_FULL), kProdThreads * CL);
+        mbar_init(bar(C::BAR_W1_FULL), 1);
         mbar_init(bar(C::BAR_W1_EMPTY), kConsWarps * CL);
         fit_cnt[0] = fit_cnt[1] = 0u;
         fence_barrier_init();
     }
     // distributed shared memory and the peer's barriers may only be used once every CTA of the cluster runs and has
-    // initialised them
-    if (CL == 2) cluster_sync_all();
-    else __syncthreads();
-    // one arrival on barrier k of every CTA of the cluster; the release orders this thread's earlier stores before it
-    auto arrive_all = [&](int k) {
-        if (CL == 2) {
-            mbar_arrive_cluster(map_cluster(bar(k), 0u));
-            mbar_arrive_cluster(map_cluster(bar(k), 1u));
-        } else {
-            mbar_arrive(bar(k));
-        }
+    // initialised them (fence_barrier_init publishes the initialisation); the CTA barrier orders fit_cnt
+    if (CL == 2) cluster_sync_relaxed();
+    __syncthreads();
+    // consumers: one arrival on empty barrier k of every CTA of the cluster, once this warp's MMAs have read the buffer
+    const uint32_t peer_bars = CL == 2 ? map_cluster(bars, rank ^ 1u) : 0u;
+    auto release_all = [&](int k) {
+        mbar_arrive(bar(k));
+        if (CL == 2) mbar_arrive_remote(peer_bars + 8u * (uint32_t)k);
     };
 
     if (warp < 4 * kProdWGs) {
         // ================= producer warpgroups: perturbed weights for the consumers, running ahead across members
         setmaxnreg_dec<prod_regs<H, X3, NA>()>();
+        DES_TRACE_INIT
         const int ptid = tid;
         uint8_t *const cache = (a.cache && a.n_pass > 1) ? a.cache + (size_t)blockIdx.x * C::NCH * C::CHUNK_BYTES : nullptr;
-        // a 16-byte chunk of an operand tile (hi plane at `off`, lo plane `lo_off` further) into this CTA and its peer
+        // a 16-byte chunk of an operand tile (hi plane at `off`, lo plane `lo_off` further) into this CTA
         auto put = [&](uint8_t *base, uint32_t off, uint32_t lo_off, const uint4 &hi, const uint4 &lo) {
             *reinterpret_cast<uint4 *>(base + off) = hi;
             if (X3) *reinterpret_cast<uint4 *>(base + lo_off + off) = lo;
-            if (CL == 2) {
-                st_cluster_v4(map_cluster(smem_u32(base + off), rank ^ 1u), hi);
-                if (X3) st_cluster_v4(map_cluster(smem_u32(base + lo_off + off), rank ^ 1u), lo);
+        };
+        // this CTA's half of a tile at `base` is stored (ncopy pieces of `bytes`, `step` apart, this CTA's at
+        // + rank * bytes): make it visible to wgmma and the bulk copy, then one thread arrives on the local full barrier
+        // k, expecting the peer's half, and pushes this CTA's half into the peer, completing on the peer's barrier k
+        auto publish = [&](int k, uint32_t base, uint32_t bytes, uint32_t ncopy, uint32_t step) {
+            fence_proxy_async_cta();
+            named_bar_sync(1, kProdThreads);
+            if (ptid == 0) {
+                if (CL == 2) {
+                    mbar_expect_tx(bar(k), ncopy * bytes);
+                    const uint32_t peer_bar = map_cluster(bar(k), rank ^ 1u);
+                    for (uint32_t j = 0; j < ncopy; ++j) {
+                        const uint32_t src = base + j * step + rank * bytes;
+                        bulk_copy_to_peer(map_cluster(src, rank ^ 1u), src, bytes, peer_bar);
+                    }
+                } else {
+                    mbar_arrive(bar(k));
+                }
             }
         };
         // this CTA's share of W2' chunk c (rows [64c, 64c + 64)) into stage `buf`; pass > 0 copies the cached image back
@@ -233,6 +279,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
             // ---- small fp32 arrays (whole, in every CTA) into buffer i & 1: b1 | b2 | W3[8][H] | b3[8]
             float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
             if (i >= 2) mbar_wait(bar(C::BAR_SMALL_EMPTY + (i & 1)), ((i >> 1) - 1) & 1);
+            DES_TRACE(TR_WAIT);
             for (int k = ptid; k < H / 4; k += kProdThreads) {
                 const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + k), member, gen, kStreamNesEps, a.key,
                                                  a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + k));
@@ -251,7 +298,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
             if (ptid < kMaxA)
                 small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, a.sigma, member, gen, a.key) : 0.f;
             // ---- W1' (this CTA's half of the rows in a cluster), once every consumer has run member i-1's layer 1
-            if (i >= 1) mbar_wait_cluster(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
+            DES_TRACE(TR_GEN);
+            if (i >= 1) mbar_wait(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
+            DES_TRACE(TR_WAIT);
             for (int idx = ptid; idx < (H / CL) * 4; idx += kProdThreads) {
                 const int n = (int)rank * (H / CL) + (idx >> 2), c8 = idx & 3;
                 float w[8];
@@ -278,22 +327,34 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                 octet<X3>(w, hi, lo);
                 put(w1, (uint32_t)(n * 128 + ((c8 ^ (n & 7)) << 4)), H * 128, hi, lo);
             }
-            fence_proxy_async_cluster();                          // generic-proxy stores -> wgmma operand fetch
-            arrive_all(C::BAR_W1_FULL);                           // publishes the small arrays too
+            DES_TRACE(TR_GEN);
+            publish(C::BAR_W1_FULL, smem_u32(w1), kW1Copy, kW1Copies, H * 128);   // and the small arrays
+            DES_TRACE(TR_SYNC);
             // ---- W2' chunks of every pass through the two-stage ring
             for (int pass = 0; pass < a.n_pass; ++pass) {
                 for (int c = 0; c < C::NCH; ++c, ++q) {
                     const int s = (int)(q & 1u);
-                    if (q >= 2) mbar_wait_cluster(bar(C::BAR_W2_EMPTY + s), ((q >> 1) - 1) & 1u);
+                    if (q >= 2) mbar_wait(bar(C::BAR_W2_EMPTY + s), ((q >> 1) - 1) & 1u);
+                    DES_TRACE(TR_WAIT);
                     gen_chunk(member, c, pass, s);
-                    fence_proxy_async_cluster();
-                    arrive_all(C::BAR_W2_FULL + s);
+                    DES_TRACE(TR_GEN);
+                    publish(C::BAR_W2_FULL + s, smem_u32(w2buf + s * C::CHUNK_BYTES), kW2Copy, kW2Copies, 8192);
+                    DES_TRACE(TR_SYNC);
                 }
             }
         }
+        // A CTA leaves only when its peer can no longer arrive on its barriers or copy into its shared memory: once
+        // every consumer warp of the cluster has released W1' and the last two W2' stages.  Those releases follow the
+        // consumers' full waits, so every bulk copy of either CTA has landed too.
+        if (CL == 2) {
+            for (uint32_t t = q > 2u ? q - 2u : 0u; t < q; ++t) mbar_wait(bar(C::BAR_W2_EMPTY + (int)(t & 1u)), (t >> 1) & 1u);
+            if (i >= 1) mbar_wait(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
+        }
+        DES_TRACE_PRINT("producer", i);
     } else {
         // ================= consumer warpgroups cw = 0, 1: rows [64 cw, 64 cw + 64) of the pass's tile
         setmaxnreg_inc<cons_regs<H, X3, NA>()>();
+        DES_TRACE_INIT
         const int cwarp = warp - 4 * kProdWGs, cw = cwarp >> 2;
         const int r_in_tile = cw * 64 + (cwarp & 3) * 16 + (lane >> 2);   // this thread: rows ra and ra + 8
         const int cq = (lane & 3) * 2;                            // column pair inside every 8-column block
@@ -302,7 +363,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
         for (int64_t m = first; m < a.n_local; m += stride, ++i) {
             const float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
             const float *b1 = small, *b2 = small + H, *w3 = small + 2 * H, *b3 = small + 2 * H + kMaxA * H;
-            mbar_wait_cluster(bar(C::BAR_W1_FULL), (uint32_t)i & 1u);
+            mbar_wait(bar(C::BAR_W1_FULL), (uint32_t)i & 1u);
+            DES_TRACE(TR_WAIT);
 
             float sq = 0.f;
             for (int pass = 0; pass < a.n_pass; ++pass) {
@@ -313,6 +375,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                 {
                     uint32_t xh[2][4], xl[2][4];
                     load_x<X3>(xh, xl, a.obs, L.d0, ra, lane);
+                    DES_TRACE(TR_OTHER);
 #pragma unroll
                     for (int c = 0; c < C::NCH; ++c) {
                         float d[32];
@@ -331,8 +394,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                         wgmma_commit();
                         wgmma_wait<0>();
                         fence_regs(d);
+                        DES_TRACE(TR_MMA);
                         // the last layer-1 MMA of the member has read W1': the producer may write the next member's
-                        if (c == C::NCH - 1 && pass == a.n_pass - 1 && lane == 0) arrive_all(C::BAR_W1_EMPTY);
+                        if (c == C::NCH - 1 && pass == a.n_pass - 1 && lane == 0) release_all(C::BAR_W1_EMPTY);
+                        DES_TRACE(TR_SYNC);
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float2 b = *reinterpret_cast<const float2 *>(b1 + c * 64 + j * 8 + cq);
@@ -344,6 +409,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                                 else h1h[s][e + r] = pack_h2(tanh_fast(v0 + b.x), tanh_fast(v1 + b.y));
                             }
                         }
+                        DES_TRACE(TR_EPI);
                     }
                 }
                 // ---------------- layer 2 + 3: per 64-feature chunk, H2 = tanh(H1 W2'^T + b2); a += H2 W3'^T
@@ -352,7 +418,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                 for (int k = 0; k < NA; ++k) act[k][0] = act[k][1] = 0.f;
                 for (int c = 0; c < C::NCH; ++c, ++q) {
                     const int st = (int)(q & 1u);
-                    mbar_wait_cluster(bar(C::BAR_W2_FULL + st), (q >> 1) & 1u);
+                    mbar_wait(bar(C::BAR_W2_FULL + st), (q >> 1) & 1u);
+                    DES_TRACE(TR_WAIT);
                     const uint32_t bbase = smem_u32(w2buf + st * C::CHUNK_BYTES);
                     float d[32];
 #pragma unroll
@@ -370,8 +437,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                     wgmma_commit();
                     wgmma_wait<0>();
                     fence_regs(d);
+                    DES_TRACE(TR_MMA);
                     // every MMA of this warp that read the stage has completed: the producer may refill it during the epilogue
-                    if (lane == 0) arrive_all(C::BAR_W2_EMPTY + st);
+                    if (lane == 0) release_all(C::BAR_W2_EMPTY + st);
+                    DES_TRACE(TR_SYNC);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         const int n = c * 64 + j * 8 + cq;
@@ -396,6 +465,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                             }
                         }
                     }
+                    DES_TRACE(TR_EPI);
                 }
                 // ---- the four lanes of a quad hold the action sums over disjoint columns of the same two rows
 #pragma unroll
@@ -443,9 +513,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
             }
             // every thread's reads of this member's small arrays (and its fitness bookkeeping) are done
             mbar_arrive(bar(C::BAR_SMALL_EMPTY + (i & 1)));
+            DES_TRACE(TR_OTHER);
         }
+        DES_TRACE_PRINT("consumer", i);
     }
-    if (CL == 2) cluster_sync_all();          // no CTA leaves while its peer may still write into its shared memory
 }
 
 template <int H, bool X3, int CL, int NA>

@@ -39,29 +39,20 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// cluster-scope acquire: also orders the stores a peer CTA released with mbar_arrive_cluster (st.shared::cluster included)
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar), "r"(parity), "r"(1000000u) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-    while (!mbar_try_wait_cluster(bar, parity)) {
-    }
-}
-// one arrival on the mbarrier at cluster address `cbar` (this CTA's or a peer's, from map_cluster), cluster-scope release
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cbar) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cbar) : "memory");
+// one arrival on the mbarrier at cluster address `cbar` (a peer CTA's, from map_cluster), default semantics: a consumer
+// whose reads of a buffer have completed releases it to the peer's producer (no cluster-scope fence)
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cbar) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cbar) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// generic-proxy writes (st.shared, st.shared::cluster) -> visible to the async proxy (wgmma operand fetch)
-__device__ __forceinline__ void fence_proxy_async_cluster() { asm volatile("fence.proxy.async.shared::cluster;" ::: "memory"); }
+// generic-proxy writes to this CTA's shared memory -> visible to the async proxy (wgmma operand fetch, bulk copies)
+__device__ __forceinline__ void fence_proxy_async_cta() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier `id` over the first `n` threads of the CTA (whole warps)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
 
 // ---- TMA ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void *map, int c0, int c1, uint32_t bar) {
@@ -83,8 +74,10 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// every CTA of the cluster has arrived (so runs), without ordering memory: a preceding fence.mbarrier_init publishes
+// mbarrier initialisation to the peers (no GPU-scope fence, unlike the .release arrive)
+__device__ __forceinline__ void cluster_sync_relaxed() {
+    asm volatile("barrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
 }
 // address of the same shared-memory offset in CTA `rank` of the cluster
 __device__ __forceinline__ uint32_t map_cluster(uint32_t saddr, uint32_t rank) {
@@ -92,9 +85,11 @@ __device__ __forceinline__ uint32_t map_cluster(uint32_t saddr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(saddr), "r"(rank));
     return ra;
 }
-__device__ __forceinline__ void st_cluster_v4(uint32_t caddr, const uint4 &v) {
-    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(caddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-                 : "memory");
+// bulk copy of `bytes` (a multiple of 16) from this CTA's shared memory at `src` to cluster address `cdst` (a peer's
+// shared memory); completes `bytes` of transaction count on the mbarrier at cluster address `cbar` in the same CTA as cdst
+__device__ __forceinline__ void bulk_copy_to_peer(uint32_t cdst, uint32_t src, uint32_t bytes, uint32_t cbar) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(cdst), "r"(src), "r"(bytes), "r"(cbar) : "memory");
 }
 
 // ---- warp specialisation: per-warpgroup register budgets (every warp of the warpgroup executes it) ----------------
