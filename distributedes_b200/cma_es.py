@@ -2,7 +2,8 @@
 reference takes from the third-party `cma` package (cma.CMAEvolutionStrategy, cma_es.py:49: ask() :62, tell() :90).
 
 The hot arithmetic — the rank-mu covariance update inside tell() — is des_cma_rank_mu + des_cma_cov_apply
-(csrc/des_cma.cu); solutions are evaluated by des_pop_eval and rank-shaped by des_centered_rank.  The small
+(csrc/des_cma.cu); solutions are evaluated by des_pop_eval on the tape, or rolled out in the environment on the device by
+des_rollout_eval_solutions (closed-loop configs), and rank-shaped by des_centered_rank.  The small
 O(n)/O(n^2) bookkeeping around it (mean, evolution paths, step size) and the library calls a CMA step needs
 (the [lambda,n]x[n,n] sampling GEMM and the symmetric eigendecomposition) go through torch (cuBLAS / cuSOLVER):
 plumbing, not kernels of this repo.  Equations: Hansen's tutorial arXiv:1604.00772 (cited at README.md:16);
@@ -172,27 +173,95 @@ class CMAEvolutionStrategy:
 
 
 class Worker:
-    """cma_es.py:13-29 re-cast: evaluates a batch of shipped solutions on one GPU (des_pop_eval)."""
+    """cma_es.py:13-29 re-cast: evaluates the solutions of this rank's shard on one GPU.
 
-    def __init__(self, id, state_normalizer, task_q, result_q, stop, config, device=None):
+    Tape configs score them with des_pop_eval.  Closed-loop configs (`config.closed_loop`) roll every solution out in the
+    environment on the device with des_rollout_eval_solutions, `config.repetitions` episodes each, and keep what the
+    reference's workers share with the master (cma_es.py:35-38): the normaliser statistics [m | v | n] on the device and
+    the fp64 (sum, sum of squares, count) of the raw observations of the last evaluation, as engine.RolloutEngine does.
+
+    `kernels` (default: distributedes_b200.ops) and `device` exist so the sharded host logic can run under gloo on CPU
+    with an oracle-backed stand-in, as in CMAEvolutionStrategy."""
+
+    def __init__(self, id, state_normalizer, task_q, result_q, stop, config, device=None, kernels=None):
         self.id, self.config = id, config
-        self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
-        env = config.env_fn()
-        self.T = env.tape_len
-        self.obs = torch.from_numpy(env.obs).to(self.device)
-        self.target = torch.from_numpy(env.target).to(self.device)
+        if kernels is None:
+            self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
+            kernels = ops
+        else:
+            self.device = torch.device(device if device is not None else 'cpu')
+        self.kn = kernels
+        self.closed_loop = bool(getattr(config, 'closed_loop', False))
+        if self.closed_loop:
+            from .engine import RolloutEngine
+            if config.task not in RolloutEngine.ENVS:
+                raise ValueError('closed-loop environments available on the device: %s (got %r)'
+                                 % (sorted(RolloutEngine.ENVS), config.task))
+            spec = RolloutEngine.ENVS[config.task]
+            self.env_id, self.T, self.d0 = spec['env'], int(spec['horizon']), int(spec['state_dim'])
+            self.normalize_obs = bool(getattr(config, 'normalize_obs', True))
+            self.obs_stats = (torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device)
+                              if self.normalize_obs else None)
+            self.obs_totals = torch.zeros(2 * self.d0 + 1, dtype=torch.float64, device=self.device)
+            self.roll_ws = None
+            self.tests_run = 0            # test() calls so far: the generation word of the next test episodes
+        else:
+            env = config.env_fn()
+            self.T = env.tape_len
+            self.obs = torch.from_numpy(env.obs).to(self.device)
+            self.target = torch.from_numpy(env.target).to(self.device)
 
-    def run(self, solutions):
-        """fitness (= cost, cma_es.py:28: Evaluator.eval returns -mean return) of every solution."""
-        fit = ops.pop_eval(solutions, self.obs, self.target, hidden=self.config.hidden_size, clip=self.config.clip)
+    def run(self, solutions, member_offset=0, generation=0):
+        """cost (cma_es.py:28: Evaluator.eval returns -mean return) of every solution; row i is global member
+        member_offset + i of generation `generation` (closed loop: its reset states)."""
+        if not self.closed_loop:
+            fit = self.kn.pop_eval(solutions, self.obs, self.target, hidden=self.config.hidden_size, clip=self.config.clip)
+            return -fit
+        c = self.config
+        n_local = int(solutions.shape[0])
+        self.obs_totals.zero_()
+        fit = torch.zeros(n_local, dtype=torch.float32, device=self.device)
+        if n_local:
+            w = 2 * self.d0 + 1
+            if self.roll_ws is None or self.roll_ws.numel() < n_local * w:
+                self.roll_ws = torch.empty(n_local * w, dtype=torch.float64, device=self.device)
+            self.kn.rollout_eval_solutions(solutions, env=self.env_id, hidden=c.hidden_size, horizon=self.T,
+                                           repetitions=c.repetitions, clip=c.clip, action_noise_std=c.action_noise_std,
+                                           seed=getattr(c, 'seed', 0), generation=generation, member_offset=member_offset,
+                                           obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                                           workspace=self.roll_ws, out=fit)
         return -fit
 
+    def test_returns(self, solution, repetitions):
+        """Returns of `repetitions` noiseless episodes of one solution (cma_es.py:102-111) with the current statistics.
+        The k-th call (k = 0 first) resets its episodes from the test stream with generation word k."""
+        c = self.config
+        sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
+        episodes = torch.empty(int(repetitions), dtype=torch.float32, device=self.device)
+        self.kn.rollout_eval(sol, env=self.env_id, hidden=c.hidden_size, horizon=self.T, repetitions=int(repetitions),
+                             sigma=0.0, clip=c.clip, action_noise_std=c.action_noise_std, seed=getattr(c, 'seed', 0),
+                             generation=self.tests_run, member_offset=0, n_local=1, noiseless=True,
+                             obs_stats=self.obs_stats, episodes_out=episodes)
+        self.tests_run += 1
+        return episodes.cpu().numpy().astype(np.float64)
 
-def train(config):
-    """cma_es.py:31-100.  Returns [training_rewards, training_steps, training_timestamps]."""
-    worker = Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
-    es = CMAEvolutionStrategy(config.initial_weight, config.sigma, config.pop_size, seed=getattr(config, 'seed', 0),
-                              device=worker.device)
+    def merge_obs_stats(self, es):
+        """cma_es.py:92-96: the statistics of this generation's observations, summed over ranks, merged into [m|v|n]."""
+        if not (self.closed_loop and self.normalize_obs):
+            return
+        if es.world > 1:
+            dist.all_reduce(self.obs_totals, group=es.pg)
+        self.kn.obs_stats_merge_totals(self.obs_stats, self.obs_totals, self.d0)
+
+
+def train(config, worker=None, es=None):
+    """cma_es.py:31-100.  Returns [training_rewards, training_steps, training_timestamps].  `worker` / `es` default to a
+    Worker and a CMAEvolutionStrategy on the current GPU; pass them to choose the device or the kernels."""
+    if worker is None:
+        worker = Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
+    if es is None:
+        es = CMAEvolutionStrategy(config.initial_weight, config.sigma, config.pop_size, seed=getattr(config, 'seed', 0),
+                                  device=worker.device, kernels=None if worker.kn is ops else worker.kn)
     total_steps = 0
     initial_time = time.time()
     training_rewards, training_steps, training_timestamps = [], [], []
@@ -204,7 +273,7 @@ def train(config):
     generation = 0
     while True:
         solutions = es.ask()                                                                # :62 (this rank's shard)
-        cost = es.gather_cost(worker.run(solutions))                                        # :63-72, all lambda costs
+        cost = es.gather_cost(worker.run(solutions, es.offset, es.gen))                     # :63-72, all lambda costs
         total_steps += config.pop_size * config.repetitions * worker.T                      # :73
         best = int(torch.argmin(cost))                                                      # :75
         elapsed_time = time.time() - initial_time
@@ -221,8 +290,10 @@ def train(config):
             break
         if getattr(config, 'max_generations', 0) and generation >= config.max_generations:
             break
-        shaped = ops.centered_rank(cost.to(torch.float32).contiguous())                     # :89 fitness_shift(cost)
+        cost32 = cost.to(torch.float32).contiguous()
+        shaped = worker.kn.centered_rank(cost32, 0, es.lam, out=torch.empty_like(cost32))   # :89 fitness_shift(cost)
         es.tell(solutions, shaped)                                                          # :90
+        worker.merge_obs_stats(es)                                                          # :92-96
     return [training_rewards, training_steps, training_timestamps]
 
 
@@ -238,9 +309,15 @@ def _fetch_member(es, solutions_local, index):
 
 
 def test(config, solution, stats, worker=None):
-    """cma_es.py:102-111 (which divides the std by config.repetitions, not test_repetitions)."""
+    """cma_es.py:102-111 (which divides the std by config.repetitions, not test_repetitions).  Closed loop: the mean of
+    `test_repetitions` episodes with the worker's current statistics (`stats`, if given, replaces them first)."""
     worker = worker if worker is not None else Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
     sol = torch.as_tensor(np.asarray(solution.detach().cpu() if isinstance(solution, torch.Tensor) else solution,
                                      dtype=np.float32)).reshape(1, -1).to(worker.device)
-    rewards = [float(-worker.run(sol)[0]) for _ in range(config.test_repetitions)]
+    if worker.closed_loop:
+        if stats is not None and worker.obs_stats is not None:
+            worker.obs_stats.copy_(torch.as_tensor(np.asarray(stats, dtype=np.float32)))
+        rewards = worker.test_returns(sol, config.test_repetitions)
+    else:
+        rewards = [float(-worker.run(sol)[0]) for _ in range(config.test_repetitions)]
     return np.mean(rewards), np.std(rewards) / config.repetitions

@@ -62,10 +62,10 @@ class ClosedLoopPendulumConfig(BasicConfig):
     200-step episodes per member (config.py:8-9), per-member observations, observation normaliser on."""
 
     def __init__(self, hidden_size=64):
-        # limits of des_rollout_eval (csrc/des_envs.cu): checked here, not at the first generation.  The reference's own
-        # default hidden_size=16 (config.py:27) is below the kernel's 32-unit granularity.
-        if hidden_size % 32 != 0 or not (32 <= hidden_size <= 128):
-            raise ValueError('ClosedLoopPendulumConfig: hidden_size must be 32, 64, 96 or 128 on the device path (got %r)'
+        # limits of des_rollout_eval (csrc/des_envs.cu): checked here, not at the first generation.  16 is the reference's
+        # own PendulumConfig default (config.py:27) and the width its CMA-ES driver uses (cma_es.py:129).
+        if hidden_size not in (16, 32, 64, 96, 128):
+            raise ValueError('ClosedLoopPendulumConfig: hidden_size must be 16, 32, 64, 96 or 128 on the device path (got %r)'
                              % (hidden_size,))
         self.task = 'Pendulum-v0'
         self.clip = 2.0

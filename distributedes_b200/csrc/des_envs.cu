@@ -4,15 +4,17 @@
 // obs 3, action 1, clip +-2, 200-step episodes).
 //
 // One warp per member steps all of the member's episodes in lockstep (see rollout_pendulum_kernel); the member's
-// perturbed weights theta + sigma*eps are generated once into shared memory with the same counter noise as every other
-// kernel.  Policy arithmetic fp32 (FFMA, MUFU-based tanh), dynamics fp64 (gym keeps its state in float64).
+// weights go once into shared memory: theta + sigma*eps generated with the same counter noise as every other kernel
+// (NES), or row i of an explicit solutions[n_local][P] matrix (des_rollout_eval_solutions: the solutions CMA-ES's ask()
+// returns, cma_es.py:22-29).  Everything after the weights are staged is the same code in both modes.
+// Policy arithmetic fp32 (FFMA, MUFU-based tanh), dynamics fp64 (gym keeps its state in float64).
 // Algorithmic work per environment step: 2*(3H + H*H + H) flop; no HBM traffic beyond theta (L2 resident).
 #include "des_common.cuh"
 
 namespace des {
 
 constexpr int kEnvPendulum = 0;
-constexpr int kMaxRollH = 128;         // hidden units (4 per lane)
+constexpr int kMaxRollH = 128;         // hidden units (R = H/16 per lane, up to 8)
 constexpr uint32_t kStreamEnvReset = 2u;
 constexpr uint32_t kStreamActNoise = 3u;
 
@@ -20,7 +22,8 @@ struct RollArgs {
     float *fitness;                    // [n_local] mean return over the repetitions (higher is better)
     float *ep_ret;                     // optional [n_local][reps] per-episode returns
     double *stat_part;                 // optional [n_local][2*d0+1]: per-member sum, sum of squares, count of RAW observations
-    const float *theta;
+    const float *theta;                // NES mode: the member's weights are theta + sigma*eps
+    const float *rows;                 // explicit mode: [n_local][P] row-major, the member's weights are row blockIdx.x
     const float *obs_stats;            // optional [m | v | n] (StaticNormalizer offline stats), NULL = identity
     const des_state *state;
     Layout L;
@@ -80,9 +83,10 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // R = H/16 hidden units rg*R.. and the episodes 5*eg..5*eg+4 — an R x 5 register tile fed per k by one LDS of R
 // transposed weights and one 5-float broadcast of h1.  The fp64 dynamics of episode 5*eg + rg%5 run in every lane
 // (the copies in rg >= 5 are redundant), i.e. once per step for the whole member.
-template <int HPL>   // H = 32*HPL
+// kRows: the weights are row blockIdx.x of a.rows (no noise is generated); otherwise theta + sigma*eps of the member.
+template <int R, bool kRows>   // H = 16*R
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
-    constexpr int H = 32 * HPL, R = 2 * HPL, C = kEpPerLane;
+    constexpr int H = 16 * R, C = kEpPerLane;
     extern __shared__ __align__(16) float sm[];
     float *W2T = sm;                     // [k][j] = W2[j][k]
     // h1 panels, one per episode half, rows in the permuted order p(k) = (k % R)*16 + k/R so that the 16 unit groups
@@ -100,22 +104,31 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
     const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
     const uint32_t member = (uint32_t)(a.member_offset + blockIdx.x);
 
-    // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30)
-    for (int q = lane; q < (L.P + 3) / 4; q += 32) {
-        float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (!a.noiseless) z = noise_quad((uint32_t)q, member, gen, kStreamNesEps, a.key);
-        const float zz[4] = {z.x, z.y, z.z, z.w};
+    // flat parameter j of the member -> its place in shared memory
+    auto stage = [&](int j, float w) {
+        if (j < L.off_b1) W1s[(j / 3) * 4 + (j % 3)] = w;
+        else if (j < L.off_w2) b1s[j - L.off_b1] = w;
+        else if (j < L.off_b2) { const int r = (j - L.off_w2) / H; const int k = j - L.off_w2 - r * H; W2T[((k % R) * 16 + k / R) * H + r] = w; }
+        else if (j < L.off_w3) b2s[j - L.off_b2] = w;
+        else if (j < L.off_b3) W3s[j - L.off_w3] = w;
+        else b3s[0] = w;
+    };
+    if constexpr (kRows) {
+        // ---- explicit solution row (cma_es.py:27-28).  P is odd, so rows are not 16-byte aligned: coalesced scalar loads
+        const float *row = a.rows + (int64_t)blockIdx.x * L.P;
+        for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
+    } else {
+        // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30)
+        for (int q = lane; q < (L.P + 3) / 4; q += 32) {
+            float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (!a.noiseless) z = noise_quad((uint32_t)q, member, gen, kStreamNesEps, a.key);
+            const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int j = 4 * q + e;
-            if (j >= L.P) break;
-            const float w = __fmaf_rn(a.sigma, zz[e], __ldg(a.theta + j));
-            if (j < L.off_b1) W1s[(j / 3) * 4 + (j % 3)] = w;
-            else if (j < L.off_w2) b1s[j - L.off_b1] = w;
-            else if (j < L.off_b2) { const int r = (j - L.off_w2) / H; const int k = j - L.off_w2 - r * H; W2T[((k % R) * 16 + k / R) * H + r] = w; }
-            else if (j < L.off_w3) b2s[j - L.off_b2] = w;
-            else if (j < L.off_b3) W3s[j - L.off_w3] = w;
-            else b3s[0] = w;
+            for (int e = 0; e < 4; ++e) {
+                const int j = 4 * q + e;
+                if (j >= L.P) break;
+                stage(j, __fmaf_rn(a.sigma, zz[e], __ldg(a.theta + j)));
+            }
         }
     }
     __syncwarp();
@@ -177,18 +190,21 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
 #pragma unroll 16
         for (int k = 0; k < H; ++k) {
             float w[R];
+            static_assert(R == 1 || R % 2 == 0, "W2T row loads cover R units: float4, float2 or one float");
             if constexpr (R % 4 == 0) {
 #pragma unroll
                 for (int r4 = 0; r4 < R / 4; ++r4) {
                     const float4 ww = *reinterpret_cast<const float4 *>(W2T + k * H + rg * R + 4 * r4);
                     w[4 * r4] = ww.x; w[4 * r4 + 1] = ww.y; w[4 * r4 + 2] = ww.z; w[4 * r4 + 3] = ww.w;
                 }
-            } else {
+            } else if constexpr (R % 2 == 0) {
 #pragma unroll
                 for (int r2 = 0; r2 < R / 2; ++r2) {
                     const float2 ww = *reinterpret_cast<const float2 *>(W2T + k * H + rg * R + 2 * r2);
                     w[2 * r2] = ww.x; w[2 * r2 + 1] = ww.y;
                 }
+            } else {                                                           // R = 1 (H = 16): one unit per lane
+                w[0] = W2T[k * H + rg];
             }
             const float4 h4 = *reinterpret_cast<const float4 *>(hp + k * kHS);      // k runs in the permuted order
             const float h5 = hp[k * kHS + 4];
@@ -277,29 +293,28 @@ __global__ void stat_part_reduce_kernel(double *__restrict__ totals, const doubl
     totals[c] = s;
 }
 
-}  // namespace des
-
-extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_returns_out_dev,
-                                        double *obs_totals_out_dev, const float *theta_dev,
-                                        const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
-                                        double sigma, double clip, double action_noise_std, uint64_t seed,
-                                        uint64_t generation, const des_state *state_dev, int64_t member_offset,
-                                        int64_t n_local, int noiseless, void *workspace_dev, size_t workspace_bytes,
-                                        void *stream) {
-    using namespace des;
-    DES_REQUIRE(env == kEnvPendulum, "des_rollout_eval: unknown environment %d (0 = Pendulum-v0)", env);
-    DES_REQUIRE(dims.state_dim == 3 && dims.action_dim == 1, "des_rollout_eval: Pendulum-v0 has state_dim 3, action_dim 1");
-    DES_REQUIRE(dims.hidden > 0 && dims.hidden % 32 == 0 && dims.hidden <= kMaxRollH,
-                "des_rollout_eval: hidden must be a multiple of 32, <= %d (got %d)", kMaxRollH, dims.hidden);
-    DES_REQUIRE(repetitions >= 1 && repetitions <= 10, "des_rollout_eval: repetitions must be in [1, 10] (one warp each)");
-    DES_REQUIRE(dims.tape_len >= 1, "des_rollout_eval: episode length (dims.tape_len) must be >= 1");
+// Shared by both entry points: argument checks (before any CUDA work), workspace, launch.  rows_mode selects the
+// explicit-solution kernels: `weights` is then rows[n_local][P] instead of the theta that sigma*eps perturbs.
+static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
+                          double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
+                          const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
+                          double clip, double action_noise_std, uint64_t seed, uint64_t generation,
+                          const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
+                          void *workspace_dev, size_t workspace_bytes, cudaStream_t st) {
+    DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
+    DES_REQUIRE(dims.state_dim == 3 && dims.action_dim == 1, "%s: Pendulum-v0 has state_dim 3, action_dim 1", who);
+    DES_REQUIRE(dims.hidden == 16 || (dims.hidden > 0 && dims.hidden % 32 == 0 && dims.hidden <= kMaxRollH),
+                "%s: hidden must be 16 or a multiple of 32, <= %d (got %d)", who, kMaxRollH, dims.hidden);
+    DES_REQUIRE(repetitions >= 1 && repetitions <= 10, "%s: repetitions must be in [1, 10] (one warp each)", who);
+    DES_REQUIRE(dims.tape_len >= 1, "%s: episode length (dims.tape_len) must be >= 1", who);
     DES_REQUIRE(n_local >= 0 && member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 28,
-                "des_rollout_eval: bad member range");
+                "%s: bad member range", who);
     if (n_local == 0) return DES_OK;
-    DES_REQUIRE(fitness_out_dev && theta_dev, "des_rollout_eval: NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
+    DES_REQUIRE(fitness_out_dev && weights_dev, "%s: NULL pointer", who);
     RollArgs a;
-    a.fitness = fitness_out_dev; a.ep_ret = episode_returns_out_dev; a.theta = theta_dev; a.obs_stats = obs_stats_dev; a.state = state_dev;
+    a.fitness = fitness_out_dev; a.ep_ret = episode_returns_out_dev;
+    a.theta = rows_mode ? nullptr : weights_dev; a.rows = rows_mode ? weights_dev : nullptr;
+    a.obs_stats = obs_stats_dev; a.state = state_dev;
     a.L = Layout(3, dims.hidden, 1);
     a.reps = repetitions; a.horizon = dims.tape_len;
     a.sigma = noiseless ? 0.f : (float)sigma; a.clip = (float)clip; a.act_noise = (float)action_noise_std;
@@ -311,7 +326,7 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     if (obs_totals_out_dev) {
         const size_t need = (size_t)n_local * 7 * sizeof(double);
         if (!workspace_dev || workspace_bytes < need) {
-            set_error("des_rollout_eval: workspace %zu B < required %zu B", workspace_bytes, need);
+            set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
             return DES_ERR_WORKSPACE;
         }
         a.stat_part = (double *)workspace_dev;
@@ -319,16 +334,18 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     const int H = dims.hidden;
     const size_t smem = sizeof(float) * ((size_t)H * H + 2 * (size_t)H * kHS + 8 + 40 + (size_t)H * 4 + 3 * (size_t)H + 4) +
                         sizeof(double) * 80;
-#define DES_ROLL_LAUNCH(HPL)                                                                                        \
+#define DES_ROLL_LAUNCH(R)                                                                                          \
     do {                                                                                                            \
-        DES_CUDA(cudaFuncSetAttribute(rollout_pendulum_kernel<HPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        rollout_pendulum_kernel<HPL><<<(unsigned)n_local, 32, smem, st>>>(a);                                  \
+        auto k__ = rows_mode ? rollout_pendulum_kernel<R, true> : rollout_pendulum_kernel<R, false>;               \
+        DES_CUDA(cudaFuncSetAttribute(k__, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));               \
+        k__<<<(unsigned)n_local, 32, smem, st>>>(a);                                                                \
     } while (0)
-    switch (H / 32) {
+    switch (H / 16) {                    // R = H/16 hidden units per lane
         case 1: DES_ROLL_LAUNCH(1); break;
         case 2: DES_ROLL_LAUNCH(2); break;
-        case 3: DES_ROLL_LAUNCH(3); break;
-        default: DES_ROLL_LAUNCH(4); break;
+        case 4: DES_ROLL_LAUNCH(4); break;
+        case 6: DES_ROLL_LAUNCH(6); break;
+        default: DES_ROLL_LAUNCH(8); break;
     }
 #undef DES_ROLL_LAUNCH
     DES_LAUNCH_CHECK("rollout_pendulum_kernel");
@@ -337,6 +354,33 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
         DES_LAUNCH_CHECK("stat_part_reduce_kernel");
     }
     return DES_OK;
+}
+
+}  // namespace des
+
+extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_returns_out_dev,
+                                        double *obs_totals_out_dev, const float *theta_dev,
+                                        const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
+                                        double sigma, double clip, double action_noise_std, uint64_t seed,
+                                        uint64_t generation, const des_state *state_dev, int64_t member_offset,
+                                        int64_t n_local, int noiseless, void *workspace_dev, size_t workspace_bytes,
+                                        void *stream) {
+    return des::rollout_launch("des_rollout_eval", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
+                               false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
+                               generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
+                               (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
+                                                  double *obs_totals_out_dev, const float *solutions_dev,
+                                                  const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
+                                                  double clip, double action_noise_std, uint64_t seed,
+                                                  uint64_t generation, int64_t member_offset, int64_t n_local,
+                                                  void *workspace_dev, size_t workspace_bytes, void *stream) {
+    return des::rollout_launch("des_rollout_eval_solutions", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
+                               solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
+                               seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
+                               (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,

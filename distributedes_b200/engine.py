@@ -268,9 +268,9 @@ class RolloutEngine(NESEngine):
                  horizon=None, action_noise_std=0.0, normalize_obs=True, **kw):
         if task not in self.ENVS:
             raise ValueError('closed-loop environments available on the device: %s (got %r)' % (sorted(self.ENVS), task))
-        if int(hidden) % 32 != 0 or not (32 <= int(hidden) <= 128):
-            raise ValueError('RolloutEngine: hidden must be 32, 64, 96 or 128 (des_rollout_eval keeps 4 units per lane); got %r'
-                             % (hidden,))
+        if int(hidden) not in (16, 32, 64, 96, 128):
+            raise ValueError('RolloutEngine: hidden must be 16, 32, 64, 96 or 128 (des_rollout_eval keeps H/16 units per lane); '
+                             'got %r' % (hidden,))
         if not (1 <= int(repetitions) <= 10):
             raise ValueError('RolloutEngine: repetitions must be in [1, 10] (one warp steps them in lockstep); got %r'
                              % (repetitions,))

@@ -144,6 +144,37 @@ def rollout_eval(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, cl
     return out
 
 
+def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions=10, clip, action_noise_std=0.0, seed,
+                           generation=0, member_offset=0, obs_stats=None, totals_out=None, workspace=None, out=None,
+                           episodes_out=None):
+    """Closed-loop fitness of explicit solutions[n_local, P] (CMA-ES's ask() rows, cma_es.py:22-29): row i is global
+    member member_offset + i, whose episodes reset from the same counter stream as rollout_eval's member."""
+    if env not in ENV_DIMS:
+        raise RuntimeError('unknown environment id %r' % (env,))
+    d0, A = ENV_DIMS[env]
+    if solutions.dim() != 2:
+        raise RuntimeError('solutions must be [n_local, P], got shape %r' % (tuple(solutions.shape),))
+    n_local, P = solutions.shape
+    if P != param_count(d0, hidden, A):
+        raise RuntimeError('solutions have %d entries, the (%d,%d,%d) MLP needs %d' % (P, d0, hidden, A, param_count(d0, hidden, A)))
+    if out is None:
+        out = torch.empty(n_local, dtype=torch.float32, device=solutions.device)
+    elif out.numel() != n_local:
+        raise RuntimeError('out has %d entries, need n_local=%d' % (out.numel(), n_local))
+    if totals_out is not None and workspace is None:
+        workspace = torch.empty(max(n_local, 1) * (2 * d0 + 1), dtype=torch.float64, device=solutions.device)
+    ws_bytes = workspace.numel() * workspace.element_size() if workspace is not None else 0
+    with _on(solutions, 'solutions'):
+        _lib.check(_lib.load().des_rollout_eval_solutions(
+            _ptr(out, torch.float32, 'out'), _ptr(episodes_out, torch.float32, 'episodes_out', True),
+            _ptr(totals_out, torch.float64, 'totals_out', True), _ptr(solutions, torch.float32, 'solutions'),
+            _ptr(obs_stats, torch.float32, 'obs_stats', True), int(env), Dims(d0, hidden, A, horizon), int(repetitions),
+            float(clip), float(action_noise_std), int(seed), int(generation), int(member_offset), int(n_local),
+            C.c_void_p(workspace.data_ptr()) if workspace is not None else C.c_void_p(0), ws_bytes, _stream()),
+            'des_rollout_eval_solutions')
+    return out
+
+
 def obs_stats_merge_totals(stats, totals, state_dim):
     """Chan merge of a batch given by fp64 [sum | sum of squares | count] into stats [m|v|n] (utils.py:85-96)."""
     with _on(stats, 'stats'):

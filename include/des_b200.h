@@ -133,13 +133,26 @@ DES_API int des_obs_normalize(float *obs_out_dev, const float *obs_dev, const fl
  * obs_totals_out_dev (optional, fp64 [2*state_dim + 1]) receives sum, sum of squares and count of the RAW observations
  * fed to the normaliser by these members — what the workers' online stats hold (utils.py:68-73) — to be summed over
  * ranks and merged with des_obs_stats_merge_totals; it needs workspace_dev of n_local * (2*state_dim+1) * 8 bytes.
- * hidden must be a multiple of 32 (<= 128), repetitions <= 10.  Arithmetic: policy in fp32 (FFMA, accurate tanh),
- * dynamics in fp64 like gym's float64 state. */
+ * hidden must be 16 or a multiple of 32 (<= 128), repetitions <= 10.  Arithmetic: policy in fp32 (FFMA, accurate
+ * tanh), dynamics in fp64 like gym's float64 state. */
 DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
                              const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                              double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                              const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                              void *workspace_dev, size_t workspace_bytes, void *stream);
+
+/* The same rollouts for explicit solutions: member i (i < n_local) takes its weights from row i of solutions_dev
+ * [n_local][P] (fp32, row-major, P = des_param_count(3, hidden, 1)) instead of theta + sigma*eps; no noise is generated.
+ * This is CMA-ES's evaluation of the solutions ask() returns: Worker.run cma_es.py:22-29 -> Evaluator.eval
+ * utils.py:116-124 -> single_run utils.py:126-139 (fitness_out_dev is the mean return, i.e. -cost of cma_es.py:28).
+ * Reset and action-noise counters use the global member index member_offset + i and `generation` exactly as
+ * des_rollout_eval does, so a shard evaluates its rows to the same bits as the whole population in one call.
+ * Outputs, normaliser, workspace, validation and the NULL / n_local == 0 rules are those of des_rollout_eval. */
+DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                       const float *solutions_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                       int32_t repetitions, double clip, double action_noise_std, uint64_t seed,
+                                       uint64_t generation, int64_t member_offset, int64_t n_local, void *workspace_dev,
+                                       size_t workspace_bytes, void *stream);
 
 /* Chan merge (utils.py:85-96) of a batch given by obs_totals_dev = [sum (d0) | sum of squares (d0) | count] into
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
