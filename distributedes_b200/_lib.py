@@ -51,21 +51,18 @@ SIGNATURES = {
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_pop_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _I64, _P]),
-    'des_rank_workspace_bytes': (_SZ, [_I64]),
-    'des_rank_workspace_bytes_n': (_SZ, [_I64, _I64]),
+    'des_rank_workspace_bytes': (_SZ, [_I64, _I64]),
     'des_centered_rank': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
     'des_grad_workspace_bytes': (_SZ, [_I64, _I64]),
     'des_nes_grad_partial': (C.c_int, [_P, _P, _I64, _I64, _U64, _U64, _P, _I64, _P, _SZ, _P]),
     'des_nes_apply': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, Opt, _P, _P]),
     'des_state_init': (C.c_int, [_P, _U64, _P]),
     'des_state_advance': (C.c_int, [_P, _D, _D, _P]),
-    'des_cma_rank_mu': (C.c_int, [_P, _P, _P, _I64, _I64, _P]),
+    'des_cma_rank_mu_workspace_bytes': (_SZ, [_I64, _I64]),
+    'des_cma_rank_mu': (C.c_int, [_P, _P, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_cma_cov_apply': (C.c_int, [_P, _P, _P, _I64, _D, _D, _D, _P]),
     'des_cma_packed_elems': (_I64, [_I64]),
-    'des_cma_rank_mu_packed': (C.c_int, [_P, _P, _P, _I64, _I64, _P]),
     'des_cma_cov_apply_packed': (C.c_int, [_P, _P, _P, _I64, _D, _D, _D, _P]),
-    'des_cma_tc_workspace_bytes': (_SZ, [_I64, _I64]),
-    'des_cma_rank_mu_tc': (C.c_int, [_P, _P, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_comm_create': (C.c_int, [C.POINTER(_P), C.c_int, C.c_int, _I64, _I64, _P]),
     'des_comm_connect': (C.c_int, [_P, _P]),
     'des_comm_destroy': (None, [_P]),

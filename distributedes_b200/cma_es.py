@@ -44,9 +44,9 @@ class CMAEvolutionStrategy:
 
     With torch.distributed initialised the lambda members are sharded contiguously over the ranks (SURVEY 8e): ask()
     returns the rank's own members (z regenerated from the counter stream, so no solution is ever shipped), tell() takes
-    the local solutions and the GLOBAL cost vector, forms the rank's partial sum_i w_i y_i y_i^T with des_cma_rank_mu and
-    all-reduces the [n, n] partial — the one collective BASELINE.json's north_star names for CMA-ES — plus the n-vector
-    sum_i w_i y_i.  Every rank then applies the identical update, so the strategy state is never broadcast.
+    the local solutions and the GLOBAL cost vector, forms the rank's partial sum_i w_i y_i y_i^T with des_cma_rank_mu as
+    packed upper-triangular tiles and all-reduces them — the one collective BASELINE.json's north_star names for CMA-ES —
+    plus the n-vector sum_i w_i y_i.  Every rank then applies the identical update, so the strategy state is never broadcast.
 
     `kernels` (default: distributedes_b200.ops) exists so the world_size > 1 host logic can run under gloo on CPU in the
     test-suite with an oracle-backed stand-in; the product never runs without the CUDA library."""
@@ -132,7 +132,7 @@ class CMAEvolutionStrategy:
         # ---- the hot part: rank-mu partial of the shard on our kernel (fp32), summed over ranks.  Sharded runs keep the
         # partial as packed upper-triangular tiles: the all-reduce moves half the bytes of the [n, n] matrix and the
         # covariance update mirrors the tiles while applying them.
-        packed = self.world > 1 and hasattr(self.kn, 'cma_rank_mu_packed')
+        packed = self.world > 1
         Y32, w32 = Y.to(torch.float32).contiguous(), w_loc64.to(torch.float32).contiguous()
         if packed:
             if getattr(self, 'dC_tiles', None) is None:
@@ -147,8 +147,6 @@ class CMAEvolutionStrategy:
                 self.kn.cma_rank_mu(Y32, w32, out=self.dC)
             else:
                 self.dC.zero_()
-            if self.world > 1:
-                dist.all_reduce(self.dC, group=self.pg)
         if self.world > 1:
             dist.all_reduce(yw, group=self.pg)
         self.m = self.m + self.sigma * yw

@@ -173,7 +173,7 @@ extern "C" DES_API int des_session_create(des_session **out, int device, des_dim
     DES_S_CUDA(cudaMalloc(&s->adam_m, P * sizeof(double)));
     DES_S_CUDA(cudaMalloc(&s->adam_v, P * sizeof(double)));
     DES_S_CUDA(cudaMalloc(&s->state, sizeof(des_state)));
-    s->rank_ws_bytes = des_rank_workspace_bytes_n(N, n_local) + 16;
+    s->rank_ws_bytes = des_rank_workspace_bytes(N, n_local) + 16;
     s->grad_ws_bytes = des_grad_workspace_bytes(n_local, P) + 16;
     DES_S_CUDA(cudaMalloc(&s->rank_ws, s->rank_ws_bytes));
     DES_S_CUDA(cudaMalloc(&s->grad_ws, s->grad_ws_bytes));

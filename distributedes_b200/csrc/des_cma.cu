@@ -11,24 +11,23 @@ namespace des {
 
 constexpr int kCmaThreads = 256;
 constexpr int kCmaKP = 16;   // members per k-panel
+constexpr int kCmaTile = 64; // output tile side; the kernel runs for n < kCmaTcMinN, where it is the packed tile side
+static_assert(cma_packed_tile(kCmaTcMinN - 1) == kCmaTile, "packed output of the FFMA kernel needs tiles of its side");
 
-// TILE x TILE outputs per CTA, 256 threads as 16 x 16.  Each thread owns (TILE/16)^2 outputs arranged as blocks of
-// 4 consecutive rows/columns spaced 64 apart (rows ty*4 + {0..3} + 64*g), so every shared-memory operand read is one
-// conflict-free LDS.128 (16 FMA per LDS for the 128 tile).  k-panels of 16 members are double buffered: the next
-// panel's global loads are in flight while the current one is multiplied.
-template <int TILE>
+// 64 x 64 outputs per CTA, 256 threads as 16 x 16.  Each thread owns a 4 x 4 block (rows ty*4 + {0..3}, columns
+// tx*4 + {0..3}), so every shared-memory operand read is one conflict-free LDS.128.  k-panels of 16 members are double
+// buffered: the next panel's global loads are in flight while the current one is multiplied.
 __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restrict__ dC, const float *__restrict__ Y,
                                                                   const float *__restrict__ w, int64_t lambda, int64_t n,
                                                                   int tiles_per_side, int packed) {
-    constexpr int G = TILE / 64;                 // 4-wide groups per thread and dimension (1 or 2)
-    constexpr int MT = 4 * G;
-    constexpr int LD = kCmaKP * TILE / kCmaThreads;   // elements each thread stages per operand and panel
-    __shared__ __align__(16) float As[2][kCmaKP][TILE];   // w_k * Y[k][i0 + i]
-    __shared__ __align__(16) float Bs[2][kCmaKP][TILE];   //       Y[k][j0 + j]
+    constexpr int MT = 4;
+    constexpr int LD = kCmaKP * kCmaTile / kCmaThreads;   // elements each thread stages per operand and panel
+    __shared__ __align__(16) float As[2][kCmaKP][kCmaTile];   // w_k * Y[k][i0 + i]
+    __shared__ __align__(16) float Bs[2][kCmaKP][kCmaTile];   //       Y[k][j0 + j]
     int bi = 0, rem = blockIdx.x;
     while (rem >= tiles_per_side - bi) { rem -= tiles_per_side - bi; ++bi; }
     const int bj = bi + rem;
-    const int64_t i0 = (int64_t)bi * TILE, j0 = (int64_t)bj * TILE;
+    const int64_t i0 = (int64_t)bi * kCmaTile, j0 = (int64_t)bj * kCmaTile;
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
 
     float acc[MT][MT];
@@ -42,7 +41,7 @@ __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restr
 #pragma unroll
         for (int e = 0; e < LD; ++e) {
             const int idx = threadIdx.x + e * kCmaThreads;
-            const int kk = idx / TILE, c = idx - kk * TILE;
+            const int kk = idx / kCmaTile, c = idx - kk * kCmaTile;
             const int64_t k = k0 + kk;
             float a = 0.f, b = 0.f;
             if (k < lambda) {
@@ -58,7 +57,7 @@ __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restr
 #pragma unroll
         for (int e = 0; e < LD; ++e) {
             const int idx = threadIdx.x + e * kCmaThreads;
-            const int kk = idx / TILE, c = idx - kk * TILE;
+            const int kk = idx / kCmaTile, c = idx - kk * kCmaTile;
             As[buf][kk][c] = ra[e];
             Bs[buf][kk][c] = rb[e];
         }
@@ -72,14 +71,9 @@ __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restr
         if (more) fetch(k0 + kCmaKP);            // global loads overlap the multiply below
 #pragma unroll
         for (int kk = 0; kk < kCmaKP; ++kk) {
-            float av[MT], bv[MT];
-#pragma unroll
-            for (int g = 0; g < G; ++g) {
-                const float4 a4 = *reinterpret_cast<const float4 *>(&As[buf][kk][ty * 4 + 64 * g]);
-                const float4 b4 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][tx * 4 + 64 * g]);
-                av[4 * g] = a4.x; av[4 * g + 1] = a4.y; av[4 * g + 2] = a4.z; av[4 * g + 3] = a4.w;
-                bv[4 * g] = b4.x; bv[4 * g + 1] = b4.y; bv[4 * g + 2] = b4.z; bv[4 * g + 3] = b4.w;
-            }
+            const float4 a4 = *reinterpret_cast<const float4 *>(&As[buf][kk][ty * 4]);
+            const float4 b4 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][tx * 4]);
+            const float av[MT] = {a4.x, a4.y, a4.z, a4.w}, bv[MT] = {b4.x, b4.y, b4.z, b4.w};
 #pragma unroll
             for (int a = 0; a < MT; ++a)
 #pragma unroll
@@ -92,32 +86,29 @@ __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restr
         }
     }
     if (packed) {
-        // upper-triangular tiles only, tile after tile ([tile][TILE][TILE], the collective's payload: half the bytes of
+        // upper-triangular tiles only, tile after tile ([tile][64][64], the collective's payload: half the bytes of
         // the full matrix); entries beyond n are zero so that partial sums of different ranks can be added blindly
-        float *tile = dC + (int64_t)blockIdx.x * TILE * TILE;
+        float *tile = dC + (int64_t)blockIdx.x * kCmaTile * kCmaTile;
+        const int lj = tx * 4;
 #pragma unroll
         for (int a = 0; a < MT; ++a) {
-            const int li = ty * 4 + (a & 3) + 64 * (a >> 2);
-#pragma unroll
-            for (int g = 0; g < G; ++g) {
-                const int lj = tx * 4 + 64 * g;
-                float4 v = make_float4(acc[a][4 * g], acc[a][4 * g + 1], acc[a][4 * g + 2], acc[a][4 * g + 3]);
-                if (i0 + li >= n) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (j0 + lj + 0 >= n) v.x = 0.f;
-                if (j0 + lj + 1 >= n) v.y = 0.f;
-                if (j0 + lj + 2 >= n) v.z = 0.f;
-                if (j0 + lj + 3 >= n) v.w = 0.f;
-                *reinterpret_cast<float4 *>(tile + li * TILE + lj) = v;
-            }
+            const int li = ty * 4 + a;
+            float4 v = make_float4(acc[a][0], acc[a][1], acc[a][2], acc[a][3]);
+            if (i0 + li >= n) v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (j0 + lj + 0 >= n) v.x = 0.f;
+            if (j0 + lj + 1 >= n) v.y = 0.f;
+            if (j0 + lj + 2 >= n) v.z = 0.f;
+            if (j0 + lj + 3 >= n) v.w = 0.f;
+            *reinterpret_cast<float4 *>(tile + li * kCmaTile + lj) = v;
         }
         return;
     }
 #pragma unroll
     for (int a = 0; a < MT; ++a) {
-        const int64_t i = i0 + ty * 4 + (a & 3) + 64 * (a >> 2);
+        const int64_t i = i0 + ty * 4 + a;
 #pragma unroll
         for (int b = 0; b < MT; ++b) {
-            const int64_t j = j0 + tx * 4 + (b & 3) + 64 * (b >> 2);
+            const int64_t j = j0 + tx * 4 + b;
             if (i < n && j < n) {
                 if (bi != bj) {
                     dC[i * n + j] = acc[a][b];
@@ -186,30 +177,39 @@ __global__ void __launch_bounds__(256) cma_cov_apply_packed_kernel(float *__rest
 
 }  // namespace des
 
-static int cma_tile(int64_t n) { return n <= 2048 ? 64 : 128; }
-
 extern "C" DES_API int64_t des_cma_packed_elems(int64_t n) {
     if (n <= 0) return 0;
-    const int64_t tile = cma_tile(n), t = (n + tile - 1) / tile;
+    const int64_t tile = des::cma_packed_tile(n), t = (n + tile - 1) / tile;
     return t * (t + 1) / 2 * tile * tile;
 }
 
-extern "C" DES_API int des_cma_rank_mu_packed(float *tiles_out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local,
-                                              int64_t n, void *stream) {
+extern "C" DES_API size_t des_cma_rank_mu_workspace_bytes(int64_t n, int64_t lambda_local) {
+    return n >= des::kCmaTcMinN && lambda_local > 0 ? des::cma_tc_workspace_bytes(n, lambda_local) : 0;
+}
+
+extern "C" DES_API int des_cma_rank_mu(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
+                                       int packed, void *workspace_dev, size_t workspace_bytes, void *stream) {
     using namespace des;
-    DES_REQUIRE(n > 0 && lambda_local >= 0, "des_cma_rank_mu_packed: bad sizes lambda=%lld n=%lld", (long long)lambda_local,
+    DES_REQUIRE(n > 0 && lambda_local >= 0, "des_cma_rank_mu: bad sizes lambda=%lld n=%lld", (long long)lambda_local,
                 (long long)n);
-    DES_REQUIRE(n <= 46340 * 16, "des_cma_rank_mu_packed: n too large");
-    DES_REQUIRE(tiles_out_dev && (lambda_local == 0 || (Y_dev && w_dev)), "des_cma_rank_mu_packed: NULL pointer");
+    DES_REQUIRE(n <= 46340 * 16, "des_cma_rank_mu: n too large");
+    DES_REQUIRE(out_dev && (lambda_local == 0 || (Y_dev && w_dev)), "des_cma_rank_mu: NULL pointer");
+    const size_t need = des_cma_rank_mu_workspace_bytes(n, lambda_local);
+    if (need && (!workspace_dev || workspace_bytes < need)) {
+        set_error("des_cma_rank_mu: workspace %zu B < required %zu B", workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
     cudaStream_t st = (cudaStream_t)stream;
     if (lambda_local == 0) {
-        DES_CUDA(cudaMemsetAsync(tiles_out_dev, 0, (size_t)des_cma_packed_elems(n) * sizeof(float), st));
+        const size_t elems = packed ? (size_t)des_cma_packed_elems(n) : (size_t)n * n;
+        DES_CUDA(cudaMemsetAsync(out_dev, 0, elems * sizeof(float), st));
         return DES_OK;
     }
-    const int tile = cma_tile(n), t = (int)((n + tile - 1) / tile);
-    if (tile == 64) cma_rank_mu_kernel<64><<<(unsigned)(t * (t + 1) / 2), kCmaThreads, 0, st>>>(tiles_out_dev, Y_dev, w_dev, lambda_local, n, t, 1);
-    else cma_rank_mu_kernel<128><<<(unsigned)(t * (t + 1) / 2), kCmaThreads, 0, st>>>(tiles_out_dev, Y_dev, w_dev, lambda_local, n, t, 1);
-    DES_LAUNCH_CHECK("cma_rank_mu_kernel(packed)");
+    if (n >= kCmaTcMinN) return cma_rank_mu_tc(out_dev, Y_dev, w_dev, lambda_local, n, packed, workspace_dev, st);
+    const int t = (int)((n + kCmaTile - 1) / kCmaTile);
+    cma_rank_mu_kernel<<<(unsigned)(t * (t + 1) / 2), kCmaThreads, 0, st>>>(out_dev, Y_dev, w_dev, lambda_local, n, t,
+                                                                            packed ? 1 : 0);
+    DES_LAUNCH_CHECK("cma_rank_mu_kernel");
     return DES_OK;
 }
 
@@ -218,36 +218,13 @@ extern "C" DES_API int des_cma_cov_apply_packed(float *C_dev, const float *tiles
     using namespace des;
     DES_REQUIRE(n > 0, "des_cma_cov_apply_packed: n=%lld", (long long)n);
     DES_REQUIRE(C_dev && tiles_dev, "des_cma_cov_apply_packed: NULL pointer");
-    const int tile = cma_tile(n), t = (int)((n + tile - 1) / tile);
+    const int tile = cma_packed_tile(n), t = (int)((n + tile - 1) / tile);
     const unsigned upper = (unsigned)(t * (t + 1) / 2);
     if (tile == 64)
         cma_cov_apply_packed_kernel<64><<<upper, 256, 0, (cudaStream_t)stream>>>(C_dev, tiles_dev, pc_dev, n, (float)decay, (float)c1, (float)cmu, t);
     else
         cma_cov_apply_packed_kernel<128><<<upper * 4, 256, 0, (cudaStream_t)stream>>>(C_dev, tiles_dev, pc_dev, n, (float)decay, (float)c1, (float)cmu, t);
     DES_LAUNCH_CHECK("cma_cov_apply_packed_kernel");
-    return DES_OK;
-}
-
-extern "C" DES_API int des_cma_rank_mu(float *dC_out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
-                               void *stream) {
-    using namespace des;
-    DES_REQUIRE(n > 0 && lambda_local >= 0, "des_cma_rank_mu: bad sizes lambda=%lld n=%lld", (long long)lambda_local,
-                (long long)n);
-    DES_REQUIRE(n <= 46340 * 16, "des_cma_rank_mu: n too large");
-    DES_REQUIRE(dC_out_dev && (lambda_local == 0 || (Y_dev && w_dev)), "des_cma_rank_mu: NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (lambda_local == 0) {
-        DES_CUDA(cudaMemsetAsync(dC_out_dev, 0, (size_t)n * n * sizeof(float), st));
-        return DES_OK;
-    }
-    if (n <= 2048) {
-        const int t = (int)((n + 63) / 64);
-        cma_rank_mu_kernel<64><<<(unsigned)(t * (t + 1) / 2), kCmaThreads, 0, st>>>(dC_out_dev, Y_dev, w_dev, lambda_local, n, t, 0);
-    } else {
-        const int t = (int)((n + 127) / 128);
-        cma_rank_mu_kernel<128><<<(unsigned)(t * (t + 1) / 2), kCmaThreads, 0, st>>>(dC_out_dev, Y_dev, w_dev, lambda_local, n, t, 0);
-    }
-    DES_LAUNCH_CHECK("cma_rank_mu_kernel");
     return DES_OK;
 }
 

@@ -8,9 +8,9 @@
 //              tiles brought in by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) through a three-stage mbarrier pipeline:
 //              warps 0-7 = two consumer warpgroups (64 output rows each: wgmma, then registers -> global), warp 8 = TMA
 //   output     the full symmetric matrix (upper entry written to both sides: exactly symmetric), or the packed
-//              upper-triangular tiles of des_cma_rank_mu_packed (the payload of the cross-rank sum)
+//              upper-triangular tiles (the payload of the cross-rank sum)
 //
-// The fp32 FFMA kernel of des_cma.cu stays as the small-n / no-workspace path.
+// des_cma_rank_mu (des_cma.cu) runs this for n >= kCmaTcMinN and the fp32 FFMA kernel below that.
 // Accuracy: measured against the fp64 restatement in tests/test_gpu_cma.py at the same 1e-5 (both norms) bar.
 #include <cuda.h>
 #include <stddef.h>
@@ -194,31 +194,20 @@ static EncodeTiledFn encode_tiled_fn() {
 static int64_t lambda_pad_of(int64_t lambda) { return (lambda + kBK - 1) / kBK * kBK; }
 
 }  // namespace cmatc
-}  // namespace des
 
-extern "C" DES_API size_t des_cma_tc_workspace_bytes(int64_t n, int64_t lambda_local) {
-    if (n <= 0 || lambda_local <= 0) return 0;
-    return 4 * (size_t)n * (size_t)des::cmatc::lambda_pad_of(lambda_local) * sizeof(__half) + 1024;
+size_t cma_tc_workspace_bytes(int64_t n, int64_t lambda) {
+    return 4 * (size_t)n * (size_t)cmatc::lambda_pad_of(lambda) * sizeof(__half) + 1024;
 }
 
-extern "C" DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
-                                          int packed, void *workspace_dev, size_t workspace_bytes, void *stream) {
-    using namespace des;
-    using namespace des::cmatc;
-    DES_REQUIRE(n > 0 && lambda_local > 0, "des_cma_rank_mu_tc: bad sizes lambda=%lld n=%lld", (long long)lambda_local, (long long)n);
-    DES_REQUIRE(n < ((int64_t)1 << 20), "des_cma_rank_mu_tc: n too large");
-    DES_REQUIRE(out_dev && Y_dev && w_dev, "des_cma_rank_mu_tc: NULL pointer");
-    const size_t need = des_cma_tc_workspace_bytes(n, lambda_local);
-    if (!workspace_dev || workspace_bytes < need) {
-        set_error("des_cma_rank_mu_tc: workspace %zu B < required %zu B", workspace_bytes, need);
-        return DES_ERR_WORKSPACE;
-    }
+// Called by des_cma_rank_mu with validated sizes (n >= kCmaTcMinN, lambda >= 1) and a large enough workspace.
+int cma_rank_mu_tc(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n, int packed,
+                   void *workspace_dev, cudaStream_t st) {
+    using namespace cmatc;
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) {
-        set_error("des_cma_rank_mu_tc: cuTensorMapEncodeTiled is not available from this driver");
+        set_error("des_cma_rank_mu: cuTensorMapEncodeTiled is not available from this driver");
         return DES_ERR_UNSUPPORTED;
     }
-    cudaStream_t st = (cudaStream_t)stream;
     const int64_t lp = lambda_pad_of(lambda_local);
     __half *base = reinterpret_cast<__half *>(((uintptr_t)workspace_dev + 1023) & ~(uintptr_t)1023);
     __half *zs_hi = base, *zs_lo = base + n * lp, *z_hi = base + 2 * n * lp, *z_lo = base + 3 * n * lp;
@@ -236,7 +225,7 @@ extern "C" DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, co
                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (cr != CUDA_SUCCESS) {
-            set_error("des_cma_rank_mu_tc: cuTensorMapEncodeTiled failed (%d)", (int)cr);
+            set_error("des_cma_rank_mu: cuTensorMapEncodeTiled failed (%d)", (int)cr);
             return DES_ERR_CUDA;
         }
     }
@@ -244,7 +233,7 @@ extern "C" DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, co
     a.out = out_dev; a.n = n; a.k_stages = (int)(lp / kBK);
     a.tiles = (int)((n + kBM - 1) / kBM);
     a.packed = packed ? 1 : 0;
-    a.ptile = n <= 2048 ? 64 : 128;
+    a.ptile = cma_packed_tile(n);
     a.ptiles_per_side = (int)((n + a.ptile - 1) / a.ptile);
     const int64_t tiles = (int64_t)a.tiles * (a.tiles + 1) / 2;
     const size_t smem = 1024 + (size_t)kStages * kStageBytes + sizeof(Bars);
@@ -253,3 +242,5 @@ extern "C" DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, co
     DES_LAUNCH_CHECK("cma_syrk_kernel");
     return DES_OK;
 }
+
+}  // namespace des

@@ -201,4 +201,12 @@ __device__ __forceinline__ uint64_t load_generation(const des_state *st, uint64_
     return st ? st->generation : fallback;
 }
 
+// ---- CMA rank-mu (des_cma.cu: fp32 FFMA kernel and the entry point; des_cma_tc.cu: split-fp16 wgmma SYRK) ----------
+constexpr int64_t kCmaTcMinN = 2048;     // n >= this runs on the tensor cores, smaller n on the FFMA kernel
+// side of the packed upper-triangular tiles (des_cma_packed_elems): 64 up to n = 2048, 128 above
+__host__ __device__ constexpr int cma_packed_tile(int64_t n) { return n <= 2048 ? 64 : 128; }
+size_t cma_tc_workspace_bytes(int64_t n, int64_t lambda);
+int cma_rank_mu_tc(float *out, const float *Y, const float *w, int64_t lambda, int64_t n, int packed, void *workspace,
+                   cudaStream_t stream);
+
 }  // namespace des

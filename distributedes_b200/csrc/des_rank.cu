@@ -3,7 +3,7 @@
 //   rank_i = #{j : f_j < f_i} + #{j < i : f_j == f_i}       (ascending; ties by index; NaN last)
 //   s_i    = rank_i/(N-1) - 0.5
 //
-// Counting rank instead of a sort: a shard needs ranks only for ITS members but against ALL N
+// Populations up to 2048: counting rank instead of a sort (larger ones take the bucketed path below).  A shard needs ranks only for ITS members but against ALL N
 // fitnesses (ranks are global), so the work is n_local x N comparisons, embarrassingly parallel,
 // integer-exact and deterministic.  Keys are order-preserving uint32 images of the floats; each
 // (i, j) pair costs one 64-bit compare.  The j range is split over blockIdx.y, partial counts are
@@ -72,15 +72,7 @@ __global__ void rank_finish_kernel(float *__restrict__ shaped, int32_t *__restri
 // Degenerate inputs (all keys equal) put everything in one bucket: still exact, cost falls back to n * N.
 constexpr int kBuckets = 1024;          // upper bound; populations up to 256k use 256 buckets / 1024 samples
 constexpr int kSamples = 4096;
-constexpr int64_t kBucketMinN = 2048;    // populations up to this size use the counting rank (DES_RANK_BUCKET_MIN overrides)
-static int64_t bucket_min_n() {
-    static const int64_t v = [] {
-        const char *e = getenv("DES_RANK_BUCKET_MIN");
-        const long long x = e ? atoll(e) : 0;
-        return x >= 1024 ? (int64_t)x : kBucketMinN;
-    }();
-    return v;
-}
+constexpr int64_t kBucketMinN = 2048;    // populations up to this size use the counting rank
 __host__ __device__ inline int buckets_for(int64_t N) { return N <= 262144 ? 256 : kBuckets; }
 
 // sample t of ns: the key of member floor(t N / ns)   (t < 4096, N < 2^31: the product fits 64 bits)
@@ -305,13 +297,9 @@ static BucketWs carve(void *ws, int64_t N) {
 
 }  // namespace des
 
-// The workspace depends on N only through the bucketed path; callers size it with des_rank_workspace_bytes_n.
-extern "C" DES_API size_t des_rank_workspace_bytes(int64_t n_local) {
+extern "C" DES_API size_t des_rank_workspace_bytes(int64_t N, int64_t n_local) {
+    if (N > des::kBucketMinN) return des::bucket_ws_bytes(N);
     return n_local > 0 ? (size_t)n_local * sizeof(int32_t) : 0;
-}
-extern "C" DES_API size_t des_rank_workspace_bytes_n(int64_t N, int64_t n_local) {
-    const size_t base = des_rank_workspace_bytes(n_local);
-    return N > des::bucket_min_n() ? (base > des::bucket_ws_bytes(N) ? base : des::bucket_ws_bytes(N)) : base;
 }
 
 extern "C" DES_API int des_centered_rank(float *shaped_out_dev, int32_t *rank_out_dev, const float *fitness_all_dev, int64_t N,
@@ -325,13 +313,13 @@ extern "C" DES_API int des_centered_rank(float *shaped_out_dev, int32_t *rank_ou
                 (long long)(member_offset + n_local), (long long)N);
     if (n_local == 0) return DES_OK;
     DES_REQUIRE(shaped_out_dev && fitness_all_dev, "des_centered_rank: NULL pointer");
-    if (!workspace_dev || workspace_bytes < des_rank_workspace_bytes(n_local)) {
-        set_error("des_centered_rank: workspace %zu B < required %zu B", workspace_bytes,
-                  des_rank_workspace_bytes(n_local));
+    const size_t need = des_rank_workspace_bytes(N, n_local);
+    if (!workspace_dev || workspace_bytes < need) {
+        set_error("des_centered_rank: workspace %zu B < required %zu B", workspace_bytes, need);
         return DES_ERR_WORKSPACE;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (N > bucket_min_n() && workspace_bytes >= bucket_ws_bytes(N)) {
+    if (N > kBucketMinN) {
         const BucketWs w = carve(workspace_dev, N);
         const unsigned gn = (unsigned)((N + 255) / 256);
         DES_CUDA(cudaMemsetAsync(w.bucket_count, 0, 2 * kBuckets * sizeof(int32_t), st));

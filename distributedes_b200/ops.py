@@ -234,9 +234,8 @@ def pop_eval(solutions, obs, target, *, hidden, clip, out=None):
     return out
 
 
-def rank_workspace(n_local, device, N=None):
-    lib = _lib.load()
-    nbytes = lib.des_rank_workspace_bytes_n(N, n_local) if N is not None else lib.des_rank_workspace_bytes(n_local)
+def rank_workspace(n_local, device, N):
+    nbytes = _lib.load().des_rank_workspace_bytes(N, n_local)
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
 
 
@@ -296,49 +295,36 @@ def nes_apply(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learning_r
             _stream()), 'des_nes_apply')
 
 
-_CMA_WS = {}      # (device, n, lambda) -> workspace tensor of the tensor-core rank-mu path
-CMA_TC_MIN_N = 2048
+_CMA_WS = {}      # (device, n, lambda) -> workspace tensor of des_cma_rank_mu (tensor-core shapes only)
+CMA_TC_MIN_N = 2048      # des_cma_rank_mu runs n >= this on the tensor cores, smaller n on the fp32 FFMA kernel
 
 
-def _cma_tc_workspace(n, lam, device):
-    key = (str(device), int(n), int(lam))
-    ws = _CMA_WS.get(key)
-    if ws is None:
-        ws = torch.empty(int(_lib.load().des_cma_tc_workspace_bytes(int(n), int(lam))), dtype=torch.uint8, device=device)
-        if len(_CMA_WS) > 8:
-            _CMA_WS.clear()
-        _CMA_WS[key] = ws
-    return ws
-
-
-def _cma_rank_mu(Y, w, out, packed, path):
-    lam, n = Y.shape
-    lib = _lib.load()
-    use_tc = (path == 'tc') or (path is None and n >= CMA_TC_MIN_N and lam >= 1)
-    with _on(Y, 'Y'):
-        if use_tc:
-            ws = _cma_tc_workspace(n, lam, Y.device)
-            _lib.check(lib.des_cma_rank_mu_tc(_ptr(out, torch.float32, 'out'), _ptr(Y, torch.float32, 'Y'),
-                                              _ptr(w, torch.float32, 'w'), lam, n, 1 if packed else 0,
-                                              C.c_void_p(ws.data_ptr()), ws.numel(), _stream()), 'des_cma_rank_mu_tc')
-        elif packed:
-            _lib.check(lib.des_cma_rank_mu_packed(_ptr(out, torch.float32, 'out'), _ptr(Y, torch.float32, 'Y'),
-                                                  _ptr(w, torch.float32, 'w'), lam, n, _stream()), 'des_cma_rank_mu_packed')
-        else:
-            _lib.check(lib.des_cma_rank_mu(_ptr(out, torch.float32, 'out'), _ptr(Y, torch.float32, 'Y'),
-                                           _ptr(w, torch.float32, 'w'), lam, n, _stream()), 'des_cma_rank_mu')
-    return out
-
-
-def cma_rank_mu(Y, w, out=None, path=None):
-    """dC[n,n] = sum_i w_i y_i y_i^T for Y[lambda_local, n] (rank-mu term of es.tell, cma_es.py:90).
-    path: None = tensor cores (split-fp16 wgmma SYRK) for n >= 256, fp32 FFMA below; 'tc' / 'ffma' force one."""
+def _cma_rank_mu(Y, w, out, packed):
     lam, n = Y.shape
     if w.numel() != lam:
         raise RuntimeError('w has %d entries, Y has %d rows' % (w.numel(), lam))
+    lib = _lib.load()
+    key = (str(Y.device), int(n), int(lam))
+    ws = _CMA_WS.get(key)
+    if ws is None:
+        ws = torch.empty(int(lib.des_cma_rank_mu_workspace_bytes(int(n), int(lam))), dtype=torch.uint8, device=Y.device)
+        if len(_CMA_WS) > 8:
+            _CMA_WS.clear()
+        _CMA_WS[key] = ws
+    with _on(Y, 'Y'):
+        _lib.check(lib.des_cma_rank_mu(_ptr(out, torch.float32, 'out'), _ptr(Y, torch.float32, 'Y'),
+                                       _ptr(w, torch.float32, 'w'), lam, n, 1 if packed else 0,
+                                       C.c_void_p(ws.data_ptr()), ws.numel(), _stream()), 'des_cma_rank_mu')
+    return out
+
+
+def cma_rank_mu(Y, w, out=None):
+    """dC[n,n] = sum_i w_i y_i y_i^T for Y[lambda_local, n] (rank-mu term of es.tell, cma_es.py:90).
+    Tensor cores (split-fp16 wgmma SYRK) for n >= CMA_TC_MIN_N, fp32 FFMA below."""
+    lam, n = Y.shape
     if out is None:
         out = torch.empty((n, n), dtype=torch.float32, device=Y.device)
-    return _cma_rank_mu(Y, w, out, False, path)
+    return _cma_rank_mu(Y, w, out, False)
 
 
 def cma_cov_apply(Cmat, dC, pc, *, decay, c1, cmu):
@@ -355,14 +341,12 @@ def cma_packed_elems(n):
     return int(_lib.load().des_cma_packed_elems(int(n)))
 
 
-def cma_rank_mu_packed(Y, w, out=None, path=None):
+def cma_rank_mu_packed(Y, w, out=None):
     """The rank-mu partial as packed upper-triangular tiles (the multi-GPU all-reduce payload: half of [n, n])."""
-    lam, n = Y.shape
-    if w.numel() != lam:
-        raise RuntimeError('w has %d entries, Y has %d rows' % (w.numel(), lam))
+    n = Y.shape[1]
     if out is None:
         out = torch.empty(cma_packed_elems(n), dtype=torch.float32, device=Y.device)
-    return _cma_rank_mu(Y, w, out, True, path)
+    return _cma_rank_mu(Y, w, out, True)
 
 
 def cma_cov_apply_packed(Cmat, tiles, pc, *, decay, c1, cmu):

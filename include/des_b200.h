@@ -191,11 +191,10 @@ DES_API int des_pop_eval(float *fitness_out_dev, const float *solutions_dev, con
  * rank_out_dev[i] = #{j : f_j < f_i} + #{j < i : f_j == f_i}  (ascending, ties by index; -0 == +0,
  * NaN ranks last) and shaped_out_dev[i] = fp32(rank/(N-1) - 0.5).  Replaces fitness_shift
  * utils.py:142-148 (whose argsort is unstable on ties; identical on tie-free input).
- * rank_out_dev may be NULL.  N >= 2.  workspace: at least des_rank_workspace_bytes(n_local); with
- * des_rank_workspace_bytes_n(N, n_local) bytes, populations above 2048 use the bucketed (sample-sort style)
- * path whose cost is ~N*N/1024 instead of n_local*N compares.  Results are identical either way. */
-DES_API size_t des_rank_workspace_bytes(int64_t n_local);
-DES_API size_t des_rank_workspace_bytes_n(int64_t N, int64_t n_local);
+ * rank_out_dev may be NULL.  N >= 2.  workspace: des_rank_workspace_bytes(N, n_local) bytes, or DES_ERR_WORKSPACE.
+ * Populations up to 2048 count n_local*N compares; larger ones take a bucketed (sample-sort style) path whose cost is
+ * ~N*N/1024 compares and whose workspace grows with N. */
+DES_API size_t des_rank_workspace_bytes(int64_t N, int64_t n_local);
 DES_API int des_centered_rank(float *shaped_out_dev, int32_t *rank_out_dev, const float *fitness_all_dev,
                       int64_t N, int64_t member_offset, int64_t n_local, void *workspace_dev,
                       size_t workspace_bytes, void *stream);
@@ -230,35 +229,31 @@ DES_API int des_state_advance(des_state *state_dev, double beta1, double beta2, 
 
 /* ---- CMA-ES rank-mu covariance update (inside es.tell, cma_es.py:90) ------------------------- */
 
-/* dC_out_dev[n][n] = sum_{i < lambda_local} w_dev[i] * y_i y_i^T with Y_dev[lambda_local][n]
- * row-major (y_i = (x_i - m_old)/sigma, already sorted/weighted by the caller).  Full symmetric
- * matrix is written.  fp32 FFMA with fp32 accumulation per k-panel. */
-DES_API int des_cma_rank_mu(float *dC_out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local,
-                    int64_t n, void *stream);
+/* dC = sum_{i < lambda_local} w_dev[i] * y_i y_i^T with Y_dev[lambda_local][n] row-major (y_i = (x_i - m_old)/sigma,
+ * already sorted/weighted by the caller), written to out_dev as the full symmetric [n][n] matrix (packed == 0) or as
+ * packed upper-triangular tiles (packed != 0, layout below).  lambda_local == 0 writes zeros.  The library picks the
+ * kernel from n: below 2048 fp32 FFMA (fp32 accumulation per k-panel); from 2048 on the tensor cores
+ * (csrc/des_cma_tc.cu: dC = Zs^T Z with Z = diag(sqrt|w|) Y, operands split into fp16 hi + lo, three wgmma MMAs per
+ * k-step, fp32 accumulation, TMA-fed; |sqrt|w_k| * y| must stay below 65504).  Both stay within 1e-5 of the fp64
+ * restatement in both norms.  workspace: des_cma_rank_mu_workspace_bytes(n, lambda_local) bytes (0 where the FFMA
+ * kernel runs: workspace_dev may then be NULL), or DES_ERR_WORKSPACE. */
+DES_API size_t des_cma_rank_mu_workspace_bytes(int64_t n, int64_t lambda_local);
+DES_API int des_cma_rank_mu(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
+                            int packed, void *workspace_dev, size_t workspace_bytes, void *stream);
 
 /* C <- decay*C + c1 * pc pc^T + cmu * dC   (decay = 1 - c1 - cmu*sum(w) [+ (1-hsig) term folded in by
  * the caller]).  pc_dev may be NULL (then no rank-one term).  In place on C_dev[n][n]. */
 DES_API int des_cma_cov_apply(float *C_dev, const float *dC_dev, const float *pc_dev, int64_t n, double decay,
                       double c1, double cmu, void *stream);
 
-/* The same two steps with the rank-mu partial kept as PACKED upper-triangular tiles — the payload to all-reduce across
- * ranks when lambda is sharded (half the bytes of the [n][n] matrix; SURVEY 8e).  Layout: tiles (bi <= bj) in row-major
- * order of (bi, bj), each [tile][tile] row-major with tile = 64 (n <= 2048) or 128; entries beyond n are zero.
- * des_cma_packed_elems(n) floats.  des_cma_cov_apply_packed mirrors the tiles while applying them (diagonal tiles take the
- * j >= i entry for both sides: C stays exactly symmetric). */
+/* The covariance update with the rank-mu partial kept as PACKED upper-triangular tiles (des_cma_rank_mu, packed != 0) —
+ * the payload to all-reduce across ranks when lambda is sharded (half the bytes of the [n][n] matrix; SURVEY 8e).
+ * Layout: tiles (bi <= bj) in row-major order of (bi, bj), each [tile][tile] row-major with tile = 64 (n <= 2048) or
+ * 128; entries beyond n are zero.  des_cma_packed_elems(n) floats.  des_cma_cov_apply_packed mirrors the tiles while
+ * applying them (diagonal tiles take the j >= i entry for both sides: C stays exactly symmetric). */
 DES_API int64_t des_cma_packed_elems(int64_t n);
-DES_API int des_cma_rank_mu_packed(float *tiles_out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local,
-                                   int64_t n, void *stream);
 DES_API int des_cma_cov_apply_packed(float *C_dev, const float *tiles_dev, const float *pc_dev, int64_t n, double decay,
                                      double c1, double cmu, void *stream);
-
-/* The rank-mu term on the tensor cores (csrc/des_cma_tc.cu): dC = Zs^T Z with Z = diag(sqrt|w|) Y, operands split into
- * fp16 hi + lo (three wgmma MMAs per k-step, fp32 accumulation, TMA-fed) — same result contract as des_cma_rank_mu
- * (packed == 0: full symmetric [n][n]) / des_cma_rank_mu_packed (packed != 0), within 1e-5 of the fp64 restatement in both
- * norms.  Needs des_cma_tc_workspace_bytes(n, lambda_local) bytes of workspace; |sqrt|w_k| * y| must stay below 65504. */
-DES_API size_t des_cma_tc_workspace_bytes(int64_t n, int64_t lambda_local);
-DES_API int des_cma_rank_mu_tc(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
-                               int packed, void *workspace_dev, size_t workspace_bytes, void *stream);
 
 /* ---- exchange steps of a sharded generation over peer memory (NVLink) ------------------------- */
 

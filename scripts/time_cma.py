@@ -1,10 +1,10 @@
-"""Time the CMA rank-mu kernels (BASELINE configs[2] and [4] shapes) with CUDA events."""
+"""Time the CMA rank-mu kernels (BASELINE configs[2] and [4] shapes, and both sides of ops.CMA_TC_MIN_N) with CUDA events."""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from distributedes_b200 import ops
 out = []
-for n, lam in [(1024, 256), (4096, 1024), (4096, 128)]:
+for n, lam in [(1024, 256), (2047, 256), (2048, 256), (4096, 1024), (4096, 128)]:   # FFMA below n = 2048, tensor cores from it
     Y = torch.randn(lam, n, device='cuda'); w = torch.rand(lam, device='cuda'); C = torch.eye(n, device='cuda'); pc = torch.randn(n, device='cuda')
     dC = ops.cma_rank_mu(Y, w)
     for _ in range(3):
@@ -20,17 +20,3 @@ for n, lam in [(1024, 256), (4096, 1024), (4096, 128)]:
     out.append(dict(n=n, lam=lam, rank_mu_ms=t1, rank_mu_tflops=2 * lam * n * n / t1 / 1e9, cov_apply_ms=t2,
                     cov_apply_gbs=12 * n * n / t2 / 1e6))
 print(json.dumps(out))
-# tensor-core path against the FFMA path
-res = []
-for n, lam in [(1024, 256), (4096, 1024), (4096, 128)]:
-    Y = torch.randn(lam, n, device='cuda'); w = torch.rand(lam, device='cuda')
-    for path in ('ffma', 'tc'):
-        dC = ops.cma_rank_mu(Y, w, path=path)
-        for _ in range(3): ops.cma_rank_mu(Y, w, out=dC, path=path)
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ev[0].record()
-        for _ in range(20): ops.cma_rank_mu(Y, w, out=dC, path=path)
-        ev[1].record(); torch.cuda.synchronize()
-        t = ev[0].elapsed_time(ev[1]) / 20
-        res.append(dict(n=n, lam=lam, path=path, ms=round(t, 4), tflops_counted=round(2 * lam * n * n / t / 1e9, 1)))
-print(json.dumps(res))

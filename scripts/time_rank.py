@@ -5,7 +5,9 @@ import torch
 from distributedes_b200 import ops
 res = []
 flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')
-for N, n in [(65536, 65536), (65536, 8192), (16384, 16384), (16384, 8192), (4096, 4096), (262144, 262144)]:
+# N <= 2048 takes the counting rank, larger populations the bucketed one
+for N, n in [(256, 256), (2048, 2048), (2048, 1024), (65536, 65536), (65536, 8192), (16384, 16384), (16384, 8192), (4096, 4096),
+             (262144, 262144)]:
     f = torch.randn(N, device='cuda')
     ws = ops.rank_workspace(n, 'cuda', N); out = torch.empty(n, device='cuda')
     for _ in range(3): ops.centered_rank(f, 0, n, workspace=ws, out=out)

@@ -22,7 +22,7 @@ def state_advance(state, beta1=0.9, beta2=0.999):
     state[3] *= beta2
 
 
-def rank_workspace(n_local, device, N=None):
+def rank_workspace(n_local, device, N):
     return torch.empty(0)
 
 
@@ -147,3 +147,21 @@ def cma_cov_apply(Cmat, dC, pc, *, decay, c1, cmu):
     new = decay * Cmat.numpy().astype(np.float64) + c1 * np.outer(p, p) + cmu * dC.numpy().astype(np.float64)
     Cmat.copy_(torch.from_numpy(new.astype(np.float32)))
     return Cmat
+
+
+# the "packed" payload of the stand-ins is the flattened full matrix: only these functions read it
+def cma_packed_elems(n):
+    return n * n
+
+
+def cma_rank_mu_packed(Y, w, out=None):
+    res = cma_rank_mu(Y, w).reshape(-1)
+    if out is None:
+        return res
+    out.copy_(res)
+    return out
+
+
+def cma_cov_apply_packed(Cmat, tiles, pc, *, decay, c1, cmu):
+    n = Cmat.shape[0]
+    return cma_cov_apply(Cmat, tiles.reshape(n, n), pc, decay=decay, c1=c1, cmu=cmu)

@@ -53,12 +53,18 @@ def test_struct_layouts_match_header(lib):
     assert C.sizeof(_lib.Dims) == 16 and C.sizeof(_lib.Opt) == 48 and C.sizeof(_lib.State) == 32
 
 
-def test_pure_functions_without_gpu(lib):
+def test_pure_functions_and_workspace_sizes_without_gpu(lib):
     assert lib.des_param_count(3, 64, 1) == 4481          # SURVEY table, confirmed on StandardFCNet(3,1,64)
     assert lib.des_param_count(24, 64, 4) == 6020
     assert lib.des_param_count(24, 256, 4) == 73220
     assert lib.des_param_count(0, 64, 1) < 0
-    assert lib.des_rank_workspace_bytes(1000) == 4000
+    assert lib.des_rank_workspace_bytes(2048, 1000) == 4000            # counting rank: one int32 count per member
+    assert lib.des_rank_workspace_bytes(4096, 16) > 3 * 4096 * 4       # bucketed rank: keys and grouped keys/indices of all N
+    # the rank-mu kernel is picked from n alone: only the tensor-core shapes need a workspace
+    from distributedes_b200 import ops
+    assert ops.CMA_TC_MIN_N == 2048
+    assert lib.des_cma_rank_mu_workspace_bytes(2047, 64) == 0 < lib.des_cma_rank_mu_workspace_bytes(2048, 64)
+    assert lib.des_cma_rank_mu_workspace_bytes(4096, 0) == 0
     assert lib.des_grad_workspace_bytes(0, 10) == 0
     assert lib.des_grad_workspace_bytes(4096, 6020) >= 6020 * 4
     assert b'sm_90a' in lib.des_version()
@@ -76,6 +82,13 @@ def test_argument_validation_precedes_cuda(lib):
     assert rc == -1 and b'NULL' in lib.des_last_error()
     rc = lib.des_nes_grad_partial(None, None, 4, 10, 0, 0, None, 0, None, 0, None)
     assert rc == -1
+    # a short workspace is DES_ERR_WORKSPACE, never a quiet switch to another kernel (dummy pointers: nothing is launched)
+    dummy = C.c_void_p(256)
+    short = lib.des_rank_workspace_bytes(2048, 4096)                   # what the counting rank would need
+    rc = lib.des_centered_rank(dummy, None, dummy, 4096, 0, 4096, dummy, short, None)
+    assert rc == -4 and b'workspace' in lib.des_last_error()
+    rc = lib.des_cma_rank_mu(dummy, dummy, dummy, 64, 2048, 0, None, 0, None)
+    assert rc == -4 and b'workspace' in lib.des_last_error()
     sess = C.c_void_p()
     theta = (C.c_float * 4481)()
     rc = lib.des_session_create(C.byref(sess), 0, _lib.Dims(3, 64, 1, 8), 1, 0, 1, _lib.Opt(0.1, 0.1, 0.005, 0.9, 0.999, 1e-8),
@@ -148,7 +161,7 @@ def test_config_surface_matches_reference_attributes():
     assert (b.state_dim, b.action_dim, len(b.initial_weight)) == (24, 4, 6020)
 
 
-def test_closed_loop_config_and_validation_without_gpu(lib):
+def test_closed_loop_config_and_packed_cma_validation_without_gpu(lib):
     """ClosedLoopPendulumConfig keeps the reference's PendulumConfig values (config.py:8-9, 26-31); the device environment
     has no host-side step; des_rollout_eval / the packed CMA entry points validate their arguments before touching CUDA."""
     from distributedes_b200 import _lib
@@ -173,7 +186,7 @@ def test_closed_loop_config_and_validation_without_gpu(lib):
     assert lib.des_cma_packed_elems(1024) == 16 * 17 // 2 * 64 * 64
     assert lib.des_cma_packed_elems(4096) == 32 * 33 // 2 * 128 * 128
     assert lib.des_cma_packed_elems(300) == 5 * 6 // 2 * 64 * 64 and lib.des_cma_packed_elems(0) == 0
-    assert lib.des_cma_rank_mu_packed(None, None, None, 4, 16, None) == -1
+    assert lib.des_cma_rank_mu(None, None, None, 4, 16, 1, None, 0, None) == -1
     assert lib.des_cma_cov_apply_packed(None, None, None, 16, 1.0, 0.0, 0.0, None) == -1
 
 

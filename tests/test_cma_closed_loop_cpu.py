@@ -136,9 +136,10 @@ def _train_worker(rank, world, port, outdir):
 
 
 @pytest.mark.parametrize('world,port', [(2, 29713), (3, 29727)])
-def test_cma_train_closed_loop_sharded_reproduces_the_reference_golden(world, port):
+def test_cma_train_closed_loop_sharded_packed_reproduces_the_reference_golden(world, port):
     """cma_es.train(ClosedLoopPendulumConfig(16)) on gloo ranks (8 + 8 members, and the ragged 6 + 5 + 5): every rank returns
-    the same triple and holds the same strategy state, equal to the reference's verbatim run."""
+    the same triple and holds the same strategy state, equal to the reference's verbatim run.  tell() all-reduces the
+    rank-mu partials in the packed form sharded GPU runs use."""
     g = np.load(GOLD)
     with tempfile.TemporaryDirectory() as outdir:
         mp.spawn(_train_worker, args=(world, port, outdir), nprocs=world, join=True)

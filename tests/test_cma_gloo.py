@@ -1,5 +1,5 @@
 """world_size=2 on CPU with gloo: cma_es.CMAEvolutionStrategy sharded over the ranks (members split, z regenerated per
-shard, all-reduce of the [n,n] rank-mu partials and of sum_i w_i y_i) must reproduce the single-process fp64 restatement
+shard, all-reduce of the packed rank-mu partials — the sharded path the GPUs run — and of sum_i w_i y_i) must reproduce the single-process fp64 restatement
 (oracle/cma_oracle.CMAState) given the same counter noise."""
 import os
 import sys
@@ -37,7 +37,7 @@ def _worker(rank, world, port, outdir):
         dist.destroy_process_group()
 
 
-def test_sharded_cma_equals_single_process_restatement():
+def test_sharded_cma_with_packed_partials_equals_single_process_restatement():
     from oracle import cma_oracle as cma
     from oracle import nes_oracle as orc
     with tempfile.TemporaryDirectory() as outdir:

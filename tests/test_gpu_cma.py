@@ -131,7 +131,7 @@ def test_pop_eval_and_cma_train_surface():
 
 @pytest.mark.parametrize('n,lam', [(300, 40), (1024, 64), (2500, 24), (4096, 16)])
 def test_packed_rank_mu_and_apply_equal_the_full_matrix_path(n, lam):
-    """des_cma_rank_mu_packed + des_cma_cov_apply_packed (the sharded runs' path: the all-reduce payload is the packed
+    """des_cma_rank_mu(packed) + des_cma_cov_apply_packed (the sharded runs' path: the all-reduce payload is the packed
     upper triangle) produce exactly the C of des_cma_rank_mu + des_cma_cov_apply, and C stays exactly symmetric."""
     from distributedes_b200 import ops
     g = torch.Generator(device='cpu').manual_seed(n)
@@ -154,10 +154,11 @@ def test_packed_rank_mu_and_apply_equal_the_full_matrix_path(n, lam):
     assert torch.equal(C3, C3.T)
 
 
-@pytest.mark.parametrize('n,lam', [(256, 64), (1000, 130), (2048, 8), (4096, 128)])
-def test_tensor_core_rank_mu_agrees_with_the_ffma_kernel(n, lam):
-    """des_cma_rank_mu_tc (split-fp16 wgmma SYRK, TMA-fed) against des_cma_rank_mu (fp32 FFMA) and the fp64 restatement,
-    signed weights, ragged sizes; full and packed outputs carry the same numbers."""
+@pytest.mark.parametrize('n,lam', [(2048, 8), (2049, 37), (2500, 130), (4096, 128),       # tensor cores (n >= 2048)
+                                   (256, 64), (1000, 130), (2047, 9)])                    # fp32 FFMA (n < 2048)
+def test_rank_mu_kernel_picked_by_n_matches_restatement(n, lam):
+    """Each rank-mu kernel, reached through its own shapes (split-fp16 wgmma SYRK for n >= 2048, fp32 FFMA below), against
+    the fp64 restatement: signed weights, ragged sizes; full and packed outputs carry the same numbers."""
     from distributedes_b200 import ops
     rs = np.random.RandomState(n * 7 + lam)
     Y = rs.randn(lam, n) * (1 + rs.rand(n))                       # columns of different scale
@@ -166,18 +167,16 @@ def test_tensor_core_rank_mu_agrees_with_the_ffma_kernel(n, lam):
     ref = cma.rank_mu_delta(Y, w)
     Yt = torch.from_numpy(Y.astype(np.float32)).to(DEV)
     wt = torch.from_numpy(w.astype(np.float32)).to(DEV)
-    tcm = ops.cma_rank_mu(Yt, wt, path='tc')
-    ffm = ops.cma_rank_mu(Yt, wt, path='ffma')
-    got = tcm.cpu().numpy()
+    full = ops.cma_rank_mu(Yt, wt)
+    got = full.cpu().numpy()
     assert np.array_equal(got, got.T)
     ref32 = cma.rank_mu_delta(Yt.cpu().numpy().astype(np.float64), wt.cpu().numpy().astype(np.float64))   # same fp32 inputs
     both_norms(got, ref32)
-    both_norms(ffm.cpu().numpy(), ref32)
     both_norms(got, ref, tol=2e-5)                                 # + the fp32 rounding of the inputs themselves
     # packed tiles hold exactly the full matrix's upper entries
-    tiles = ops.cma_rank_mu_packed(Yt, wt, path='tc')
+    tiles = ops.cma_rank_mu_packed(Yt, wt)
     C1 = torch.zeros((n, n), device=DEV)
     C2 = torch.zeros((n, n), device=DEV)
-    ops.cma_cov_apply(C1, tcm, None, decay=0.0, c1=0.0, cmu=1.0)
+    ops.cma_cov_apply(C1, full, None, decay=0.0, c1=0.0, cmu=1.0)
     ops.cma_cov_apply_packed(C2, tiles, None, decay=0.0, c1=0.0, cmu=1.0)
     assert torch.equal(C1, C2)
