@@ -48,6 +48,8 @@ SIGNATURES = {
     'des_rollout_eval_solutions': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _P,
                                              C.c_size_t, _P]),
     'des_obs_stats_merge_totals': (C.c_int, [_P, _P, _I32, _P]),
+    'des_policy_act': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _I64, _P]),
+    'des_obs_parts_reduce': (C.c_int, [_P, _P, _I64, _I32, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_pop_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _I64, _P]),

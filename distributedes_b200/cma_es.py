@@ -189,8 +189,24 @@ class Worker:
         else:
             self.device = torch.device(device if device is not None else 'cpu')
         self.kn = kernels
-        self.closed_loop = bool(getattr(config, 'closed_loop', False))
-        if self.closed_loop:
+        self.host_env = bool(getattr(config, 'host_env', False))
+        self.closed_loop = bool(getattr(config, 'closed_loop', False)) or self.host_env
+        if self.host_env:
+            # environments stepped on the host, the solutions' policy step on the device (engine.HostEpisodes)
+            self.d0, self.A, self.T = int(config.state_dim), int(config.action_dim), 0
+            self.normalize_obs = bool(getattr(config, 'normalize_obs', True))
+            self.obs_stats = (torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device)
+                              if self.normalize_obs else None)
+            self.obs_totals = torch.zeros(2 * self.d0 + 1, dtype=torch.float64, device=self.device)
+            batch_env_fn = getattr(config, 'batch_env_fn', None)
+            if batch_env_fn is None:
+                from .envs import GymEnvBatch
+                batch_env_fn = lambda B: GymEnvBatch(config.env_fn, B, getattr(config, 'seed', 0))     # noqa: E731
+            self.batch_env_fn = batch_env_fn
+            self._episodes = {}           # (members, repetitions) -> engine.HostEpisodes
+            self.steps_taken = 0          # environment steps of the last run() on this rank
+            self.tests_run = 0
+        elif self.closed_loop:
             from .engine import RolloutEngine
             if config.task not in RolloutEngine.ENVS:
                 raise ValueError('closed-loop environments available on the device: %s (got %r)'
@@ -215,6 +231,8 @@ class Worker:
         if not self.closed_loop:
             fit = self.kn.pop_eval(solutions, self.obs, self.target, hidden=self.config.hidden_size, clip=self.config.clip)
             return -fit
+        if self.host_env:
+            return self._run_host(solutions, member_offset, generation)
         c = self.config
         n_local = int(solutions.shape[0])
         self.obs_totals.zero_()
@@ -230,10 +248,51 @@ class Worker:
                                            workspace=self.roll_ws, out=fit)
         return -fit
 
+    def _host_episodes(self, n, reps):
+        ep = self._episodes.get((n, reps))
+        if ep is None:
+            from .engine import HostEpisodes
+            c = self.config
+            ep = HostEpisodes(self.kn, self.device, self.batch_env_fn(n * reps), n, reps, self.d0, c.hidden_size,
+                              self.A, c.clip, c.action_noise_std, getattr(c, 'seed', 0))
+            self._episodes[(n, reps)] = ep
+        return ep
+
+    def _run_host(self, solutions, member_offset, generation):
+        c = self.config
+        n_local = int(solutions.shape[0])
+        self.obs_totals.zero_()
+        fit = torch.zeros(n_local, dtype=torch.float32, device=self.device)
+        self.steps_taken = 0
+        if n_local:
+            rows = solutions.to(device=self.device, dtype=torch.float32).contiguous()
+            part = (torch.zeros((n_local, 2 * self.d0 + 1), dtype=torch.float64, device=self.device)
+                    if self.normalize_obs else None)
+            ret, self.steps_taken = self._host_episodes(n_local, c.repetitions).run(
+                rows, generation=generation, member_offset=member_offset, obs_stats=self.obs_stats, stat_part=part)
+            fit.copy_(torch.from_numpy(ret.mean(axis=1).astype(np.float32)))
+            if part is not None:
+                self.kn.obs_parts_reduce(part, self.d0, out=self.obs_totals)
+        return -fit
+
+    def steps_over_ranks(self, es):
+        """Environment steps of the last run(), summed over ranks (cma_es.py:73 sums the episodes' real lengths)."""
+        total = torch.tensor([self.steps_taken], dtype=torch.int64, device=self.device)
+        if es.world > 1:
+            dist.all_reduce(total, group=es.pg)
+        return int(total.item())
+
     def test_returns(self, solution, repetitions):
         """Returns of `repetitions` noiseless episodes of one solution (cma_es.py:102-111) with the current statistics.
         The k-th call (k = 0 first) resets its episodes from the test stream with generation word k."""
         c = self.config
+        if self.host_env:
+            from .envs import TEST_MEMBER
+            row = solution.reshape(1, -1).to(device=self.device, dtype=torch.float32).contiguous()
+            ret, _ = self._host_episodes(1, int(repetitions)).run(row, generation=self.tests_run, key_member=TEST_MEMBER,
+                                                                 obs_stats=self.obs_stats)
+            self.tests_run += 1
+            return ret[0]
         sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
         episodes = torch.empty(int(repetitions), dtype=torch.float32, device=self.device)
         self.kn.rollout_eval(sol, env=self.env_id, hidden=c.hidden_size, horizon=self.T, repetitions=int(repetitions),
@@ -272,7 +331,10 @@ def train(config, worker=None, es=None):
     while True:
         solutions = es.ask()                                                                # :62 (this rank's shard)
         cost = es.gather_cost(worker.run(solutions, es.offset, es.gen))                     # :63-72, all lambda costs
-        total_steps += config.pop_size * config.repetitions * worker.T                      # :73
+        if getattr(worker, 'host_env', False):                                             # :73, real lengths
+            total_steps += worker.steps_over_ranks(es)
+        else:
+            total_steps += config.pop_size * config.repetitions * worker.T
         best = int(torch.argmin(cost))                                                      # :75
         elapsed_time = time.time() - initial_time
         best_solution = _fetch_member(es, solutions, best)

@@ -85,3 +85,49 @@ class BipedalWalkerConfig(SynthTapeConfig):
 
     def __init__(self, hidden_size=16, tape_len=256):
         SynthTapeConfig.__init__(self, hidden_size, 24, 4, tape_len, 1.0)
+
+
+class HostEnvConfig(BasicConfig):
+    """Any environment with the classic gym API (reset() -> obs, step(a) -> (obs, reward, done, info), optionally
+    seed(s)), stepped on the host by the user's own code, with the population's policy step on the device
+    (engine.HostEnvEngine for NES, cma_es.Worker for CMA-ES).  The reference's BasicConfig (config.py:5-21): env_fn is
+    probed for state_dim / action_dim, 10 repetitions and 10 test repetitions (config.py:8-9), the observation
+    normaliser on.  `batch_env_fn(num_slots)`, if given, builds a vectorised environment implementing the batch protocol
+    of envs.py (otherwise envs.GymEnvBatch wraps num_slots environments from env_fn)."""
+
+    def __init__(self, env_fn, hidden_size=16, clip=1.0, task=None, batch_env_fn=None):
+        if hidden_size not in (16, 32, 64, 96, 128):
+            raise ValueError('HostEnvConfig: hidden_size must be 16, 32, 64, 96 or 128 (des_policy_act); got %r'
+                             % (hidden_size,))
+        self.env_fn = env_fn
+        self.batch_env_fn = batch_env_fn
+        self.task = task if task is not None else 'host-env'
+        self.clip = float(clip)
+        self.action_clip = lambda a: np.clip(a, -self.clip, self.clip)
+        self.target = 10000
+        BasicConfig.__init__(self, hidden_size)
+        if not (1 <= self.state_dim <= 32 and 1 <= self.action_dim <= 8):
+            raise ValueError('HostEnvConfig: des_policy_act takes state_dim <= 32 and action_dim <= 8; the environment '
+                             'has %d and %d' % (self.state_dim, self.action_dim))
+        self.host_env = True
+        self.repetitions = 10         # config.py:8
+        self.test_repetitions = 10    # config.py:9
+        self.normalize_obs = True
+
+
+class GymConfig(HostEnvConfig):
+    """A gym task by name, e.g. GymConfig('BipedalWalker-v2', 64): gym.make(task) with the action clip of the
+    reference's config for that task (config.py:29, 37, 44, 51; 1 for tasks it does not list).  Needs the `gym`
+    package with the classic API; it is imported when the config is constructed."""
+
+    CLIPS = {'Pendulum-v0': 2.0, 'BipedalWalker-v2': 1.0, 'LunarLanderContinuous-v2': 1.0,
+             'BipedalWalkerHardcore-v2': 1.0}
+
+    def __init__(self, task, hidden_size=16):
+        try:
+            import gym
+        except ImportError as e:
+            raise ImportError('GymConfig(%r) needs the gym package (classic API: reset() -> obs, step(a) -> '
+                              '(obs, reward, done, info)), which is not installed; or pass any such environment '
+                              'factory to HostEnvConfig' % (task,)) from e
+        HostEnvConfig.__init__(self, lambda: gym.make(task), hidden_size, self.CLIPS.get(task, 1.0), task)

@@ -134,6 +134,16 @@ __device__ __forceinline__ float cos_approx(float x) {
     return y;
 }
 
+// tanh as 1 - 2/(1 + 2^(2x log2 e)): two MUFU + three FP32 ops, abs error ~2e-7 (fp32 rounding level of the
+// reference's torch.tanh).  40*H/32 of these per member-step make the libm tanhf a third of the instruction count.
+// Shared by the closed-loop policies: rollout_pendulum_kernel (des_envs.cu) and policy_act_kernel (des_act.cu).
+__device__ __forceinline__ float tanh_mufu(float x) {
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.8853900817779268f));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+    return __fmaf_rn(-2.0f, r, 1.0f);
+}
+
 constexpr float kTwoPiF = 6.283185307179586f;             // fl32(2*pi)
 constexpr float kAngOffF = 9.424777586262351f;            // fl32(3*pi - pi*2^-23)
 

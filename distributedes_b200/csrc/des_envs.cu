@@ -66,15 +66,6 @@ struct Pendulum {
     }
 };
 
-// tanh as 1 - 2/(1 + 2^(2x log2 e)): two MUFU + three FP32 ops, abs error ~2e-7 (fp32 rounding level of the
-// reference's torch.tanh).  40*H/32 of these per member-step make the libm tanhf a third of the instruction count.
-__device__ __forceinline__ float tanh_mufu(float x) {
-    float e, r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.8853900817779268f));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-    return __fmaf_rn(-2.0f, r, 1.0f);
-}
-
 constexpr int kEpPerLane = 5;          // episodes per lane half: 2 halves x 5 = up to 10 repetitions (config.py:8)
 constexpr int kHS = 8;                 // row stride of an h1 panel (one panel per episode half): 5 episodes + pad
 
@@ -381,6 +372,17 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
                                (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_obs_parts_reduce(double *obs_totals_out_dev, const double *parts_dev, int64_t n_local,
+                                            int32_t state_dim, void *stream) {
+    DES_REQUIRE(state_dim > 0 && state_dim <= 511 && n_local >= 0, "des_obs_parts_reduce: bad arguments");
+    DES_REQUIRE(obs_totals_out_dev && (parts_dev || n_local == 0), "des_obs_parts_reduce: NULL pointer");
+    const int width = 2 * state_dim + 1;
+    des::stat_part_reduce_kernel<<<1, (unsigned)((width + 31) / 32 * 32), 0, (cudaStream_t)stream>>>(
+        obs_totals_out_dev, parts_dev, n_local, width);
+    DES_LAUNCH_CHECK("stat_part_reduce_kernel");
+    return DES_OK;
 }
 
 extern "C" DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,

@@ -340,3 +340,178 @@ class RolloutEngine(NESEngine):
 
     def noiseless_fitness(self, solution=None):
         return float(self.test_returns(solution).mean())
+
+
+class HostEpisodes:
+    """The bridge between environments stepped on the host and the population's policy on the device: runs the episodes
+    of `n` weight rows x `repetitions` in lockstep until every slot is done (Evaluator.eval / single_run,
+    utils.py:116-139).  Per step: observations -> pinned buffer -> device, des_policy_act, actions -> host, env.step,
+    fp64 return accumulation per slot.  Slot b = i * repetitions + r of the batch environment is episode r of row i.
+
+    `batch_env` implements the protocol of envs.py (num_envs, reset(keys), step(actions, alive)); its num_envs must be
+    n * repetitions."""
+
+    def __init__(self, kernels, device, batch_env, n, repetitions, state_dim, hidden, action_dim, clip, action_noise_std,
+                 seed):
+        self.k, self.device, self.env = kernels, torch.device(device), batch_env
+        self.n, self.reps = int(n), int(repetitions)
+        self.d0, self.H, self.A = int(state_dim), int(hidden), int(action_dim)
+        self.clip, self.action_noise_std, self.seed = float(clip), float(action_noise_std), int(seed)
+        B = self.n * self.reps
+        if int(batch_env.num_envs) != B:
+            raise ValueError('the batch environment has %d slots; %d members x %d repetitions need %d'
+                             % (batch_env.num_envs, self.n, self.reps, B))
+        pin = self.device.type == 'cuda'
+        self.obs_h = torch.empty((B, self.d0), dtype=torch.float32, pin_memory=pin)
+        self.alive_h = torch.empty(B, dtype=torch.uint8, pin_memory=pin)
+        self.act_h = torch.empty((B, self.A), dtype=torch.float32, pin_memory=pin)
+        self.obs_d = torch.empty((B, self.d0), dtype=torch.float32, device=self.device)
+        self.alive_d = torch.empty(B, dtype=torch.uint8, device=self.device)
+        self.act_d = torch.empty((B, self.A), dtype=torch.float32, device=self.device)
+
+    def run(self, rows, *, generation, member_offset=0, key_member=None, obs_stats=None, stat_part=None):
+        """Returns (returns[n, repetitions] fp64, environment steps taken).  Episode (i, r) resets with the key
+        (generation, member_offset + i, r), or (generation, key_member, r) when key_member is given (test episodes,
+        whose action noise then uses member 0 as des_rollout_eval's test episodes do)."""
+        n, reps, B = self.n, self.reps, self.n * self.reps
+        if B == 0:
+            return np.zeros((n, reps)), 0
+        members = (np.full(n, int(key_member), dtype=np.int64) if key_member is not None
+                   else int(member_offset) + np.arange(n, dtype=np.int64))
+        keys = np.stack([np.full(B, int(generation) & 0xFFFFFFFF, dtype=np.int64), np.repeat(members, reps),
+                         np.tile(np.arange(reps, dtype=np.int64), n)], axis=1)
+        noise_offset = 0 if key_member is not None else int(member_offset)
+        obs = self.env.reset(keys)
+        alive = np.ones(B, dtype=bool)
+        returns = np.zeros(B, dtype=np.float64)
+        steps, t = 0, 0
+        cuda = self.device.type == 'cuda'
+        obs_h, alive_h, act_h = self.obs_h.numpy(), self.alive_h.numpy(), self.act_h.numpy()
+        while alive.any():
+            obs_h[:] = obs                                              # fp32 cast: FloatTensor(o), utils.py:42-45
+            alive_h[:] = alive
+            self.obs_d.copy_(self.obs_h, non_blocking=True)
+            self.alive_d.copy_(self.alive_h, non_blocking=True)
+            self.k.policy_act(rows, self.obs_d, self.alive_d, state_dim=self.d0, hidden=self.H, action_dim=self.A,
+                              repetitions=reps, clip=self.clip, action_noise_std=self.action_noise_std, seed=self.seed,
+                              generation=generation, member_offset=noise_offset, t=t, obs_stats=obs_stats,
+                              stat_part=stat_part, out=self.act_d)
+            self.act_h.copy_(self.act_d, non_blocking=True)
+            if cuda:
+                torch.cuda.current_stream(self.device).synchronize()
+            obs, reward, done = self.env.step(act_h, alive)
+            returns[alive] += np.asarray(reward, dtype=np.float64)[alive]      # utils.py:137
+            steps += int(alive.sum())
+            alive &= ~np.asarray(done, dtype=bool)
+            t += 1
+        return returns.reshape(n, reps), steps
+
+
+class HostEnvEngine(NESEngine):
+    """NES generation over environments stepped on the HOST by the user's own code (any gym-style task), with the
+    population's per-step policy on the device (des_policy_act): Evaluator.eval utils.py:116-124 for every member of the
+    rank's shard, `repetitions` episodes each.
+
+    Per generation: des_nes_perturb materialises the shard's rows theta + sigma*eps once; every slot resets with its key
+    (generation, global member, repetition); HostEpisodes steps until no slot is alive; fitness = mean return over the
+    repetitions (utils.py:124) into the shard of fitness_all, then the fitness all-gather.  The raw observations of the
+    alive slots accumulate per member on the device, are reduced in member order and, sharded, all-reduced (as
+    RolloutEngine).  `steps_taken` is the number of environment steps of the generation, summed over ranks
+    (natural_es.py:75).  Rank, gradient and apply are NESEngine's; the generation stays eager (the host loop is inside it).
+
+    env_fn: a single environment with the classic gym API (probed for the dimensions); batch_env_fn(num_slots), if given,
+    builds a vectorised environment implementing the batch protocol of envs.py instead of envs.GymEnvBatch."""
+
+    HIDDEN = (16, 32, 64, 96, 128)
+
+    def __init__(self, *, env_fn, hidden, pop_size, theta0, sigma, learning_rate, state_dim=None, action_dim=None,
+                 repetitions=10, test_repetitions=None, action_noise_std=0.0, normalize_obs=True, batch_env_fn=None,
+                 **kw):
+        if state_dim is None or action_dim is None:
+            probe = env_fn()
+            state_dim, action_dim = probe.observation_space.shape[0], probe.action_space.shape[0]
+        if int(hidden) not in self.HIDDEN:
+            raise ValueError('HostEnvEngine: hidden must be 16, 32, 64, 96 or 128 (des_policy_act); got %r' % (hidden,))
+        if not (1 <= int(state_dim) <= 32 and 1 <= int(action_dim) <= 8):
+            raise ValueError('HostEnvEngine: des_policy_act takes state_dim <= 32 and action_dim <= 8; got %r, %r'
+                             % (state_dim, action_dim))
+        for name, r in (('repetitions', repetitions), ('test_repetitions', test_repetitions or repetitions)):
+            if not (1 <= int(r) <= 16):
+                raise ValueError('HostEnvEngine: %s must be in [1, 16]; got %r' % (name, r))
+        self.env_fn = env_fn
+        self.action_noise_std = float(action_noise_std)
+        self.test_repetitions = int(test_repetitions or repetitions)
+        kw.pop('precision', None)
+        kw.pop('use_graph', None)
+        super().__init__(state_dim=state_dim, hidden=hidden, action_dim=action_dim, pop_size=pop_size, theta0=theta0,
+                         obs=None, target=None, sigma=sigma, learning_rate=learning_rate, precision='fp32',
+                         normalize_obs=normalize_obs, repetitions=repetitions, **kw)
+        if batch_env_fn is None:
+            from .envs import GymEnvBatch
+            batch_env_fn = lambda B: GymEnvBatch(env_fn, B, self.seed)      # noqa: E731
+        self.batch_env_fn = batch_env_fn
+        self.episodes = self._bridge(batch_env_fn(self.n_local * self.repetitions), self.n_local, self.repetitions)
+        self._test_episodes = None
+        self.steps_taken = 0
+
+    def _bridge(self, batch_env, n, reps):
+        return HostEpisodes(self.k, self.device, batch_env, n, reps, self.d0, self.H, self.A, self.clip,
+                            self.action_noise_std, self.seed)
+
+    def _setup_inputs(self, obs, target):
+        self.T = 0                   # no fixed horizon: episodes end when the environment says so
+        self.eval_ws = None
+        w = 2 * self.d0 + 1
+        self.rows = torch.empty((self.n_local, self.P), dtype=torch.float32, device=self.device)
+        self.stat_part = torch.zeros((self.n_local, w), dtype=torch.float64, device=self.device)
+        self.obs_totals = torch.zeros(w, dtype=torch.float64, device=self.device)
+
+    def set_tape(self, obs, target):
+        raise TypeError('HostEnvEngine steps its environments on the host; there is no tape to set')
+
+    def evaluate(self):
+        gen = self.generation_index
+        if self.world > 1 and self.comm is None:
+            self.fitness_all.zero_()
+        self.obs_totals.zero_()
+        steps = 0
+        if self.n_local:
+            self.k.nes_perturb(self.theta, self.n_local, self.sigma, self.seed, gen, member_offset=self.offset,
+                               out=self.rows)                                  # natural_es.py:28-30
+            self.stat_part.zero_()
+            ret, steps = self.episodes.run(self.rows, generation=gen, member_offset=self.offset,
+                                           obs_stats=self.obs_stats if self.normalize_obs else None,
+                                           stat_part=self.stat_part if self.normalize_obs else None)
+            fit = ret.mean(axis=1)                                             # -cost, utils.py:124
+            self.fitness_shard_out.copy_(torch.from_numpy(fit.astype(np.float32)))
+            if self.normalize_obs:
+                self.k.obs_parts_reduce(self.stat_part, self.d0, out=self.obs_totals)
+        self._gather_fitness()
+        total = torch.tensor([steps], dtype=torch.int64, device=self.device)
+        if self.world > 1:
+            if self.normalize_obs:
+                dist.all_reduce(self.obs_totals, group=self.pg)
+            dist.all_reduce(total, group=self.pg)
+        self.steps_taken = int(total.item())
+        return self.fitness_all
+
+    def _merge_obs_stats(self):
+        if self.normalize_obs:
+            self.k.obs_stats_merge_totals(self.obs_stats, self.obs_totals, self.d0)
+
+    def test_returns(self, solution=None, repetitions=None):
+        """Returns of `repetitions` episodes of the unperturbed solution (test(), natural_es.py:101-110) with the current
+        statistics, which they do not feed; keys (generation word, 0x40000000, repetition)."""
+        from .envs import TEST_MEMBER
+        theta = self.theta if solution is None else torch.as_tensor(
+            np.ascontiguousarray(solution, dtype=np.float32)).to(self.device)
+        reps = int(repetitions or self.test_repetitions)
+        if self._test_episodes is None or self._test_episodes.reps != reps:
+            self._test_episodes = self._bridge(self.batch_env_fn(reps), 1, reps)
+        ret, _ = self._test_episodes.run(theta.reshape(1, -1).contiguous(), generation=self.generation_index,
+                                         key_member=TEST_MEMBER,
+                                         obs_stats=self.obs_stats if self.normalize_obs else None)
+        return ret[0]
+
+    def noiseless_fitness(self, solution=None):
+        return float(self.test_returns(solution).mean())

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .engine import NESEngine, RolloutEngine
+from .engine import HostEnvEngine, NESEngine, RolloutEngine
 from .utils import Evaluator, SharedStats, StaticNormalizer, logger
 
 
@@ -41,8 +41,17 @@ class Worker:
 
 
 def build_engine(config, param=None, **kw):
-    env = config.env_fn()
     theta0 = config.initial_weight if param is None else np.asarray(param, dtype=np.float32)
+    if getattr(config, 'host_env', False):            # environments stepped on the host, policy step on the device
+        return HostEnvEngine(env_fn=config.env_fn, batch_env_fn=getattr(config, 'batch_env_fn', None),
+                             state_dim=config.state_dim, action_dim=config.action_dim, hidden=config.hidden_size,
+                             pop_size=config.pop_size, theta0=theta0, sigma=config.sigma,
+                             learning_rate=config.learning_rate, weight_decay=config.weight_decay, clip=config.clip,
+                             seed=getattr(config, 'seed', 0), beta1=config.opt.beta1, beta2=config.opt.beta2,
+                             epsilon=config.opt.epsilon, repetitions=config.repetitions,
+                             test_repetitions=config.test_repetitions, action_noise_std=config.action_noise_std,
+                             normalize_obs=getattr(config, 'normalize_obs', True), **kw)
+    env = config.env_fn()
     if getattr(config, 'closed_loop', False):         # environment stepped on the device (SURVEY 8f row 3)
         return RolloutEngine(task=config.task, hidden=config.hidden_size, pop_size=config.pop_size, theta0=theta0,
                              sigma=config.sigma, learning_rate=config.learning_rate, weight_decay=config.weight_decay,
@@ -80,7 +89,8 @@ def train(config, engine=None):
 
         worker.run()                                                           # :62-73 (evaluate + gather)
         rewards = engine.fitness_all
-        total_steps += steps_per_generation                                    # :75
+        # :75 sums the episodes' real lengths: engines that step their environments until done report them
+        total_steps += engine.steps_taken if hasattr(engine, 'steps_taken') else steps_per_generation
         r_mean = float(rewards.mean())
         r_std = float(rewards.std(unbiased=False))
         if engine.rank == 0:

@@ -85,10 +85,14 @@ def noise_fill(n_members, P, seed, generation, member_offset=0, stream_tag=0, de
     return out
 
 
-def nes_perturb(theta, n_members, sigma, seed, generation, member_offset=0):
-    """theta'[n_members, P] = fp32(theta + sigma*eps) — debug/parity op (natural_es.py:28-30)."""
+def nes_perturb(theta, n_members, sigma, seed, generation, member_offset=0, out=None):
+    """theta'[n_members, P] = fp32(theta + sigma*eps) (natural_es.py:28-30): a parity op, and the weight rows of
+    host-stepped environments (policy_act).  `out`: an optional [n_members, P] buffer."""
     P = theta.numel()
-    out = torch.empty((n_members, P), dtype=torch.float32, device=theta.device)
+    if out is None:
+        out = torch.empty((n_members, P), dtype=torch.float32, device=theta.device)
+    elif out.numel() != n_members * P:
+        raise RuntimeError('out has %d entries, need %d x %d' % (out.numel(), n_members, P))
     with _on(theta, 'theta'):
         _lib.check(_lib.load().des_nes_perturb(_ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'),
                                                n_members, P, sigma, seed, generation, member_offset, _stream()),
@@ -182,6 +186,49 @@ def obs_stats_merge_totals(stats, totals, state_dim):
                                                           _ptr(totals, torch.float64, 'totals'), int(state_dim), _stream()),
                    'des_obs_stats_merge_totals')
     return stats
+
+
+def policy_act(rows, obs, alive, *, state_dim, hidden, action_dim, repetitions, clip, action_noise_std=0.0, seed,
+               generation, member_offset=0, t, obs_stats=None, stat_part=None, out=None):
+    """One environment step of host-stepped episodes (Evaluator.single_run utils.py:128-134 minus env.step):
+    actions[n_local, repetitions, A] of rows[n_local, P] for raw obs[n_local, repetitions, d0] and alive (uint8) of the
+    same leading shape; dead slots get 0.  stat_part (fp64 [n_local, 2*d0+1]) accumulates the raw observation
+    statistics of the alive slots."""
+    if rows.dim() != 2:
+        raise RuntimeError('rows must be [n_local, P], got shape %r' % (tuple(rows.shape),))
+    n_local, P = rows.shape
+    d0, A, reps = int(state_dim), int(action_dim), int(repetitions)
+    if obs.numel() != n_local * reps * d0 or alive.numel() != n_local * reps:
+        raise RuntimeError('obs / alive have %d / %d entries, need %d x %d x %d / %d x %d'
+                           % (obs.numel(), alive.numel(), n_local, reps, d0, n_local, reps))
+    if stat_part is not None and stat_part.numel() != n_local * (2 * d0 + 1):
+        raise RuntimeError('stat_part has %d entries, need %d x %d' % (stat_part.numel(), n_local, 2 * d0 + 1))
+    if out is None:
+        out = torch.empty((n_local, reps, A), dtype=torch.float32, device=rows.device)
+    elif out.numel() != n_local * reps * A:
+        raise RuntimeError('out has %d entries, need %d x %d x %d' % (out.numel(), n_local, reps, A))
+    with _on(rows, 'rows'):
+        _lib.check(_lib.load().des_policy_act(
+            _ptr(out, torch.float32, 'out'), _ptr(stat_part, torch.float64, 'stat_part', True),
+            _ptr(rows, torch.float32, 'rows'), int(P), _ptr(obs, torch.float32, 'obs'), _ptr(alive, torch.uint8, 'alive'),
+            _ptr(obs_stats, torch.float32, 'obs_stats', True), Dims(d0, int(hidden), A, 0), reps, float(clip),
+            float(action_noise_std), int(seed), int(generation), int(member_offset), int(n_local), int(t), _stream()),
+            'des_policy_act')
+    return out
+
+
+def obs_parts_reduce(parts, state_dim, out=None):
+    """totals[2*d0+1] fp64 = sum of the stat_part rows [n_local, 2*d0+1] in member order."""
+    w = 2 * int(state_dim) + 1
+    n_local = parts.numel() // w
+    if parts.numel() != n_local * w:
+        raise RuntimeError('parts has %d entries, not a multiple of 2*d0+1 = %d' % (parts.numel(), w))
+    if out is None:
+        out = torch.empty(w, dtype=torch.float64, device=parts.device)
+    with _on(parts, 'parts'):
+        _lib.check(_lib.load().des_obs_parts_reduce(_ptr(out, torch.float64, 'out'), _ptr(parts, torch.float64, 'parts'),
+                                                    int(n_local), int(state_dim), _stream()), 'des_obs_parts_reduce')
+    return out
 
 
 def eval_workspace(state_dim, hidden, action_dim, tape_len, precision, device):

@@ -158,6 +158,45 @@ DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_re
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
 DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim, void *stream);
 
+/* ---- environments stepped on the host: the population's policy step on the device ------------------------------ */
+
+/* One environment step of n_local members x `repetitions` episodes whose environments the caller steps on the host:
+ * the part of Evaluator.single_run utils.py:126-139 that is not env.step — normalise (utils.py:128 -> 48-51), forward
+ * (utils.py:129 -> model.py:34-39), action noise (utils.py:133), clip (utils.py:134).  Launch once per step.
+ *   actions_out_dev  [n_local][repetitions][action_dim] fp32: the clipped actions; slots not alive are written as 0.
+ *   stat_part_dev    optional [n_local][2*state_dim+1] fp64, caller-zeroed before the first step: member i's row
+ *                    accumulates sum, sum of squares and count of the RAW observations of its alive slots (what the
+ *                    worker's online statistics are fed, utils.py:45), slots in repetition order within a step, steps in
+ *                    launch order.  One CTA owns a row: deterministic and shard-invariant.  Reduce the rows with
+ *                    des_obs_parts_reduce after the episode loop.  NULL = do not accumulate (test episodes).
+ *   rows_dev         [n_local][P] fp32 explicit weights, flat layout above: theta + sigma*eps from des_nes_perturb (NES,
+ *                    natural_es.py:28-30) or the solutions ask() returned (CMA-ES, cma_es.py:62).
+ *   P                row length; must equal des_param_count(state_dim, hidden, action_dim).
+ *   obs_dev          [n_local][repetitions][state_dim] fp32 raw observations as the environments returned them.
+ *   alive_dev        [n_local][repetitions] uint8, nonzero = the episode is running (required).
+ *   obs_stats_dev    optional [m|v|n] statistics: x = (o - m)/sqrtf(v + 1e-6f), o itself while n == 0 or NULL.
+ *   dims             state_dim in [1, 32], hidden in {16, 32, 64, 96, 128}, action_dim in [1, 8]; tape_len is ignored.
+ *   repetitions      [1, 16] episodes per member.
+ *   clip             actions are clipped to [-clip, clip] (config.action_clip).
+ *   action_noise_std std of the action noise (config.action_noise_std); 0 = none.  Action c of episode (m, r) at step t
+ *                    adds std * normal (c % 4) of the quad of Philox(t + (c/4)*2^31, 16 m + r, generation, stream 3)
+ *                    (noise contract above), m = member_offset + i: des_rollout_eval's action noise.
+ *   seed, generation the run's key and generation word.
+ *   member_offset    global index of row 0; member_offset + n_local <= 2^28.
+ *   t                step index within the episodes, [0, 2^31).
+ * Arithmetic: the contract of des_rollout_eval (fp32 FMA chains, the same tanh, the same summation order), so a
+ * Pendulum-v0 slot gets the action des_rollout_eval computes for the same observation and weights. */
+DES_API int des_policy_act(float *actions_out_dev, double *stat_part_dev, const float *rows_dev, int64_t P,
+                           const float *obs_dev, const uint8_t *alive_dev, const float *obs_stats_dev, des_dims dims,
+                           int32_t repetitions, double clip, double action_noise_std, uint64_t seed, uint64_t generation,
+                           int64_t member_offset, int64_t n_local, int64_t t, void *stream);
+
+/* obs_totals_out_dev [2*state_dim+1] = the sum of the n_local rows of parts_dev [n_local][2*state_dim+1] (the
+ * stat_part rows of des_policy_act), in member order: fp64, deterministic.  Sum the totals over ranks, then merge them
+ * with des_obs_stats_merge_totals (natural_es.py:85-89). */
+DES_API int des_obs_parts_reduce(double *obs_totals_out_dev, const double *parts_dev, int64_t n_local, int32_t state_dim,
+                                 void *stream);
+
 /* ---- fused sample + forward + fitness ------------------------------------------------------ */
 
 /* fitness_out_dev[i] (i < n_local) = sum_t -|| clip(pi_{theta+sigma*eps_m}(obs_t), -clip, clip) - target_t ||^2
