@@ -41,10 +41,13 @@ SIGNATURES = {
     'des_param_count': (_I64, [_I32, _I32, _I32]),
     'des_noise_fill': (C.c_int, [_P, _I64, _I64, _U64, _U64, _I64, _U32, _P]),
     'des_nes_perturb': (C.c_int, [_P, _P, _I64, _I64, _D, _U64, _U64, _I64, _P]),
+    'des_nes_perturb_mirrored': (C.c_int, [_P, _P, _I64, _I64, _D, _U64, _U64, _I64, _P]),
     'des_obs_stats_merge': (C.c_int, [_P, _P, _I32, _I32, _D, _P]),
     'des_obs_normalize': (C.c_int, [_P, _P, _P, _I32, _I32, _P]),
     'des_rollout_eval': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int,
                                    _P, C.c_size_t, _P]),
+    'des_rollout_eval_mirrored': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _D, _U64, _U64, _P, _I64, _I64,
+                                            C.c_int, _P, C.c_size_t, _P]),
     'des_rollout_eval_solutions': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _P,
                                              C.c_size_t, _P]),
     'des_obs_stats_merge_totals': (C.c_int, [_P, _P, _I32, _P]),
@@ -52,11 +55,13 @@ SIGNATURES = {
     'des_obs_parts_reduce': (C.c_int, [_P, _P, _I64, _I32, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
+    'des_nes_eval_mirrored': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_pop_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _I64, _P]),
     'des_rank_workspace_bytes': (_SZ, [_I64, _I64]),
     'des_centered_rank': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
     'des_grad_workspace_bytes': (_SZ, [_I64, _I64]),
     'des_nes_grad_partial': (C.c_int, [_P, _P, _I64, _I64, _U64, _U64, _P, _I64, _P, _SZ, _P]),
+    'des_nes_grad_partial_mirrored': (C.c_int, [_P, _P, _I64, _I64, _U64, _U64, _P, _I64, _P, _SZ, _P]),
     'des_nes_apply': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, Opt, _P, _P]),
     'des_state_init': (C.c_int, [_P, _U64, _P]),
     'des_state_advance': (C.c_int, [_P, _D, _D, _P]),

@@ -38,6 +38,7 @@ class BasicConfig:
         self.precision = 'fp32'
         self.max_generations = 0      # 0 = unbounded (stop on max_steps like the reference)
         self.normalize_obs = False    # True = the reference's StaticNormalizer/SharedStats behaviour (utils.py:37-106)
+        self.mirrored = False         # True = mirrored sampling for NES: members 2p, 2p+1 are theta +- sigma*eps_p (even pop_size)
 
 
 class SynthTapeConfig(BasicConfig):

@@ -23,11 +23,11 @@ int cuda_fail(cudaError_t e, const char *what) {
 
 int eval_ffma_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                      double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
-                     int64_t member_offset, int64_t n_local, const float *solutions, cudaStream_t st);
+                     int64_t member_offset, int64_t n_local, const float *solutions, bool mirrored, cudaStream_t st);
 int eval_tc_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                    double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
                    int64_t member_offset, int64_t n_local, int precision, void *workspace, size_t workspace_bytes,
-                   cudaStream_t st);
+                   bool mirrored, cudaStream_t st);
 size_t eval_tc_workspace_bytes(des_dims dims, int precision);
 
 }  // namespace des
@@ -64,38 +64,61 @@ extern "C" DES_API int des_pop_eval(float *fitness_out_dev, const float *solutio
     if (n_solutions == 0) return DES_OK;
     DES_REQUIRE(fitness_out_dev && solutions_dev && obs_dev && target_dev, "des_pop_eval: NULL pointer");
     return eval_ffma_launch(fitness_out_dev, solutions_dev, obs_dev, target_dev, dims, 0.0, clip, 0, 0, nullptr, 0, n_solutions,
-                            solutions_dev, (cudaStream_t)stream);
+                            solutions_dev, false, (cudaStream_t)stream);
 }
+
+namespace des {
+
+// Shared by des_nes_eval and des_nes_eval_mirrored: argument checks (before any CUDA work), then the precision's launcher.
+static int nes_eval(const char *who, float *fitness_out_dev, const float *theta_dev, const float *obs_dev,
+                    const float *target_dev, des_dims dims, double sigma, double clip, uint64_t seed, uint64_t generation,
+                    const des_state *state_dev, int64_t member_offset, int64_t n_local, int precision, void *workspace_dev,
+                    size_t workspace_bytes, bool mirrored, cudaStream_t st) {
+    DES_REQUIRE(dims.state_dim > 0 && dims.hidden > 0 && dims.action_dim > 0 && dims.tape_len > 0,
+                "%s: bad dims (d0=%d H=%d A=%d T=%d)", who, dims.state_dim, dims.hidden, dims.action_dim, dims.tape_len);
+    DES_REQUIRE(des_param_count(dims.state_dim, dims.hidden, dims.action_dim) < ((int64_t)1 << 31),
+                "%s: parameter count exceeds 2^31", who);
+    DES_REQUIRE(n_local >= 0 && n_local < ((int64_t)1 << 31), "%s: bad n_local=%lld", who, (long long)n_local);
+    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32, "%s: member index must fit 32 bits", who);
+    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0),
+                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
+                (long long)member_offset, (long long)n_local);
+    DES_REQUIRE(clip >= 0.0, "%s: clip must be >= 0", who);
+    if (n_local == 0) return DES_OK;
+    DES_REQUIRE(fitness_out_dev && theta_dev && obs_dev && target_dev, "%s: NULL pointer", who);
+    switch (precision) {
+        case DES_FWD_FP32:
+            return eval_ffma_launch(fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip, seed, generation,
+                                    state_dev, member_offset, n_local, nullptr, mirrored, st);
+        case DES_FWD_F16:
+        case DES_FWD_F16X3:
+            return eval_tc_launch(fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip, seed, generation,
+                                  state_dev, member_offset, n_local, precision, workspace_dev, workspace_bytes, mirrored, st);
+        default:
+            set_error("%s: unknown precision %d", who, precision);
+            return DES_ERR_INVALID_ARGUMENT;
+    }
+}
+
+}  // namespace des
 
 extern "C" DES_API int des_nes_eval(float *fitness_out_dev, const float *theta_dev, const float *obs_dev, const float *target_dev,
                             des_dims dims, double sigma, double clip, uint64_t seed, uint64_t generation,
                             const des_state *state_dev, int64_t member_offset, int64_t n_local, int precision,
                             void *workspace_dev, size_t workspace_bytes, void *stream) {
-    using namespace des;
-    DES_REQUIRE(dims.state_dim > 0 && dims.hidden > 0 && dims.action_dim > 0 && dims.tape_len > 0,
-                "des_nes_eval: bad dims (d0=%d H=%d A=%d T=%d)", dims.state_dim, dims.hidden, dims.action_dim,
-                dims.tape_len);
-    DES_REQUIRE(des_param_count(dims.state_dim, dims.hidden, dims.action_dim) < ((int64_t)1 << 31),
-                "des_nes_eval: parameter count exceeds 2^31");
-    DES_REQUIRE(n_local >= 0 && n_local < ((int64_t)1 << 31), "des_nes_eval: bad n_local=%lld", (long long)n_local);
-    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32,
-                "des_nes_eval: member index must fit 32 bits");
-    DES_REQUIRE(clip >= 0.0, "des_nes_eval: clip must be >= 0");
-    if (n_local == 0) return DES_OK;
-    DES_REQUIRE(fitness_out_dev && theta_dev && obs_dev && target_dev, "des_nes_eval: NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (precision) {
-        case DES_FWD_FP32:
-            return eval_ffma_launch(fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip, seed, generation,
-                                    state_dev, member_offset, n_local, nullptr, st);
-        case DES_FWD_F16:
-        case DES_FWD_F16X3:
-            return eval_tc_launch(fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip, seed, generation,
-                                  state_dev, member_offset, n_local, precision, workspace_dev, workspace_bytes, st);
-        default:
-            set_error("des_nes_eval: unknown precision %d", precision);
-            return DES_ERR_INVALID_ARGUMENT;
-    }
+    return des::nes_eval("des_nes_eval", fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip, seed,
+                         generation, state_dev, member_offset, n_local, precision, workspace_dev, workspace_bytes, false,
+                         (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_nes_eval_mirrored(float *fitness_out_dev, const float *theta_dev, const float *obs_dev,
+                                             const float *target_dev, des_dims dims, double sigma, double clip,
+                                             uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                             int64_t member_offset, int64_t n_local, int precision, void *workspace_dev,
+                                             size_t workspace_bytes, void *stream) {
+    return des::nes_eval("des_nes_eval_mirrored", fitness_out_dev, theta_dev, obs_dev, target_dev, dims, sigma, clip,
+                         seed, generation, state_dev, member_offset, n_local, precision, workspace_dev, workspace_bytes,
+                         true, (cudaStream_t)stream);
 }
 
 // ---- host-buffer session --------------------------------------------------------------------------------

@@ -34,6 +34,7 @@ struct RollArgs {
     uint64_t member_offset;
     uint32_t reset_member_base;        // counter word for the reset stream: member index (or the test-episode index)
     int noiseless;                     // 1: evaluate theta itself (test(), natural_es.py:101-110)
+    int mirrored;                      // NES mode: member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1
 };
 
 __device__ __forceinline__ double unit_open(uint32_t x) { return ((double)(x & 0x7FFFFFu) + 0.5) * (1.0 / 8388608.0); }
@@ -109,16 +110,19 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
         const float *row = a.rows + (int64_t)blockIdx.x * L.P;
         for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
     } else {
-        // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30)
+        // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30); mirrored, the noise
+        // of counter word member >> 1 with sigma negated for the odd member: fma(-sigma, eps, theta) = fp32(theta - sigma*eps)
+        const uint32_t word = a.mirrored ? member >> 1 : member;
+        const float sigma = a.mirrored && (member & 1u) ? -a.sigma : a.sigma;
         for (int q = lane; q < (L.P + 3) / 4; q += 32) {
             float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (!a.noiseless) z = noise_quad((uint32_t)q, member, gen, kStreamNesEps, a.key);
+            if (!a.noiseless) z = noise_quad((uint32_t)q, word, gen, kStreamNesEps, a.key);
             const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int j = 4 * q + e;
                 if (j >= L.P) break;
-                stage(j, __fmaf_rn(a.sigma, zz[e], __ldg(a.theta + j)));
+                stage(j, __fmaf_rn(sigma, zz[e], __ldg(a.theta + j)));
             }
         }
     }
@@ -291,8 +295,12 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                           double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
-                          void *workspace_dev, size_t workspace_bytes, cudaStream_t st) {
+                          void *workspace_dev, size_t workspace_bytes, bool mirrored, cudaStream_t st) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
+    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0 && member_offset >= 0 && n_local >= 0),
+                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
+                (long long)member_offset, (long long)n_local);
+    DES_REQUIRE(!mirrored || !noiseless, "%s: test episodes (noiseless) have no pairs; use des_rollout_eval", who);
     DES_REQUIRE(dims.state_dim == 3 && dims.action_dim == 1, "%s: Pendulum-v0 has state_dim 3, action_dim 1", who);
     DES_REQUIRE(dims.hidden == 16 || (dims.hidden > 0 && dims.hidden % 32 == 0 && dims.hidden <= kMaxRollH),
                 "%s: hidden must be 16 or a multiple of 32, <= %d (got %d)", who, kMaxRollH, dims.hidden);
@@ -313,6 +321,7 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     a.member_offset = (uint64_t)member_offset;
     a.reset_member_base = noiseless ? 0x40000000u : (uint32_t)member_offset;     // test episodes use their own reset stream
     a.noiseless = noiseless ? 1 : 0;
+    a.mirrored = mirrored ? 1 : 0;
     a.stat_part = nullptr;
     if (obs_totals_out_dev) {
         const size_t need = (size_t)n_local * 7 * sizeof(double);
@@ -359,7 +368,20 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     return des::rollout_launch("des_rollout_eval", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               (cudaStream_t)stream);
+                               false, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,
+                                                 double *obs_totals_out_dev, const float *theta_dev,
+                                                 const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
+                                                 double sigma, double clip, double action_noise_std, uint64_t seed,
+                                                 uint64_t generation, const des_state *state_dev, int64_t member_offset,
+                                                 int64_t n_local, int noiseless, void *workspace_dev, size_t workspace_bytes,
+                                                 void *stream) {
+    return des::rollout_launch("des_rollout_eval_mirrored", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
+                               theta_dev, false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
+                               generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
+                               true, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -371,7 +393,7 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
     return des::rollout_launch("des_rollout_eval_solutions", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
-                               (cudaStream_t)stream);
+                               false, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_obs_parts_reduce(double *obs_totals_out_dev, const double *parts_dev, int64_t n_local,

@@ -29,6 +29,7 @@ struct EvalArgs {
     PhiloxKey key;
     uint32_t gen;
     uint64_t member_offset;
+    int mirrored;     // member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1
 };
 
 __device__ __forceinline__ int round_up4(int x) { return (x + 3) & ~3; }
@@ -80,7 +81,9 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
     const Layout L = a.L;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
-    const uint32_t member = (uint32_t)(a.member_offset + blockIdx.x);
+    const uint64_t gm = a.member_offset + blockIdx.x;
+    const uint32_t member = (uint32_t)(a.mirrored ? gm >> 1 : gm);       // the counter word of the noise
+    const float sigma = a.mirrored && (gm & 1u) ? -a.sigma : a.sigma;    // fma(-sigma, eps, theta) = fp32(theta - sigma*eps)
     const float *wsrc = FROM_MATRIX ? a.solutions + (int64_t)blockIdx.x * L.P : a.theta;
     double fit = 0.0;                       // meaningful in thread 0 only
 
@@ -106,7 +109,7 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
                 const int R = min(kRows, Nout - n0);
                 __syncthreads();            // previous chunk's readers of Ws/bias (and obs load) done
                 if (R > 0) {
-                    gen_rows<FROM_MATRIX>(Ws, wsrc, off_w + n0 * K, R, K, Kp, S, a.sigma, member, gen, a.key);
+                    gen_rows<FROM_MATRIX>(Ws, wsrc, off_w + n0 * K, R, K, Kp, S, sigma, member, gen, a.key);
                     // biases of the chunk: off_b + n0 .. + R
                     const int ob = off_b + n0;
                     if (FROM_MATRIX) {
@@ -120,7 +123,7 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
                             for (int e = 0; e < 4; ++e) {
                                 const int local = 4 * q + e - ob;
                                 if (local >= 0 && local < R)
-                                    bias[local] = __fmaf_rn(a.sigma, zz[e], __ldg(a.theta + ob + local));
+                                    bias[local] = __fmaf_rn(sigma, zz[e], __ldg(a.theta + ob + local));
                             }
                         }
                     }
@@ -182,9 +185,10 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
 
 int eval_ffma_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                      double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
-                     int64_t member_offset, int64_t n_local, const float *solutions, cudaStream_t st) {
+                     int64_t member_offset, int64_t n_local, const float *solutions, bool mirrored, cudaStream_t st) {
     EvalArgs a;
     a.solutions = solutions;
+    a.mirrored = mirrored ? 1 : 0;
     a.fitness = fitness; a.theta = theta; a.obs = obs; a.target = target; a.state = state;
     a.L = Layout(dims.state_dim, dims.hidden, dims.action_dim);
     a.T = dims.tape_len;

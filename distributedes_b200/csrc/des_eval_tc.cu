@@ -36,6 +36,9 @@
 // mirrored to global memory (L2-resident) and copied back in the later passes, without it they are regenerated (same
 // bytes either way).
 //
+// Mirrored sampling (des_nes_eval_mirrored): eval_tc_mirrored_kernel is the same body with the producers' kMirror flag
+// set (member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1); eval_tc_kernel compiles to the plain code.
+//
 // Precision modes
 //   F16    operands rounded to fp16 (11 significant bits, as TF32), fp32 accumulate, MUFU tanh.approx.
 //   F16X3  every operand split x = hi + lo (fp16 each, ~22 bits); D += A_hi B_hi + A_lo B_hi + A_hi B_lo;
@@ -128,6 +131,21 @@ __device__ __forceinline__ float perturbed1(const float *__restrict__ theta, int
     return __fmaf_rn(sigma, zz, __ldg(theta + j));
 }
 
+// perturbed_quad of the NES stream; mirrored (kMirror): sgn = -1 for the odd member of a pair.  sigma is folded into the
+// radius through sigma^2, which loses its sign, so the radius itself is negated: fma(-r, c, theta) is exactly
+// fp32(theta - sigma*eps), and sgn = +1 gives the bits of the plain member.
+template <bool kMirror>
+__device__ __forceinline__ float4 member_quad(uint32_t q, uint32_t member, uint32_t gen, const PhiloxKey &key,
+                                              float neg2ln2_sigma2, float4 base, float sgn) {
+    if (!kMirror) return perturbed_quad(q, member, gen, kStreamNesEps, key, neg2ln2_sigma2, base);
+    const uint4 x = philox4x32(q, member, gen, kStreamNesEps, key);
+    const BmParts a = box_muller_parts(x.x, x.y, neg2ln2_sigma2, key.one_bits);
+    const BmParts b = box_muller_parts(x.z, x.w, neg2ln2_sigma2, key.one_bits);
+    const float ra = a.nr * sgn, rb = b.nr * sgn;
+    return make_float4(__fmaf_rn(ra, a.c, base.x), __fmaf_rn(ra, a.s, base.y), __fmaf_rn(rb, b.c, base.z),
+                       __fmaf_rn(rb, b.s, base.w));
+}
+
 template <bool X3>
 __device__ __forceinline__ void octet(const float (&w)[8], uint4 &hi, uint4 &lo) {
     if (X3) {
@@ -156,9 +174,10 @@ __device__ __forceinline__ void load_x(uint32_t (&xh)[2][4], uint32_t (&xl)[2][4
     }
 }
 
-// NA: compile-time bound on the action count (4 or 8) that sizes the per-thread action sums
-template <int H, bool X3, int CL, int NA>
-__global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
+// NA: compile-time bound on the action count (4 or 8) that sizes the per-thread action sums.  kMirror: mirrored
+// sampling, member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1 (producers only; the consumers are the same)
+template <int H, bool X3, int CL, int NA, bool kMirror>
+__device__ __forceinline__ void eval_tc_body(const TcArgs &a) {
     using C = TcCfg<H, X3>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -244,7 +263,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
         // this CTA's share of W2' chunk c (rows [64c, 64c + 64)) into stage `buf`; pass > 0 copies the cached image back
         constexpr int kOct = H / 8;                               // octets per row
         constexpr int kRows = 64 / CL;                            // rows of a chunk generated here
-        auto gen_chunk = [&](uint32_t member, int c, int pass, int buf) {
+        auto gen_chunk = [&](uint32_t member, float sgn, int c, int pass, int buf) {
             uint8_t *dst = w2buf + buf * C::CHUNK_BYTES;
             uint8_t *mirror = cache ? cache + (size_t)c * C::CHUNK_BYTES : nullptr;
             for (int idx = ptid; idx < kRows * kOct; idx += kProdThreads) {
@@ -257,10 +276,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                     else lo = hi;
                 } else {
                     const int j0 = L.off_w2 + (c * 64 + rr) * H + o * 8;
-                    const float4 p0 = perturbed_quad((uint32_t)(j0 >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                                     __ldg(reinterpret_cast<const float4 *>(a.theta + j0)));
-                    const float4 p1 = perturbed_quad((uint32_t)(j0 >> 2) + 1, member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                                     __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4)));
+                    const float4 p0 = member_quad<kMirror>((uint32_t)(j0 >> 2), member, gen, a.key, a.neg2ln2_sigma2,
+                                                           __ldg(reinterpret_cast<const float4 *>(a.theta + j0)), sgn);
+                    const float4 p1 = member_quad<kMirror>((uint32_t)(j0 >> 2) + 1, member, gen, a.key, a.neg2ln2_sigma2,
+                                                           __ldg(reinterpret_cast<const float4 *>(a.theta + j0 + 4)), sgn);
                     const float w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
                     octet<X3>(w, hi, lo);
                     if (mirror) {       // the same thread reads exactly these bytes back in the later passes
@@ -275,16 +294,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
         uint32_t q = 0;                                           // running W2' chunk counter, as in the consumers
         int i = 0;
         for (int64_t m = first; m < a.n_local; m += stride, ++i) {
-            const uint32_t member = (uint32_t)(a.member_offset + (uint64_t)m);
+            // the counter word of the noise and, mirrored, the sign of the pair member
+            const uint32_t member = kMirror ? (uint32_t)((a.member_offset + (uint64_t)m) >> 1)
+                                            : (uint32_t)(a.member_offset + (uint64_t)m);
+            const float sgn = kMirror && ((a.member_offset + (uint64_t)m) & 1u) ? -1.0f : 1.0f;
             // ---- small fp32 arrays (whole, in every CTA) into buffer i & 1: b1 | b2 | W3[8][H] | b3[8]
             float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
             if (i >= 2) mbar_wait(bar(C::BAR_SMALL_EMPTY + (i & 1)), ((i >> 1) - 1) & 1);
             DES_TRACE(TR_WAIT);
             for (int k = ptid; k < H / 4; k += kProdThreads) {
-                const float4 v1 = perturbed_quad((uint32_t)((L.off_b1 >> 2) + k), member, gen, kStreamNesEps, a.key,
-                                                 a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + k));
-                const float4 v2 = perturbed_quad((uint32_t)((L.off_b2 >> 2) + k), member, gen, kStreamNesEps, a.key,
-                                                 a.neg2ln2_sigma2, __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + k));
+                const float4 v1 = member_quad<kMirror>((uint32_t)((L.off_b1 >> 2) + k), member, gen, a.key, a.neg2ln2_sigma2,
+                                                       __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b1) + k), sgn);
+                const float4 v2 = member_quad<kMirror>((uint32_t)((L.off_b2 >> 2) + k), member, gen, a.key, a.neg2ln2_sigma2,
+                                                       __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_b2) + k), sgn);
                 // the f16x3 epilogue evaluates tanh(v + b) as 1 - 2/(1 + 2^(v*c + b*c)), c = 2 log2 e: store b*c
                 const float bsc = X3 ? kTwoLog2e : 1.0f;
                 reinterpret_cast<float4 *>(small)[k] = make_float4(v1.x * bsc, v1.y * bsc, v1.z * bsc, v1.w * bsc);
@@ -292,11 +314,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
             }
             for (int k = ptid; k < L.A * H / 4; k += kProdThreads)             // W3' [q][n] row-major: aligned quads
                 reinterpret_cast<float4 *>(small + 2 * H)[k] =
-                    perturbed_quad((uint32_t)((L.off_w3 >> 2) + k), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                   __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + k));
+                    member_quad<kMirror>((uint32_t)((L.off_w3 >> 2) + k), member, gen, a.key, a.neg2ln2_sigma2,
+                                         __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + k), sgn);
             for (int k = L.A * H + ptid; k < H * kMaxA; k += kProdThreads) small[2 * H + k] = 0.f;   // unused action rows
             if (ptid < kMaxA)
-                small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, a.sigma, member, gen, a.key) : 0.f;
+                small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, kMirror ? sgn * a.sigma : a.sigma, member, gen, a.key) : 0.f;
             // ---- W1' (this CTA's half of the rows in a cluster), once every consumer has run member i-1's layer 1
             DES_TRACE(TR_GEN);
             if (i >= 1) mbar_wait(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
@@ -311,8 +333,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                         if (k < L.d0) {
                             const int j = L.off_w1 + n * L.d0 + k;
-                            v = perturbed_quad((uint32_t)(j >> 2), member, gen, kStreamNesEps, a.key, a.neg2ln2_sigma2,
-                                               __ldg(reinterpret_cast<const float4 *>(a.theta + j)));
+                            v = member_quad<kMirror>((uint32_t)(j >> 2), member, gen, a.key, a.neg2ln2_sigma2,
+                                                     __ldg(reinterpret_cast<const float4 *>(a.theta + j)), sgn);
                         }
                         w[4 * hq] = v.x; w[4 * hq + 1] = v.y; w[4 * hq + 2] = v.z; w[4 * hq + 3] = v.w;
                     }
@@ -320,7 +342,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
                         const int k = c8 * 8 + e;
-                        w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, a.sigma, member, gen, a.key) : 0.f;
+                        w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, kMirror ? sgn * a.sigma : a.sigma, member, gen, a.key) : 0.f;
                     }
                 }
                 uint4 hi, lo;
@@ -336,7 +358,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
                     const int s = (int)(q & 1u);
                     if (q >= 2) mbar_wait(bar(C::BAR_W2_EMPTY + s), ((q >> 1) - 1) & 1u);
                     DES_TRACE(TR_WAIT);
-                    gen_chunk(member, c, pass, s);
+                    gen_chunk(member, sgn, c, pass, s);
                     DES_TRACE(TR_GEN);
                     publish(C::BAR_W2_FULL + s, smem_u32(w2buf + s * C::CHUNK_BYTES), kW2Copy, kW2Copies, 8192);
                     DES_TRACE(TR_SYNC);
@@ -520,13 +542,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) {
 }
 
 template <int H, bool X3, int CL, int NA>
+__global__ void __launch_bounds__(kTcThreads, 1) eval_tc_kernel(TcArgs a) { eval_tc_body<H, X3, CL, NA, false>(a); }
+
+template <int H, bool X3, int CL, int NA>
+__global__ void __launch_bounds__(kTcThreads, 1) eval_tc_mirrored_kernel(TcArgs a) { eval_tc_body<H, X3, CL, NA, true>(a); }
+
+template <int H, bool X3, int CL, int NA, bool kMirror>
 static int launch_tc(TcArgs &a, cudaStream_t st) {
     using C = TcCfg<H, X3>;
+    const auto kernel = kMirror ? eval_tc_mirrored_kernel<H, X3, CL, NA> : eval_tc_kernel<H, X3, CL, NA>;
     a.n_pass = a.T / 128 / CL;
     int dev = 0, sms = 132;
     DES_CUDA(cudaGetDevice(&dev));
     DES_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    DES_CUDA(cudaFuncSetAttribute(eval_tc_kernel<H, X3, CL, NA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    DES_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     if (CL == 2) {
         // each cluster accumulates its two halves into the output with atomicAdd: zero it first
         DES_CUDA(cudaMemsetAsync(a.fitness, 0, (size_t)a.n_local * sizeof(float), st));
@@ -543,20 +572,25 @@ static int launch_tc(TcArgs &a, cudaStream_t st) {
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        DES_CUDA(cudaLaunchKernelEx(&cfg, eval_tc_kernel<H, X3, CL, NA>, a));
+        DES_CUDA(cudaLaunchKernelEx(&cfg, kernel, a));
     } else {
         const int64_t grid = a.n_local < sms ? a.n_local : sms;
-        eval_tc_kernel<H, X3, CL, NA><<<(unsigned)grid, kTcThreads, C::SMEM, st>>>(a);
+        kernel<<<(unsigned)grid, kTcThreads, C::SMEM, st>>>(a);
     }
     DES_LAUNCH_CHECK("eval_tc_kernel");
     return DES_OK;
 }
 
-template <int H, bool X3>
-static int launch_tc_h(TcArgs &a, cudaStream_t st) {
+template <int H, bool X3, bool kMirror>
+static int launch_tc_m(TcArgs &a, cudaStream_t st) {
     const bool even = (a.T / 128) % 2 == 0;
-    if (a.L.A <= 4) return even ? launch_tc<H, X3, 2, 4>(a, st) : launch_tc<H, X3, 1, 4>(a, st);
-    return even ? launch_tc<H, X3, 2, kMaxA>(a, st) : launch_tc<H, X3, 1, kMaxA>(a, st);
+    if (a.L.A <= 4) return even ? launch_tc<H, X3, 2, 4, kMirror>(a, st) : launch_tc<H, X3, 1, 4, kMirror>(a, st);
+    return even ? launch_tc<H, X3, 2, kMaxA, kMirror>(a, st) : launch_tc<H, X3, 1, kMaxA, kMirror>(a, st);
+}
+
+template <int H, bool X3>
+static int launch_tc_h(TcArgs &a, bool mirrored, cudaStream_t st) {
+    return mirrored ? launch_tc_m<H, X3, true>(a, st) : launch_tc_m<H, X3, false>(a, st);
 }
 
 static int tc_passes(int T) { const int tiles = T / 128; return tiles % 2 == 0 ? tiles / 2 : tiles; }
@@ -576,7 +610,7 @@ size_t eval_tc_workspace_bytes(des_dims dims, int precision) {
 int eval_tc_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                    double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
                    int64_t member_offset, int64_t n_local, int precision, void *workspace, size_t workspace_bytes,
-                   cudaStream_t st) {
+                   bool mirrored, cudaStream_t st) {
     const int H = dims.hidden;
     if (!(H == 64 || H == 128 || H == 256) || dims.state_dim > kK1 || dims.action_dim > kMaxA || dims.tape_len % 128 != 0) {
         set_error("des_nes_eval(tensor): needs hidden in {64,128,256}, state_dim <= %d, action_dim <= %d, tape_len %% 128 == 0 "
@@ -600,9 +634,9 @@ int eval_tc_launch(float *fitness, const float *theta, const float *obs, const f
     const size_t need = eval_tc_workspace_bytes(dims, precision);
     a.cache = (need > 0 && workspace && workspace_bytes >= need && ((uintptr_t)workspace & 15) == 0) ? (uint8_t *)workspace : nullptr;
     switch (H) {
-        case 64: return x3 ? launch_tc_h<64, true>(a, st) : launch_tc_h<64, false>(a, st);
-        case 128: return x3 ? launch_tc_h<128, true>(a, st) : launch_tc_h<128, false>(a, st);
-        default: return x3 ? launch_tc_h<256, true>(a, st) : launch_tc_h<256, false>(a, st);
+        case 64: return x3 ? launch_tc_h<64, true>(a, mirrored, st) : launch_tc_h<64, false>(a, mirrored, st);
+        case 128: return x3 ? launch_tc_h<128, true>(a, mirrored, st) : launch_tc_h<128, false>(a, mirrored, st);
+        default: return x3 ? launch_tc_h<256, true>(a, mirrored, st) : launch_tc_h<256, false>(a, mirrored, st);
     }
 }
 

@@ -6,29 +6,32 @@
 namespace des {
 
 // One thread per (member, quad).  Rows are P floats with arbitrary P, so stores are scalar and guarded.
+// mirrored (perturb rows only): member m is theta + (-1)^(m & 1) sigma * eps of counter word m >> 1.
 template <bool kPerturb>
 __global__ void noise_rows_kernel(float *__restrict__ out, const float *__restrict__ theta, int64_t n_members,
                                   int64_t P, float sigma, PhiloxKey key, uint32_t gen,
-                                  uint32_t tag, uint64_t member_offset) {
+                                  uint32_t tag, uint64_t member_offset, int mirrored) {
     const int64_t nq = (P + 3) >> 2;
     const int64_t total = n_members * nq;
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
          idx += (int64_t)gridDim.x * blockDim.x) {
         const int64_t m = idx / nq;
         const int64_t q = idx - m * nq;
-        const float4 z = noise_quad((uint32_t)q, (uint32_t)(member_offset + m), gen, tag, key);
+        const uint64_t gm = member_offset + m;
+        const float4 z = noise_quad((uint32_t)q, (uint32_t)(mirrored ? gm >> 1 : gm), gen, tag, key);
+        const float s = mirrored && (gm & 1u) ? -sigma : sigma;
         const float zz[4] = {z.x, z.y, z.z, z.w};
         float *row = out + m * P;
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int64_t j = 4 * q + e;
-            if (j < P) row[j] = kPerturb ? __fmaf_rn(sigma, zz[e], theta[j]) : zz[e];
+            if (j < P) row[j] = kPerturb ? __fmaf_rn(s, zz[e], theta[j]) : zz[e];
         }
     }
 }
 
 static int launch_rows(bool perturb, float *out, const float *theta, int64_t n, int64_t P, double sigma,
-                       uint64_t seed, uint64_t gen, int64_t member_offset, uint32_t tag, cudaStream_t st) {
+                       uint64_t seed, uint64_t gen, int64_t member_offset, uint32_t tag, bool mirrored, cudaStream_t st) {
     if (n == 0 || P == 0) return DES_OK;
     const int64_t total = n * ((P + 3) / 4);
     const int threads = 256;
@@ -37,10 +40,11 @@ static int launch_rows(bool perturb, float *out, const float *theta, int64_t n, 
     const PhiloxKey key = make_philox_key(seed);
     if (perturb)
         noise_rows_kernel<true><<<(unsigned)blocks, threads, 0, st>>>(out, theta, n, P, (float)sigma, key,
-                                                                      (uint32_t)gen, tag, (uint64_t)member_offset);
+                                                                      (uint32_t)gen, tag, (uint64_t)member_offset,
+                                                                      mirrored ? 1 : 0);
     else
         noise_rows_kernel<false><<<(unsigned)blocks, threads, 0, st>>>(out, nullptr, n, P, 0.f, key,
-                                                                       (uint32_t)gen, tag, (uint64_t)member_offset);
+                                                                       (uint32_t)gen, tag, (uint64_t)member_offset, 0);
     DES_LAUNCH_CHECK("noise_rows_kernel");
     return DES_OK;
 }
@@ -56,18 +60,38 @@ extern "C" DES_API int des_noise_fill(float *eps_out_dev, int64_t n_members, int
                 "des_noise_fill: member index must fit 32 bits");
     DES_REQUIRE(P <= ((int64_t)1 << 34), "des_noise_fill: P too large for the 32-bit quad counter");
     return des::launch_rows(false, eps_out_dev, nullptr, n_members, P, 0.0, seed, generation, member_offset,
-                            stream_tag, (cudaStream_t)stream);
+                            stream_tag, false, (cudaStream_t)stream);
 }
+
+namespace des {
+
+static int nes_perturb(const char *who, float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
+                       double sigma, uint64_t seed, uint64_t generation, int64_t member_offset, bool mirrored,
+                       cudaStream_t st) {
+    DES_REQUIRE(n_members >= 0 && P >= 0, "%s: negative size", who);
+    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_members % 2 == 0),
+                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_members (%lld) must be even", who,
+                (long long)member_offset, (long long)n_members);
+    DES_REQUIRE((theta_out_dev && theta_dev) || n_members * P == 0, "%s: NULL pointer", who);
+    DES_REQUIRE(member_offset >= 0 && member_offset + n_members <= (int64_t)1 << 32, "%s: member index must fit 32 bits", who);
+    return launch_rows(true, theta_out_dev, theta_dev, n_members, P, sigma, seed, generation, member_offset, kStreamNesEps,
+                       mirrored, st);
+}
+
+}  // namespace des
 
 extern "C" DES_API int des_nes_perturb(float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
                                double sigma, uint64_t seed, uint64_t generation, int64_t member_offset,
                                void *stream) {
-    DES_REQUIRE(n_members >= 0 && P >= 0, "des_nes_perturb: negative size");
-    DES_REQUIRE((theta_out_dev && theta_dev) || n_members * P == 0, "des_nes_perturb: NULL pointer");
-    DES_REQUIRE(member_offset >= 0 && member_offset + n_members <= (int64_t)1 << 32,
-                "des_nes_perturb: member index must fit 32 bits");
-    return des::launch_rows(true, theta_out_dev, theta_dev, n_members, P, sigma, seed, generation, member_offset,
-                            des::kStreamNesEps, (cudaStream_t)stream);
+    return des::nes_perturb("des_nes_perturb", theta_out_dev, theta_dev, n_members, P, sigma, seed, generation,
+                            member_offset, false, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_nes_perturb_mirrored(float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
+                                                double sigma, uint64_t seed, uint64_t generation, int64_t member_offset,
+                                                void *stream) {
+    return des::nes_perturb("des_nes_perturb_mirrored", theta_out_dev, theta_dev, n_members, P, sigma, seed, generation,
+                            member_offset, true, (cudaStream_t)stream);
 }
 
 // ---- observation normaliser (SURVEY 8f row 1): StaticNormalizer / SharedStats, utils.py:37-106 ---------------------

@@ -51,6 +51,9 @@ __host__ inline GradPlan grad_plan(int64_t n_local, int64_t P) {
     return p;
 }
 
+// kMirror: i runs over the n_local pairs of a mirrored shard, member_offset is the pair index of its first pair, and
+// pair i contributes (s_2i - s_2i+1) * eps_i: sum_m s_m eps_m with eps_2i+1 = -eps_2i, half the normals to regenerate
+template <bool kMirror>
 __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restrict__ ws, const float *__restrict__ shaped,
                                                                    int64_t n_local, int64_t nq, int64_t Ppad,
                                                                    int64_t per_chunk, PhiloxKey key,
@@ -64,7 +67,8 @@ __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restr
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll kGradUnroll
     for (int64_t i = i0; i < i1; ++i) {
-        const float s = __ldg(shaped + i);     // warp-uniform broadcast load
+        // warp-uniform broadcast loads
+        const float s = kMirror ? __fsub_rn(__ldg(shaped + 2 * i), __ldg(shaped + 2 * i + 1)) : __ldg(shaped + i);
         const uint4 x = philox4x32((uint32_t)q, (uint32_t)(member_offset + i), gen, kStreamNesEps, key);
         const BmParts a = box_muller_parts(x.x, x.y, kNeg2Ln2, key.one_bits);
         const BmParts b = box_muller_parts(x.z, x.w, kNeg2Ln2, key.one_bits);
@@ -147,37 +151,68 @@ extern "C" DES_API size_t des_grad_workspace_bytes(int64_t n_local, int64_t P) {
     return (size_t)p.chunks * (size_t)p.Ppad * sizeof(float);
 }
 
-extern "C" DES_API int des_nes_grad_partial(float *partial_out_dev, const float *shaped_local_dev, int64_t n_local, int64_t P,
-                                    uint64_t seed, uint64_t generation, const des_state *state_dev,
-                                    int64_t member_offset, void *workspace_dev, size_t workspace_bytes, void *stream) {
-    using namespace des;
-    DES_REQUIRE(n_local >= 0 && P > 0, "des_nes_grad_partial: bad sizes n_local=%lld P=%lld", (long long)n_local,
-                (long long)P);
-    DES_REQUIRE(partial_out_dev, "des_nes_grad_partial: partial_out_dev is NULL");
-    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32,
-                "des_nes_grad_partial: member index must fit 32 bits");
-    cudaStream_t st = (cudaStream_t)stream;
+namespace des {
+
+// Shared by both entry points.  Mirrored shards are planned by pairs: the slices of the plain plan of n_local members,
+// each holding half as many pairs, so the mirrored call never needs more slices (nor workspace) than the plain one.
+static int grad_partial(const char *who, float *partial_out_dev, const float *shaped_local_dev, int64_t n_local, int64_t P,
+                        uint64_t seed, uint64_t generation, const des_state *state_dev, int64_t member_offset,
+                        void *workspace_dev, size_t workspace_bytes, bool mirrored, cudaStream_t st) {
+    DES_REQUIRE(n_local >= 0 && P > 0, "%s: bad sizes n_local=%lld P=%lld", who, (long long)n_local, (long long)P);
+    DES_REQUIRE(partial_out_dev, "%s: partial_out_dev is NULL", who);
+    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32, "%s: member index must fit 32 bits", who);
+    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0),
+                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
+                (long long)member_offset, (long long)n_local);
     if (n_local == 0) {
         DES_CUDA(cudaMemsetAsync(partial_out_dev, 0, (size_t)P * sizeof(float), st));
         return DES_OK;
     }
-    DES_REQUIRE(shaped_local_dev, "des_nes_grad_partial: shaped_local_dev is NULL");
+    DES_REQUIRE(shaped_local_dev, "%s: shaped_local_dev is NULL", who);
     const GradPlan p = grad_plan(n_local, P);
     const size_t need = (size_t)p.chunks * (size_t)p.Ppad * sizeof(float);
     if (!workspace_dev || workspace_bytes < need) {
-        set_error("des_nes_grad_partial: workspace %zu B < required %zu B", workspace_bytes, need);
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
         return DES_ERR_WORKSPACE;
     }
-    DES_REQUIRE(((uintptr_t)workspace_dev & 15) == 0, "des_nes_grad_partial: workspace must be 16-byte aligned");
+    DES_REQUIRE(((uintptr_t)workspace_dev & 15) == 0, "%s: workspace must be 16-byte aligned", who);
     float *ws = (float *)workspace_dev;
     const unsigned bx = (unsigned)((p.nq + kGradThreads - 1) / kGradThreads);
-    grad_chunk_kernel<<<dim3(bx, (unsigned)p.chunks), kGradThreads, 0, st>>>(
-        ws, shaped_local_dev, n_local, p.nq, p.Ppad, p.per_chunk, make_philox_key(seed),
-        (uint32_t)generation, state_dev, (uint64_t)member_offset);
+    const PhiloxKey key = make_philox_key(seed);
+    int chunks = p.chunks;
+    if (mirrored) {
+        const int64_t pairs = n_local / 2, per_chunk = (p.per_chunk + 1) / 2;
+        chunks = (int)((pairs + per_chunk - 1) / per_chunk);     // <= p.chunks
+        grad_chunk_kernel<true><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
+            ws, shaped_local_dev, pairs, p.nq, p.Ppad, per_chunk, key, (uint32_t)generation, state_dev,
+            (uint64_t)member_offset / 2);
+    } else {
+        grad_chunk_kernel<false><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
+            ws, shaped_local_dev, n_local, p.nq, p.Ppad, p.per_chunk, key, (uint32_t)generation, state_dev,
+            (uint64_t)member_offset);
+    }
     DES_LAUNCH_CHECK("grad_chunk_kernel");
-    grad_reduce_kernel<<<(unsigned)((P + 31) / 32), dim3(32, kReduceRows), 0, st>>>(partial_out_dev, ws, P, p.Ppad, p.chunks);
+    grad_reduce_kernel<<<(unsigned)((P + 31) / 32), dim3(32, kReduceRows), 0, st>>>(partial_out_dev, ws, P, p.Ppad, chunks);
     DES_LAUNCH_CHECK("grad_reduce_kernel");
     return DES_OK;
+}
+
+}  // namespace des
+
+extern "C" DES_API int des_nes_grad_partial(float *partial_out_dev, const float *shaped_local_dev, int64_t n_local, int64_t P,
+                                    uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                    int64_t member_offset, void *workspace_dev, size_t workspace_bytes, void *stream) {
+    return des::grad_partial("des_nes_grad_partial", partial_out_dev, shaped_local_dev, n_local, P, seed, generation,
+                             state_dev, member_offset, workspace_dev, workspace_bytes, false, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_nes_grad_partial_mirrored(float *partial_out_dev, const float *shaped_local_dev, int64_t n_local,
+                                                     int64_t P, uint64_t seed, uint64_t generation,
+                                                     const des_state *state_dev, int64_t member_offset, void *workspace_dev,
+                                                     size_t workspace_bytes, void *stream) {
+    return des::grad_partial("des_nes_grad_partial_mirrored", partial_out_dev, shaped_local_dev, n_local, P, seed,
+                             generation, state_dev, member_offset, workspace_dev, workspace_bytes, true,
+                             (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_nes_apply(float *theta_dev, double *adam_m_dev, double *adam_v_dev, float *update_out_dev,

@@ -34,7 +34,8 @@ def shard_bounds(N, world_size, rank):
 class NESEngine:
     def __init__(self, *, state_dim, hidden, action_dim, pop_size, theta0, obs, target, sigma, learning_rate,
                  weight_decay=0.005, clip=1.0, seed=0, precision='fp32', beta1=0.9, beta2=0.999, epsilon=1e-8,
-                 device=None, process_group=None, kernels=None, use_graph=False, normalize_obs=False, repetitions=1):
+                 device=None, process_group=None, kernels=None, use_graph=False, normalize_obs=False, repetitions=1,
+                 mirrored=False):
         if kernels is None:
             from . import ops as kernels          # loads libdes_b200.so; raises if it is missing
         self.k = kernels
@@ -49,7 +50,15 @@ class NESEngine:
         self.N = int(pop_size)
         if self.N < 2:
             raise ValueError('pop_size must be >= 2 (fitness_shift divides by N-1, utils.py:146)')
-        self.offset, self.n_local = shard_bounds(self.N, self.world, self.rank)
+        # mirrored sampling: members 2p and 2p+1 are theta +- sigma*eps_p; a shard holds whole pairs
+        self.mirrored = bool(mirrored)
+        if self.mirrored:
+            if self.N % 2:
+                raise ValueError('mirrored sampling needs an even pop_size (members come in +-eps pairs); got %d' % self.N)
+            pair_offset, pairs = shard_bounds(self.N // 2, self.world, self.rank)
+            self.offset, self.n_local = 2 * pair_offset, 2 * pairs
+        else:
+            self.offset, self.n_local = shard_bounds(self.N, self.world, self.rank)
         self.sigma, self.lr, self.wd, self.clip = float(sigma), float(learning_rate), float(weight_decay), float(clip)
         self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
         self.seed, self.precision = int(seed), precision
@@ -133,6 +142,10 @@ class NESEngine:
                 self.eval_ws = self.k.eval_workspace(self.d0, self.H, self.A, int(obs.shape[0]), self.precision, self.device)
         self.T = int(obs.shape[0])
 
+    def _op(self, name):
+        """The device op `name`, or its mirrored-noise counterpart when the engine samples mirrored pairs."""
+        return getattr(self.k, name + '_mirrored' if self.mirrored else name)
+
     # -- the three phases around the two collectives -------------------------------------------------------
     def evaluate(self):
         if self.normalize_obs:        # utils.py:48-51 with the statistics of the previous generations
@@ -140,7 +153,7 @@ class NESEngine:
         if self.world > 1 and self.comm is None:
             self.fitness_all.zero_()
         if self.n_local:
-            self.k.nes_eval(self.theta, self.obs, self.target, hidden=self.H, sigma=self.sigma, clip=self.clip,
+            self._op('nes_eval')(self.theta, self.obs, self.target, hidden=self.H, sigma=self.sigma, clip=self.clip,
                             seed=self.seed, state=self.state, member_offset=self.offset, n_local=self.n_local,
                             precision=self.precision, out=self.fitness_shard_out,
                             workspace=self.eval_ws)
@@ -162,8 +175,9 @@ class NESEngine:
 
     def rank_and_reduce(self):
         self.k.centered_rank(self.fitness_all, self.offset, self.n_local, workspace=self.rank_ws, out=self.shaped)
-        self.k.nes_grad_partial(self.shaped, self.P, seed=self.seed, state=self.state, member_offset=self.offset,
-                                workspace=self.grad_ws, out=self.partial_local if self.comm is not None else self.partial)
+        self._op('nes_grad_partial')(self.shaped, self.P, seed=self.seed, state=self.state, member_offset=self.offset,
+                                     workspace=self.grad_ws,
+                                     out=self.partial_local if self.comm is not None else self.partial)
         if self.world > 1:
             if self.comm is not None:
                 self.comm.allreduce_partial(self.partial_local, self.partial)   # slots over NVLink, summed in rank order
@@ -300,13 +314,13 @@ class RolloutEngine(NESEngine):
             self.fitness_all.zero_()
         self.obs_totals.zero_()
         if self.n_local:
-            self.k.rollout_eval(self.theta, env=self.env_id, hidden=self.H, horizon=self.horizon,
-                                repetitions=self.repetitions, sigma=self.sigma, clip=self.clip,
-                                action_noise_std=self.action_noise_std, seed=self.seed, state=self.state,
-                                member_offset=self.offset, n_local=self.n_local,
-                                obs_stats=self.obs_stats if self.normalize_obs else None,
-                                totals_out=self.obs_totals if self.normalize_obs else None, workspace=self.roll_ws,
-                                out=self.fitness_shard_out)
+            self._op('rollout_eval')(self.theta, env=self.env_id, hidden=self.H, horizon=self.horizon,
+                                     repetitions=self.repetitions, sigma=self.sigma, clip=self.clip,
+                                     action_noise_std=self.action_noise_std, seed=self.seed, state=self.state,
+                                     member_offset=self.offset, n_local=self.n_local,
+                                     obs_stats=self.obs_stats if self.normalize_obs else None,
+                                     totals_out=self.obs_totals if self.normalize_obs else None, workspace=self.roll_ws,
+                                     out=self.fitness_shard_out)
         self._gather_fitness()
         if self.world > 1 and self.normalize_obs:
             dist.all_reduce(self.obs_totals, group=self.pg)
@@ -476,8 +490,8 @@ class HostEnvEngine(NESEngine):
         self.obs_totals.zero_()
         steps = 0
         if self.n_local:
-            self.k.nes_perturb(self.theta, self.n_local, self.sigma, self.seed, gen, member_offset=self.offset,
-                               out=self.rows)                                  # natural_es.py:28-30
+            self._op('nes_perturb')(self.theta, self.n_local, self.sigma, self.seed, gen, member_offset=self.offset,
+                                    out=self.rows)                             # natural_es.py:28-30
             self.stat_part.zero_()
             ret, steps = self.episodes.run(self.rows, generation=gen, member_offset=self.offset,
                                            obs_stats=self.obs_stats if self.normalize_obs else None,

@@ -50,7 +50,8 @@ def build_engine(config, param=None, **kw):
                              seed=getattr(config, 'seed', 0), beta1=config.opt.beta1, beta2=config.opt.beta2,
                              epsilon=config.opt.epsilon, repetitions=config.repetitions,
                              test_repetitions=config.test_repetitions, action_noise_std=config.action_noise_std,
-                             normalize_obs=getattr(config, 'normalize_obs', True), **kw)
+                             normalize_obs=getattr(config, 'normalize_obs', True),
+                             mirrored=getattr(config, 'mirrored', False), **kw)
     env = config.env_fn()
     if getattr(config, 'closed_loop', False):         # environment stepped on the device (SURVEY 8f row 3)
         return RolloutEngine(task=config.task, hidden=config.hidden_size, pop_size=config.pop_size, theta0=theta0,
@@ -58,13 +59,15 @@ def build_engine(config, param=None, **kw):
                              clip=config.clip, seed=getattr(config, 'seed', 0), beta1=config.opt.beta1,
                              beta2=config.opt.beta2, epsilon=config.opt.epsilon, repetitions=config.repetitions,
                              action_noise_std=config.action_noise_std,
-                             normalize_obs=getattr(config, 'normalize_obs', True), **kw)
+                             normalize_obs=getattr(config, 'normalize_obs', True),
+                             mirrored=getattr(config, 'mirrored', False), **kw)
     return NESEngine(state_dim=config.state_dim, hidden=config.hidden_size, action_dim=config.action_dim,
                      pop_size=config.pop_size, theta0=theta0, obs=env.obs, target=env.target, sigma=config.sigma,
                      learning_rate=config.learning_rate, weight_decay=config.weight_decay, clip=config.clip,
                      seed=getattr(config, 'seed', 0), precision=getattr(config, 'precision', 'fp32'),
                      beta1=config.opt.beta1, beta2=config.opt.beta2, epsilon=config.opt.epsilon,
-                     normalize_obs=getattr(config, 'normalize_obs', False), repetitions=config.repetitions, **kw)
+                     normalize_obs=getattr(config, 'normalize_obs', False), repetitions=config.repetitions,
+                     mirrored=getattr(config, 'mirrored', False), **kw)
 
 
 def train(config, engine=None):
@@ -198,6 +201,7 @@ def save_checkpoint(engine, path):
                 beta1_t=np.float64(st['beta1_t']), beta2_t=np.float64(st['beta2_t']),
                 seed=np.uint64(engine.seed), pop_size=np.int64(engine.N), dims=np.asarray([engine.d0, engine.H, engine.A]),
                 precision=np.str_(engine.precision), normalize_obs=np.bool_(engine.normalize_obs),
+                mirrored=np.bool_(engine.mirrored),
                 hyper=np.asarray([getattr(engine, k) for k in _CKPT_SCALARS], dtype=np.float64))
     if engine.normalize_obs:
         blob['obs_stats'] = engine.obs_stats.cpu().numpy()
@@ -216,6 +220,10 @@ def load_checkpoint(engine, path):
         if str(blob['precision']) != engine.precision or bool(blob['normalize_obs']) != engine.normalize_obs:
             raise ValueError('checkpoint was written with precision=%s normalize_obs=%s; the engine has %s / %s' %
                              (blob['precision'], bool(blob['normalize_obs']), engine.precision, engine.normalize_obs))
+        # checkpoints written before mirrored sampling existed have no key: they are plain runs
+        mirrored = bool(blob['mirrored']) if 'mirrored' in blob.files else False
+        if mirrored != engine.mirrored:
+            raise ValueError('checkpoint was written with mirrored=%s; the engine has mirrored=%s' % (mirrored, engine.mirrored))
         mine = np.asarray([getattr(engine, k) for k in _CKPT_SCALARS], dtype=np.float64)
         if not np.array_equal(mine, blob['hyper']):
             raise ValueError('checkpoint hyper-parameters %r differ from the engine\'s %r (%s)' %

@@ -88,15 +88,24 @@ def noise_fill(n_members, P, seed, generation, member_offset=0, stream_tag=0, de
 def nes_perturb(theta, n_members, sigma, seed, generation, member_offset=0, out=None):
     """theta'[n_members, P] = fp32(theta + sigma*eps) (natural_es.py:28-30): a parity op, and the weight rows of
     host-stepped environments (policy_act).  `out`: an optional [n_members, P] buffer."""
+    return _perturb('des_nes_perturb', theta, n_members, sigma, seed, generation, member_offset, out)
+
+
+def nes_perturb_mirrored(theta, n_members, sigma, seed, generation, member_offset=0, out=None):
+    """nes_perturb with mirrored noise: row i = fp32(theta + (-1)^(m & 1) sigma*eps[m >> 1]), m = member_offset + i
+    (member_offset and n_members even)."""
+    return _perturb('des_nes_perturb_mirrored', theta, n_members, sigma, seed, generation, member_offset, out)
+
+
+def _perturb(fn, theta, n_members, sigma, seed, generation, member_offset, out):
     P = theta.numel()
     if out is None:
         out = torch.empty((n_members, P), dtype=torch.float32, device=theta.device)
     elif out.numel() != n_members * P:
         raise RuntimeError('out has %d entries, need %d x %d' % (out.numel(), n_members, P))
     with _on(theta, 'theta'):
-        _lib.check(_lib.load().des_nes_perturb(_ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'),
-                                               n_members, P, sigma, seed, generation, member_offset, _stream()),
-                   'des_nes_perturb')
+        _lib.check(getattr(_lib.load(), fn)(_ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'),
+                                            n_members, P, sigma, seed, generation, member_offset, _stream()), fn)
     return out
 
 
@@ -128,6 +137,23 @@ def rollout_eval(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, cl
                  workspace=None, out=None, episodes_out=None):
     """Closed-loop fitness of members [member_offset, member_offset + n_local): mean return over `repetitions`
     episodes stepped on the device (Evaluator.eval utils.py:116-124 over single_run utils.py:126-139)."""
+    return _rollout('des_rollout_eval', theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed,
+                    generation, state, member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out,
+                    episodes_out)
+
+
+def rollout_eval_mirrored(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, clip, action_noise_std=0.0, seed,
+                          generation=0, state=None, member_offset=0, n_local, noiseless=False, obs_stats=None,
+                          totals_out=None, workspace=None, out=None, episodes_out=None):
+    """rollout_eval with mirrored noise: member m's weights are theta + (-1)^(m & 1) sigma*eps[m >> 1] (member_offset and
+    n_local even; noiseless is rejected: test episodes use rollout_eval).  Episodes stay keyed by the global member."""
+    return _rollout('des_rollout_eval_mirrored', theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std,
+                    seed, generation, state, member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out,
+                    episodes_out)
+
+
+def _rollout(fn, theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed, generation, state,
+             member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out, episodes_out):
     if env not in ENV_DIMS:
         raise RuntimeError('unknown environment id %r' % (env,))
     d0, A = ENV_DIMS[env]
@@ -137,14 +163,13 @@ def rollout_eval(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, cl
         workspace = torch.empty(max(n_local, 1) * (2 * d0 + 1), dtype=torch.float64, device=theta.device)
     ws_bytes = workspace.numel() * workspace.element_size() if workspace is not None else 0
     with _on(theta, 'theta'):
-        _lib.check(_lib.load().des_rollout_eval(
+        _lib.check(getattr(_lib.load(), fn)(
             _ptr(out, torch.float32, 'out'), _ptr(episodes_out, torch.float32, 'episodes_out', True),
             _ptr(totals_out, torch.float64, 'totals_out', True), _ptr(theta, torch.float32, 'theta'),
             _ptr(obs_stats, torch.float32, 'obs_stats', True), int(env), Dims(d0, hidden, A, horizon), int(repetitions),
             float(sigma), float(clip), float(action_noise_std), int(seed), int(generation),
             _ptr(state, torch.uint8, 'state', True), int(member_offset), int(n_local), 1 if noiseless else 0,
-            C.c_void_p(workspace.data_ptr()) if workspace is not None else C.c_void_p(0), ws_bytes, _stream()),
-            'des_rollout_eval')
+            C.c_void_p(workspace.data_ptr()) if workspace is not None else C.c_void_p(0), ws_bytes, _stream()), fn)
     return out
 
 
@@ -244,6 +269,20 @@ def nes_eval(theta, obs, target, *, hidden, sigma, clip, seed, generation=0, sta
 
     precision 'f16' / 'f16x3' run the hidden layers on tensor cores with fp16 operands: |obs| and |theta'| must stay
     below 65520, or they overflow to inf.  A NaN action gives a NaN fitness on every path (np.clip keeps NaN)."""
+    return _nes_eval('des_nes_eval', theta, obs, target, hidden, sigma, clip, seed, generation, state, member_offset,
+                     n_local, precision, out, workspace)
+
+
+def nes_eval_mirrored(theta, obs, target, *, hidden, sigma, clip, seed, generation=0, state=None, member_offset=0,
+                      n_local, precision='fp32', out=None, workspace=None):
+    """nes_eval with mirrored noise: member m's weights are theta + (-1)^(m & 1) sigma*eps[m >> 1], so member 2p's
+    fitness is bit-equal to nes_eval's member p (member_offset and n_local even)."""
+    return _nes_eval('des_nes_eval_mirrored', theta, obs, target, hidden, sigma, clip, seed, generation, state,
+                     member_offset, n_local, precision, out, workspace)
+
+
+def _nes_eval(fn, theta, obs, target, hidden, sigma, clip, seed, generation, state, member_offset, n_local, precision,
+              out, workspace):
     T, d0 = obs.shape
     A = target.shape[1]
     if target.shape[0] != T:
@@ -256,12 +295,12 @@ def nes_eval(theta, obs, target, *, hidden, sigma, clip, seed, generation=0, sta
     elif out.numel() != n_local:
         raise RuntimeError('out has %d entries, need n_local=%d' % (out.numel(), n_local))
     with _on(theta, 'theta'):
-        _lib.check(_lib.load().des_nes_eval(
+        _lib.check(getattr(_lib.load(), fn)(
             _ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'), _ptr(obs, torch.float32, 'obs'),
             _ptr(target, torch.float32, 'target'), Dims(d0, hidden, A, T), sigma, clip, seed, generation,
             _ptr(state, torch.uint8, 'state', allow_none=True), member_offset, n_local, _precision(precision),
             _ptr(workspace, torch.uint8, 'workspace', allow_none=True), workspace.numel() if workspace is not None else 0,
-            _stream()), 'des_nes_eval')
+            _stream()), fn)
     return out
 
 
@@ -313,6 +352,18 @@ def grad_workspace(n_local, P, device):
 
 def nes_grad_partial(shaped_local, P, *, seed, generation=0, state=None, member_offset=0, workspace=None, out=None):
     """partial[P] = sum_i shaped[i] * eps[member_offset+i] (natural_es.py:91, per shard; eps regenerated)."""
+    return _grad_partial('des_nes_grad_partial', shaped_local, P, seed, generation, state, member_offset, workspace, out)
+
+
+def nes_grad_partial_mirrored(shaped_local, P, *, seed, generation=0, state=None, member_offset=0, workspace=None,
+                              out=None):
+    """The partial of a mirrored shard: sum_p (shaped[2p] - shaped[2p+1]) * eps[member_offset/2 + p], one eps per pair
+    (member_offset and n_local even; grad_workspace(n_local, P) suffices)."""
+    return _grad_partial('des_nes_grad_partial_mirrored', shaped_local, P, seed, generation, state, member_offset,
+                         workspace, out)
+
+
+def _grad_partial(fn, shaped_local, P, seed, generation, state, member_offset, workspace, out):
     _on(shaped_local, 'shaped_local')
     n_local = shaped_local.numel()
     dev = shaped_local.device
@@ -321,10 +372,10 @@ def nes_grad_partial(shaped_local, P, *, seed, generation=0, state=None, member_
     if workspace is None:
         workspace = grad_workspace(n_local, P, dev)
     with _on(shaped_local, 'shaped_local'):
-        _lib.check(_lib.load().des_nes_grad_partial(
+        _lib.check(getattr(_lib.load(), fn)(
             _ptr(out, torch.float32, 'out'), _ptr(shaped_local, torch.float32, 'shaped_local'), n_local, P, seed,
             generation, _ptr(state, torch.uint8, 'state', allow_none=True), member_offset,
-            _ptr(workspace, torch.uint8, 'workspace'), workspace.numel(), _stream()), 'des_nes_grad_partial')
+            _ptr(workspace, torch.uint8, 'workspace'), workspace.numel(), _stream()), fn)
     return out
 
 

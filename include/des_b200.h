@@ -26,6 +26,13 @@
  *     z_first = -sqrt(-2 ln u1) cos(ang), z_second = -sqrt(-2 ln u1) sin(ang).
  *     (oracle/nes_oracle.py restates it bit-exactly for the uint32 words.)  It replaces
  *     np.random.randn at natural_es.py:29; eps never crosses a process/GPU boundary.
+ *   - Mirrored (antithetic) noise, the *_mirrored entry points: members come in pairs (2p, 2p+1) that share one eps,
+ *       eps_mirrored[m][j] = (-1)^(m & 1) * eps[m >> 1][j]
+ *     with eps[p] the stream-0 row above of "member" p (counter (j/4, p, generation, 0)).  So member 2p's weights are
+ *     exactly those of plain member p, and member 2p+1's are fmaf(-sigma, eps_p, theta) = fp32(theta - sigma*eps_p).
+ *     N must be even and every shard holds whole pairs: member_offset and n_local (n_members) even, or
+ *     DES_ERR_INVALID_ARGUMENT before any CUDA work.  Reset states (stream 2), action noise (stream 3) and episode seeds
+ *     (stream 4) stay keyed by the global member m: the two members of a pair see different episodes.
  */
 #ifndef DES_B200_H
 #define DES_B200_H
@@ -105,6 +112,10 @@ DES_API int des_noise_fill(float *eps_out_dev, int64_t n_members, int64_t P, uin
 DES_API int des_nes_perturb(float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
                     double sigma, uint64_t seed, uint64_t generation, int64_t member_offset,
                     void *stream);
+/* The same rows for mirrored noise: row i = fp32(theta + (-1)^(m & 1) sigma*eps[m >> 1]), m = member_offset + i (see the
+ * mirrored noise contract above; member_offset and n_members even).  The rows of HostEnvEngine's mirrored generations. */
+DES_API int des_nes_perturb_mirrored(float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
+                                     double sigma, uint64_t seed, uint64_t generation, int64_t member_offset, void *stream);
 
 /* ---- observation normaliser (StaticNormalizer / SharedStats, utils.py:37-106) -------------------------- */
 
@@ -140,6 +151,14 @@ DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_returns_out_
                              double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                              const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                              void *workspace_dev, size_t workspace_bytes, void *stream);
+/* des_rollout_eval with mirrored noise (contract above): member m's weights are theta + (-1)^(m & 1) sigma*eps[m >> 1].
+ * Same arguments; member_offset and n_local even, and noiseless != 0 is rejected (test episodes use des_rollout_eval). */
+DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                      const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                      int32_t repetitions, double sigma, double clip, double action_noise_std,
+                                      uint64_t seed, uint64_t generation, const des_state *state_dev, int64_t member_offset,
+                                      int64_t n_local, int noiseless, void *workspace_dev, size_t workspace_bytes,
+                                      void *stream);
 
 /* The same rollouts for explicit solutions: member i (i < n_local) takes its weights from row i of solutions_dev
  * [n_local][P] (fp32, row-major, P = des_param_count(3, hidden, 1)) instead of theta + sigma*eps; no noise is generated.
@@ -217,6 +236,12 @@ DES_API int des_nes_eval(float *fitness_out_dev, const float *theta_dev, const f
                  uint64_t generation, const des_state *state_dev, int64_t member_offset,
                  int64_t n_local, int precision, void *workspace_dev, size_t workspace_bytes,
                  void *stream);
+/* des_nes_eval with mirrored noise (contract above): member m's weights are theta + (-1)^(m & 1) sigma*eps[m >> 1], so
+ * member 2p's fitness is bit-equal to plain member p's.  Same arguments; member_offset and n_local even. */
+DES_API int des_nes_eval_mirrored(float *fitness_out_dev, const float *theta_dev, const float *obs_dev,
+                                  const float *target_dev, des_dims dims, double sigma, double clip, uint64_t seed,
+                                  uint64_t generation, const des_state *state_dev, int64_t member_offset, int64_t n_local,
+                                  int precision, void *workspace_dev, size_t workspace_bytes, void *stream);
 
 /* fitness_out_dev[i] = the same tape fitness for EXPLICIT weight vectors solutions_dev[n_solutions][P] (no noise):
  * the evaluation CMA-ES needs, where the master ships sampled solutions to the workers (cma_es.py:62-64,
@@ -249,6 +274,13 @@ DES_API int des_nes_grad_partial(float *partial_out_dev, const float *shaped_loc
                          int64_t P, uint64_t seed, uint64_t generation, const des_state *state_dev,
                          int64_t member_offset, void *workspace_dev, size_t workspace_bytes,
                          void *stream);
+/* The same partial for a mirrored shard: sum_p (s[2p] - s[2p+1]) * eps[member_offset/2 + p][j] over its n_local/2 pairs
+ * (the pair difference in fp32; one eps regenerated per pair), which equals sum_i s_i eps_mirrored[i].  Same arguments;
+ * member_offset and n_local even; the workspace of des_grad_workspace_bytes(n_local, P) suffices. */
+DES_API int des_nes_grad_partial_mirrored(float *partial_out_dev, const float *shaped_local_dev, int64_t n_local,
+                                          int64_t P, uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                          int64_t member_offset, void *workspace_dev, size_t workspace_bytes,
+                                          void *stream);
 
 /* ---- (1-wd) scale + Adam + step ------------------------------------------------------------- */
 

@@ -1,0 +1,259 @@
+"""Mirrored (antithetic) sampling on the device: members 2p and 2p+1 are theta +- sigma*eps_p (include/des_b200.h).
+
+* Tape forward: member 2p is bit-equal to plain member p on every kernel shape (fp32; f16 / f16x3 on 2-CTA clusters,
+  single-CTA and multi-pass tapes, with and without the tile workspace); member 2p+1 matches the fp32 forward of the
+  des_nes_perturb_mirrored rows within the per-precision tolerances of test_gpu_ops.py.
+* Rows, the pair-form reduction (against an fp64 sum over the device's own normals), closed-loop and host-stepped
+  Pendulum, natural_es.train against the reference's verbatim run on explicit +-eps pairs (tests/golden/*_mirrored*),
+  graph capture and two GPUs."""
+import os
+
+import numpy as np
+import pytest
+
+torch = pytest.importorskip('torch')
+
+from oracle import mirrored_oracle as mo
+from oracle import nes_oracle as orc
+from oracle import pendulum_oracle as po
+
+pytestmark = pytest.mark.gpu
+DEV = 'cuda:0'
+HERE = os.path.dirname(os.path.abspath(__file__))
+TOL = {'fp32': 2e-5, 'f16x3': 3e-5, 'f16': 4e-3}
+RTOL = 2e-4
+
+
+def ops():
+    from distributedes_b200 import ops as o
+    return o
+
+
+def dev(x, dtype=torch.float32):
+    return torch.as_tensor(np.ascontiguousarray(x)).to(dtype).to(DEV)
+
+
+# T = 256: 2-CTA cluster, one pass; 128: single CTA; 384: single CTA, three passes; 512: 2-CTA cluster, two passes
+@pytest.mark.parametrize('T', [128, 256, 384, 512])
+@pytest.mark.parametrize('H', [64, 128, 256])
+@pytest.mark.parametrize('precision', ['fp32', 'f16', 'f16x3'])
+def test_tape_forward_pairs(precision, H, T):
+    d0, A, pairs, off = 24, 4, 40, 6
+    obs, target = orc.synthetic_tape(T, d0, A)
+    th, o, t = dev(orc.synthetic_theta(d0, H, A)), dev(obs), dev(target)
+    kw = dict(hidden=H, sigma=0.1, clip=1.0, seed=9, generation=2, precision=precision)
+    plain = ops().nes_eval(th, o, t, member_offset=off // 2, n_local=pairs, **kw)
+    ws = ops().eval_workspace(d0, H, A, T, precision, DEV) if precision != 'fp32' else None
+    for workspace in ([None, ws] if ws is not None else [None]):
+        mir = ops().nes_eval_mirrored(th, o, t, member_offset=off, n_local=2 * pairs, workspace=workspace, **kw)
+        assert torch.equal(mir[0::2], plain), workspace is not None
+    rows = ops().nes_perturb_mirrored(th, 2 * pairs, 0.1, 9, 2, member_offset=off)
+    ref = ops().pop_eval(rows[1::2].contiguous(), o, t, hidden=H, clip=1.0)
+    rel = ((mir[1::2] - ref).abs() / ref.abs()).max().item()
+    assert rel < TOL[precision], rel
+
+
+def test_perturb_rows():
+    P, pairs, off = 6020, 12, 10
+    theta = dev(orc.synthetic_theta(24, 64, 4))
+    rows = ops().nes_perturb_mirrored(theta, 2 * pairs, 0.1, 3, 5, member_offset=off)
+    plain = ops().nes_perturb(theta, pairs, 0.1, 3, 5, member_offset=off // 2)
+    assert torch.equal(rows[0::2], plain)
+    eps = ops().noise_fill(pairs, P, 3, 5, member_offset=off // 2).double()
+    ref = (theta.double() - float(np.float32(0.1)) * eps).float()
+    ulp = (torch.nextafter(ref, torch.full_like(ref, np.inf)) - ref).abs()
+    assert bool(((rows[1::2] - ref).abs() <= ulp).all())
+
+
+def _pair_reference(shaped, P, seed, gen, member_offset, chunk=2048):
+    s = shaped.double()
+    c = s[0::2] - s[1::2]
+    g = torch.zeros(P, dtype=torch.float64, device=DEV)
+    for o in range(0, c.numel(), chunk):
+        n = min(chunk, c.numel() - o)
+        g += c[o:o + n] @ ops().noise_fill(n, P, seed, gen, member_offset=member_offset // 2 + o).double()
+    return g
+
+
+@pytest.mark.parametrize('P', [6020, 73220])
+@pytest.mark.parametrize('N', [64, 4096, 65536])
+def test_pair_form_reduction(N, P):
+    rs = np.random.RandomState(N + P)
+    shaped = dev(orc.fitness_shift(rs.randn(N)))
+    kw = dict(seed=12, generation=3)
+    got = ops().nes_grad_partial_mirrored(shaped, P, **kw).double()
+    ref = _pair_reference(shaped, P, 12, 3, 0)
+    assert ((got - ref).norm() / ref.norm()).item() <= 1e-5
+    assert ((got - ref).abs().max() / ref.abs().max()).item() <= 1e-5
+    # shards at even offsets sum to the whole
+    cuts = [0, 2 * (N // 6), 2 * (N // 3), N]
+    parts = sum(ops().nes_grad_partial_mirrored(shaped[a:b].contiguous(), P, member_offset=a, **kw).double()
+                for a, b in zip(cuts[:-1], cuts[1:]))
+    assert ((parts - ref).norm() / ref.norm()).item() <= 1e-5
+    # the plain workspace query sizes the mirrored call; a short workspace is DES_ERR_WORKSPACE
+    ws = ops().grad_workspace(N, P, DEV)
+    assert torch.equal(ops().nes_grad_partial_mirrored(shaped, P, workspace=ws, **kw).double(), got)
+    with pytest.raises(RuntimeError, match='status -4'):
+        ops().nes_grad_partial_mirrored(shaped, P, workspace=torch.empty(16, dtype=torch.uint8, device=DEV), **kw)
+
+
+@pytest.mark.parametrize('H', [16, 32, 64, 96, 128])
+def test_closed_loop_equals_explicit_rows(H):
+    n, off, reps, seed, gen = 12, 4, 10, 21, 3
+    theta = dev(orc.synthetic_theta(3, H, 1, seed=H))
+    st = dev(np.array([-0.2, 0.01, 0.3, 0.5, 0.4, 20.0, 32000.0], np.float32))
+    kw = dict(hidden=H, horizon=120, repetitions=reps, clip=2.0, action_noise_std=0.2, seed=seed, generation=gen,
+              member_offset=off, obs_stats=st)
+    tot_a = torch.zeros(7, dtype=torch.float64, device=DEV)
+    tot_b = torch.zeros(7, dtype=torch.float64, device=DEV)
+    a = ops().rollout_eval_mirrored(theta, sigma=0.1, n_local=n, totals_out=tot_a, **kw)
+    rows = ops().nes_perturb_mirrored(theta, n, 0.1, seed, gen, member_offset=off)
+    b = ops().rollout_eval_solutions(rows, totals_out=tot_b, **kw)
+    assert torch.equal(a, b) and torch.equal(tot_a, tot_b)
+    # shard invariance: [off, off + 4) + [off + 4, off + n) in two launches
+    kw.pop('member_offset')
+    lo = ops().rollout_eval_mirrored(theta, sigma=0.1, n_local=4, member_offset=off, **kw)
+    hi = ops().rollout_eval_mirrored(theta, sigma=0.1, n_local=n - 4, member_offset=off + 4, **kw)
+    assert torch.equal(a, torch.cat([lo, hi]))
+    with pytest.raises(RuntimeError, match='whole pairs'):
+        ops().rollout_eval_mirrored(theta, sigma=0.1, n_local=3, member_offset=off, **kw)
+
+
+def test_host_stepped_pendulum_equals_closed_loop():
+    """HostEnvEngine(mirrored=True) stepping Pendulum-v0 on the host evaluates the members RolloutEngine(mirrored=True)
+    evaluates on the device, and both match the oracle's mirrored closed-loop fitness."""
+    import sys
+    sys.path.insert(0, HERE)
+    import host_env_support as hs
+    from distributedes_b200.engine import HostEnvEngine, RolloutEngine
+    H, N, reps, seed = 32, 12, 3, 5
+    theta0 = orc.synthetic_theta(3, H, 1, seed=4)
+    kw = dict(hidden=H, pop_size=N, theta0=theta0, sigma=0.1, learning_rate=0.1, repetitions=reps, seed=seed,
+              mirrored=True)
+    host = HostEnvEngine(env_fn=None, state_dim=3, action_dim=1, batch_env_fn=lambda B: hs.PendulumBatch(B, seed),
+                         clip=2.0, **kw)
+    roll = RolloutEngine(**kw)
+    fh, fr = host.evaluate().cpu().numpy(), roll.evaluate().cpu().numpy()
+    assert host.steps_taken == N * reps * po.HORIZON
+    assert np.max(np.abs(fh - fr) / np.abs(fr)) < RTOL
+    ref, _ = mo.closed_fitness(theta0, H, 0.1, seed, 0, 0, N, reps)
+    assert np.max(np.abs(fh - ref) / np.abs(ref)) < RTOL
+    assert np.array_equal(host.rows[0::2].cpu().numpy(), ops().nes_perturb(dev(theta0), N // 2, 0.1, seed, 0).cpu().numpy())
+
+
+def relnorm(a, b):
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    return np.linalg.norm(a - b) / np.linalg.norm(b)
+
+
+def test_tape_train_matches_reference_golden():
+    """NESEngine(mirrored=True) against natural_es.train() run verbatim on explicit +-eps pairs: test rewards, gradient
+    after weight decay, Adam update and parameters for three generations (no rank flips at N = 24)."""
+    from distributedes_b200.engine import NESEngine
+    g = np.load(os.path.join(HERE, 'golden', 'train_b64_mirrored.npz'))
+    d0, H, A, T = (int(v) for v in g['dims'])
+    N, seed = int(g['N']), int(g['seed'])
+    obs, target = orc.synthetic_tape(T, d0, A)
+    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=g['theta0'], obs=obs, target=target,
+                    sigma=float(g['sigma']), learning_rate=float(g['lr']), weight_decay=float(g['wd']),
+                    clip=float(g['clip']), seed=seed, precision='fp32', device=DEV, mirrored=True)
+    for gen in range(int(g['gens'])):
+        rew = eng.noiseless_fitness()
+        assert abs(rew - g['test_rewards'][gen]) < 2e-5 * abs(g['test_rewards'][gen])
+        eng.generation()
+        grad = eng.partial.cpu().numpy().astype(np.float64) / N / float(g['sigma']) * (1 - float(g['wd']))
+        assert relnorm(grad, g['grad_after_wd'][gen]) <= 2e-5, gen
+        if gen >= 1:
+            assert relnorm(eng.update.cpu().numpy(), g['update'][gen]) <= 2e-5, gen
+        assert np.max(np.abs(eng.theta_numpy() - g['theta'][gen])) <= 2e-5
+
+
+def test_closed_loop_train_matches_reference_golden():
+    """natural_es.train(ClosedLoopPendulumConfig) with config.mirrored = True against the reference's verbatim run
+    (layered: the gradient chain on the device's own fitness, then against the golden when no rank flipped)."""
+    from distributedes_b200 import natural_es
+    from distributedes_b200.config import ClosedLoopPendulumConfig
+    g = np.load(os.path.join(HERE, 'golden', 'train_closed_mirrored_pend.npz'))
+    H, N, reps, seed, gens = int(g['H']), int(g['N']), int(g['reps']), int(g['seed']), int(g['gens'])
+    cfg = ClosedLoopPendulumConfig(hidden_size=H)
+    cfg.initial_weight = g['theta0'].copy()
+    cfg.pop_size, cfg.sigma, cfg.learning_rate, cfg.seed = N, float(g['sigma']), float(g['lr']), seed
+    cfg.repetitions = cfg.test_repetitions = reps
+    cfg.max_steps = (gens + 1) * N * reps * 200 - 1
+    cfg.mirrored = True
+    eng = natural_es.build_engine(cfg)
+    assert eng.mirrored
+    fits, stats = [], []
+    real_rank, real_apply = eng.rank_and_reduce, eng.apply
+
+    def spy_rank():
+        fits.append(eng.fitness_all.cpu().numpy().astype(np.float64))
+        return real_rank()
+
+    def spy_apply():
+        real_apply()
+        stats.append(eng.obs_stats.cpu().numpy().copy())
+    eng.rank_and_reduce, eng.apply = spy_rank, spy_apply
+    rewards, steps, _ = natural_es.train(cfg, engine=eng)
+    assert steps == list(g['train_steps'])
+    assert np.allclose(rewards, g['test_rewards'], rtol=RTOL)
+    theta, opt, P = g['theta0'].copy(), orc.Adam(), g['theta0'].size
+    for gen in range(gens):
+        assert np.allclose(stats[gen], g['stats'][gen], rtol=5e-4, atol=5e-5)
+        grad = mo.nes_gradient_streamed(orc.fitness_shift(fits[gen]), float(g['sigma']), seed, gen, P)
+        theta, _ = orc.nes_update(theta, grad, opt, float(g['wd']), float(g['lr']))
+    assert np.max(np.abs(eng.theta_numpy() - theta)) <= 1e-5 * np.max(np.abs(theta - g['theta0']))
+    if np.max(np.abs(theta - g['theta'][-1])) <= 2e-6:
+        assert np.max(np.abs(eng.theta_numpy() - g['theta'][-1])) <= 1e-5 * np.max(np.abs(g['theta'][-1] - g['theta0']))
+
+
+@pytest.mark.parametrize('precision', ['f16x3', 'f16'])
+def test_graph_captured_generation_equals_eager(precision):
+    from distributedes_b200.engine import NESEngine
+    d0, H, A, T, N = 24, 64, 4, 256, 400
+    obs, target = orc.synthetic_tape(T, d0, A)
+    kw = dict(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
+              target=target, sigma=0.1, learning_rate=0.05, seed=3, precision=precision, device=DEV, mirrored=True)
+    a, b = NESEngine(use_graph=True, **kw), NESEngine(use_graph=False, **kw)
+    for _ in range(3):
+        a.generation()
+        b.generation()
+        assert torch.equal(a.fitness_all, b.fitness_all) and torch.equal(a.theta, b.theta)
+    assert not torch.equal(a.theta, torch.from_numpy(kw['theta0']).to(DEV))
+
+
+def _two_gpu_worker(rank, world, port, outdir):
+    import torch.distributed as dist
+    from distributedes_b200.engine import NESEngine
+    torch.cuda.set_device(rank)
+    dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
+    try:
+        d0, H, A, T = 24, 64, 4, 256
+        obs, target = orc.synthetic_tape(T, d0, A)
+        eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=22, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
+                        target=target, sigma=0.1, learning_rate=0.05, seed=3, precision='f16x3',
+                        device=torch.device('cuda', rank), mirrored=True)
+        for _ in range(2):
+            eng.generation()
+        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), theta=eng.theta_numpy(), fit=eng.fitness_all.cpu().numpy(),
+                 offset=eng.offset, n_local=eng.n_local)
+    finally:
+        dist.destroy_process_group()
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason='needs 2 GPUs')
+def test_two_gpu_mirrored_equals_one_gpu(tmp_path):
+    import torch.multiprocessing as mp
+    from distributedes_b200.engine import NESEngine
+    mp.spawn(_two_gpu_worker, args=(2, 29871, str(tmp_path)), nprocs=2, join=True)
+    r = [np.load(str(tmp_path / ('rank%d.npz' % k))) for k in range(2)]
+    assert (int(r[0]['n_local']), int(r[1]['offset'])) == (12, 12)
+    assert np.array_equal(r[0]['theta'], r[1]['theta']) and np.array_equal(r[0]['fit'], r[1]['fit'])
+    d0, H, A, T = 24, 64, 4, 256
+    obs, target = orc.synthetic_tape(T, d0, A)
+    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=22, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
+                    target=target, sigma=0.1, learning_rate=0.05, seed=3, precision='f16x3', device=DEV, mirrored=True)
+    for _ in range(2):
+        eng.generation()
+    assert np.array_equal(eng.fitness_all.cpu().numpy(), r[0]['fit'])
+    assert np.max(np.abs(eng.theta_numpy() - r[0]['theta'])) <= 1e-6
