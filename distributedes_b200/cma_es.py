@@ -2,11 +2,10 @@
 reference takes from the third-party `cma` package (cma.CMAEvolutionStrategy, cma_es.py:49: ask() :62, tell() :90).
 
 The hot arithmetic — the rank-mu covariance update inside tell() — is des_cma_rank_mu + des_cma_cov_apply
-(csrc/des_cma.cu); solutions are evaluated by des_pop_eval on the tape, or rolled out in the environment on the device by
-des_rollout_eval_solutions (closed-loop configs), and rank-shaped by des_centered_rank.  The small
-O(n)/O(n^2) bookkeeping around it (mean, evolution paths, step size) and the library calls a CMA step needs
-(the [lambda,n]x[n,n] sampling GEMM and the symmetric eigendecomposition) go through torch (cuBLAS / cuSOLVER):
-plumbing, not kernels of this repo.  Equations: Hansen's tutorial arXiv:1604.00772 (cited at README.md:16);
+(csrc/des_cma.cu); solutions are evaluated through a fitness source (fitness.py) and rank-shaped by
+des_centered_rank.  The small O(n)/O(n^2) bookkeeping around it (mean, evolution paths, step size) and the library
+calls a CMA step needs (the [lambda,n]x[n,n] sampling GEMM and the symmetric eigendecomposition) go through torch
+(cuBLAS / cuSOLVER): plumbing, not kernels of this repo.  Equations: Hansen's tutorial arXiv:1604.00772 (cited at README.md:16);
 pycma itself is not available here, so this follows oracle/cma_oracle.py's restatement ("parity unpinned").
 """
 from __future__ import annotations
@@ -18,7 +17,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import fitness, ops
 from .engine import shard_bounds
 from .utils import StaticNormalizer, logger
 
@@ -171,12 +170,9 @@ class CMAEvolutionStrategy:
 
 
 class Worker:
-    """cma_es.py:13-29 re-cast: evaluates the solutions of this rank's shard on one GPU.
-
-    Tape configs score them with des_pop_eval.  Closed-loop configs (`config.closed_loop`) roll every solution out in the
-    environment on the device with des_rollout_eval_solutions, `config.repetitions` episodes each, and keep what the
-    reference's workers share with the master (cma_es.py:35-38): the normaliser statistics [m | v | n] on the device and
-    the fp64 (sum, sum of squares, count) of the raw observations of the last evaluation, as engine.RolloutEngine does.
+    """cma_es.py:13-29 re-cast: evaluates the solutions of this rank's shard on one GPU through the fitness source its
+    config describes (fitness.from_config), which keeps what the reference's workers share with the master
+    (cma_es.py:35-38): the statistics `obs_stats` and the observation totals `obs_totals` of the last evaluation.
 
     `kernels` (default: distributedes_b200.ops) and `device` exist so the sharded host logic can run under gloo on CPU
     with an oracle-backed stand-in, as in CMAEvolutionStrategy."""
@@ -189,126 +185,30 @@ class Worker:
         else:
             self.device = torch.device(device if device is not None else 'cpu')
         self.kn = kernels
-        self.host_env = bool(getattr(config, 'host_env', False))
-        self.closed_loop = bool(getattr(config, 'closed_loop', False)) or self.host_env
-        if self.host_env:
-            # environments stepped on the host, the solutions' policy step on the device (engine.HostEpisodes)
-            self.d0, self.A, self.T = int(config.state_dim), int(config.action_dim), 0
-            self.normalize_obs = bool(getattr(config, 'normalize_obs', True))
-            self.obs_stats = (torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device)
-                              if self.normalize_obs else None)
-            self.obs_totals = torch.zeros(2 * self.d0 + 1, dtype=torch.float64, device=self.device)
-            batch_env_fn = getattr(config, 'batch_env_fn', None)
-            if batch_env_fn is None:
-                from .envs import GymEnvBatch
-                batch_env_fn = lambda B: GymEnvBatch(config.env_fn, B, getattr(config, 'seed', 0))     # noqa: E731
-            self.batch_env_fn = batch_env_fn
-            self._episodes = {}           # (members, repetitions) -> engine.HostEpisodes
-            self.steps_taken = 0          # environment steps of the last run() on this rank
-            self.tests_run = 0
-        elif self.closed_loop:
-            from .engine import RolloutEngine
-            if config.task not in RolloutEngine.ENVS:
-                raise ValueError('closed-loop environments available on the device: %s (got %r)'
-                                 % (sorted(RolloutEngine.ENVS), config.task))
-            spec = RolloutEngine.ENVS[config.task]
-            self.env_id, self.T, self.d0 = spec['env'], int(spec['horizon']), int(spec['state_dim'])
-            self.normalize_obs = bool(getattr(config, 'normalize_obs', True))
-            self.obs_stats = (torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device)
-                              if self.normalize_obs else None)
-            self.obs_totals = torch.zeros(2 * self.d0 + 1, dtype=torch.float64, device=self.device)
-            self.roll_ws = None
-            self.tests_run = 0            # test() calls so far: the generation word of the next test episodes
-        else:
-            env = config.env_fn()
-            self.T = env.tape_len
-            self.obs = torch.from_numpy(env.obs).to(self.device)
-            self.target = torch.from_numpy(env.target).to(self.device)
+        self.source = fitness.from_config(config, kernels, self.device)
+        self.obs_stats, self.obs_totals = self.source.obs_stats, self.source.obs_totals
+        self.tests_run = 0            # test() calls so far: the generation word of the next test episodes
 
     def run(self, solutions, member_offset=0, generation=0):
         """cost (cma_es.py:28: Evaluator.eval returns -mean return) of every solution; row i is global member
-        member_offset + i of generation `generation` (closed loop: its reset states)."""
-        if not self.closed_loop:
-            fit = self.kn.pop_eval(solutions, self.obs, self.target, hidden=self.config.hidden_size, clip=self.config.clip)
-            return -fit
-        if self.host_env:
-            return self._run_host(solutions, member_offset, generation)
-        c = self.config
-        n_local = int(solutions.shape[0])
-        self.obs_totals.zero_()
-        fit = torch.zeros(n_local, dtype=torch.float32, device=self.device)
-        if n_local:
-            w = 2 * self.d0 + 1
-            if self.roll_ws is None or self.roll_ws.numel() < n_local * w:
-                self.roll_ws = torch.empty(n_local * w, dtype=torch.float64, device=self.device)
-            self.kn.rollout_eval_solutions(solutions, env=self.env_id, hidden=c.hidden_size, horizon=self.T,
-                                           repetitions=c.repetitions, clip=c.clip, action_noise_std=c.action_noise_std,
-                                           seed=getattr(c, 'seed', 0), generation=generation, member_offset=member_offset,
-                                           obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
-                                           workspace=self.roll_ws, out=fit)
-        return -fit
-
-    def _host_episodes(self, n, reps):
-        ep = self._episodes.get((n, reps))
-        if ep is None:
-            from .engine import HostEpisodes
-            c = self.config
-            ep = HostEpisodes(self.kn, self.device, self.batch_env_fn(n * reps), n, reps, self.d0, c.hidden_size,
-                              self.A, c.clip, c.action_noise_std, getattr(c, 'seed', 0))
-            self._episodes[(n, reps)] = ep
-        return ep
-
-    def _run_host(self, solutions, member_offset, generation):
-        c = self.config
-        n_local = int(solutions.shape[0])
-        self.obs_totals.zero_()
-        fit = torch.zeros(n_local, dtype=torch.float32, device=self.device)
-        self.steps_taken = 0
-        if n_local:
-            rows = solutions.to(device=self.device, dtype=torch.float32).contiguous()
-            part = (torch.zeros((n_local, 2 * self.d0 + 1), dtype=torch.float64, device=self.device)
-                    if self.normalize_obs else None)
-            ret, self.steps_taken = self._host_episodes(n_local, c.repetitions).run(
-                rows, generation=generation, member_offset=member_offset, obs_stats=self.obs_stats, stat_part=part)
-            fit.copy_(torch.from_numpy(ret.mean(axis=1).astype(np.float32)))
-            if part is not None:
-                self.kn.obs_parts_reduce(part, self.d0, out=self.obs_totals)
-        return -fit
+        member_offset + i of generation `generation` (its reset states, on an environment)."""
+        return -self.source.solutions(solutions, offset=member_offset, generation=generation)
 
     def steps_over_ranks(self, es):
         """Environment steps of the last run(), summed over ranks (cma_es.py:73 sums the episodes' real lengths)."""
-        total = torch.tensor([self.steps_taken], dtype=torch.int64, device=self.device)
-        if es.world > 1:
-            dist.all_reduce(total, group=es.pg)
-        return int(total.item())
+        return self.source.steps(es.lam, es.world, es.pg)
 
     def test_returns(self, solution, repetitions):
         """Returns of `repetitions` noiseless episodes of one solution (cma_es.py:102-111) with the current statistics.
         The k-th call (k = 0 first) resets its episodes from the test stream with generation word k."""
-        c = self.config
-        if self.host_env:
-            from .envs import TEST_MEMBER
-            row = solution.reshape(1, -1).to(device=self.device, dtype=torch.float32).contiguous()
-            ret, _ = self._host_episodes(1, int(repetitions)).run(row, generation=self.tests_run, key_member=TEST_MEMBER,
-                                                                 obs_stats=self.obs_stats)
-            self.tests_run += 1
-            return ret[0]
-        sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
-        episodes = torch.empty(int(repetitions), dtype=torch.float32, device=self.device)
-        self.kn.rollout_eval(sol, env=self.env_id, hidden=c.hidden_size, horizon=self.T, repetitions=int(repetitions),
-                             sigma=0.0, clip=c.clip, action_noise_std=c.action_noise_std, seed=getattr(c, 'seed', 0),
-                             generation=self.tests_run, member_offset=0, n_local=1, noiseless=True,
-                             obs_stats=self.obs_stats, episodes_out=episodes)
+        ret = self.source.test_returns(solution, int(repetitions), self.tests_run)
         self.tests_run += 1
-        return episodes.cpu().numpy().astype(np.float64)
+        return ret
 
     def merge_obs_stats(self, es):
         """cma_es.py:92-96: the statistics of this generation's observations, summed over ranks, merged into [m|v|n]."""
-        if not (self.closed_loop and self.normalize_obs):
-            return
-        if es.world > 1:
-            dist.all_reduce(self.obs_totals, group=es.pg)
-        self.kn.obs_stats_merge_totals(self.obs_stats, self.obs_totals, self.d0)
+        self.source.share_totals(es.world, es.pg)
+        self.source.merge(es.lam)
 
 
 def train(config, worker=None, es=None):
@@ -331,10 +231,7 @@ def train(config, worker=None, es=None):
     while True:
         solutions = es.ask()                                                                # :62 (this rank's shard)
         cost = es.gather_cost(worker.run(solutions, es.offset, es.gen))                     # :63-72, all lambda costs
-        if getattr(worker, 'host_env', False):                                             # :73, real lengths
-            total_steps += worker.steps_over_ranks(es)
-        else:
-            total_steps += config.pop_size * config.repetitions * worker.T
+        total_steps += worker.steps_over_ranks(es)                                          # :73
         best = int(torch.argmin(cost))                                                      # :75
         elapsed_time = time.time() - initial_time
         best_solution = _fetch_member(es, solutions, best)
@@ -374,10 +271,7 @@ def test(config, solution, stats, worker=None):
     worker = worker if worker is not None else Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
     sol = torch.as_tensor(np.asarray(solution.detach().cpu() if isinstance(solution, torch.Tensor) else solution,
                                      dtype=np.float32)).reshape(1, -1).to(worker.device)
-    if worker.closed_loop:
-        if stats is not None and worker.obs_stats is not None:
-            worker.obs_stats.copy_(torch.as_tensor(np.asarray(stats, dtype=np.float32)))
-        rewards = worker.test_returns(sol, config.test_repetitions)
-    else:
-        rewards = [float(-worker.run(sol)[0]) for _ in range(config.test_repetitions)]
+    if stats is not None and worker.obs_stats is not None:
+        worker.obs_stats.copy_(torch.as_tensor(np.asarray(stats, dtype=np.float32)))
+    rewards = worker.test_returns(sol, config.test_repetitions)
     return np.mean(rewards), np.std(rewards) / config.repetitions

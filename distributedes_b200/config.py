@@ -7,6 +7,7 @@ from __future__ import annotations
 import numpy as np
 
 from .envs import DeviceEnv, TapeEnv
+from .fitness import POLICY_WIDTHS
 from .model import StandardFCNet
 from .utils import Adam
 
@@ -65,9 +66,9 @@ class ClosedLoopPendulumConfig(BasicConfig):
     def __init__(self, hidden_size=64):
         # limits of des_rollout_eval (csrc/des_envs.cu): checked here, not at the first generation.  16 is the reference's
         # own PendulumConfig default (config.py:27) and the width its CMA-ES driver uses (cma_es.py:129).
-        if hidden_size not in (16, 32, 64, 96, 128):
-            raise ValueError('ClosedLoopPendulumConfig: hidden_size must be 16, 32, 64, 96 or 128 on the device path (got %r)'
-                             % (hidden_size,))
+        if hidden_size not in POLICY_WIDTHS:
+            raise ValueError('ClosedLoopPendulumConfig: hidden_size must be one of %s on the device path (got %r)'
+                             % (POLICY_WIDTHS, hidden_size))
         self.task = 'Pendulum-v0'
         self.clip = 2.0
         self.action_clip = lambda a: np.clip(a, -2, 2)
@@ -91,15 +92,15 @@ class BipedalWalkerConfig(SynthTapeConfig):
 class HostEnvConfig(BasicConfig):
     """Any environment with the classic gym API (reset() -> obs, step(a) -> (obs, reward, done, info), optionally
     seed(s)), stepped on the host by the user's own code, with the population's policy step on the device
-    (engine.HostEnvEngine for NES, cma_es.Worker for CMA-ES).  The reference's BasicConfig (config.py:5-21): env_fn is
+    (fitness.HostRollouts, for NES and CMA-ES).  The reference's BasicConfig (config.py:5-21): env_fn is
     probed for state_dim / action_dim, 10 repetitions and 10 test repetitions (config.py:8-9), the observation
     normaliser on.  `batch_env_fn(num_slots)`, if given, builds a vectorised environment implementing the batch protocol
     of envs.py (otherwise envs.GymEnvBatch wraps num_slots environments from env_fn)."""
 
     def __init__(self, env_fn, hidden_size=16, clip=1.0, task=None, batch_env_fn=None):
-        if hidden_size not in (16, 32, 64, 96, 128):
-            raise ValueError('HostEnvConfig: hidden_size must be 16, 32, 64, 96 or 128 (des_policy_act); got %r'
-                             % (hidden_size,))
+        if hidden_size not in POLICY_WIDTHS:
+            raise ValueError('HostEnvConfig: hidden_size must be one of %s (des_policy_act); got %r'
+                             % (POLICY_WIDTHS, hidden_size))
         self.env_fn = env_fn
         self.batch_env_fn = batch_env_fn
         self.task = task if task is not None else 'host-env'

@@ -38,8 +38,9 @@ class TapeEnv:
 
 class DeviceEnv:
     """Shape descriptor of an environment that is stepped INSIDE des_rollout_eval (closed loop, per-member
-    observations): there is no host-side step().  'Pendulum-v0': config.py:26-31."""
-    SPECS = {'Pendulum-v0': dict(state_dim=3, action_dim=1, horizon=200, clip=2.0)}
+    observations): there is no host-side step().  SPECS is the table of them; `env` is the library's environment id
+    (DES_ENV_PENDULUM = 0).  'Pendulum-v0': config.py:26-31."""
+    SPECS = {'Pendulum-v0': dict(env=0, state_dim=3, action_dim=1, horizon=200, clip=2.0)}
 
     def __init__(self, task):
         if task not in self.SPECS:

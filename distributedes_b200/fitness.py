@@ -1,0 +1,337 @@
+"""Fitness sources, one per kind of environment: the tape (Tape), episodes stepped on the device (DeviceRollouts) and
+episodes stepped on the host (HostRollouts).  engine.NESEngine and cma_es.Worker evaluate through one and never ask
+which.  A source evaluates NES members theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
+holds the normaliser statistics `obs_stats` [m | v | n] (or None) and the fp64 observation totals `obs_totals` of its
+last evaluation, shares and merges them, counts its environment steps and says whether a CUDA graph may capture it."""
+from __future__ import annotations
+
+import numpy as np
+import torch
+import torch.distributed as dist
+
+from .envs import TEST_MEMBER, DeviceEnv, GymEnvBatch
+
+POLICY_WIDTHS = (16, 32, 64, 96, 128)     # hidden widths des_rollout_eval and des_policy_act take (H/16 units per lane)
+
+
+class Tape:
+    """Fitness on the observation tape.  NES members go through des_nes_eval (after des_obs_normalize of the tape with
+    the statistics of the previous generations, when normalising); explicit rows through des_pop_eval, without a
+    normaliser.  Every member sees the whole tape, so the statistics merge needs no collective."""
+
+    test_repetitions = 1          # the tape is deterministic
+
+    def __init__(self, kernels, device, obs, target, *, state_dim, hidden, action_dim, clip, repetitions=1,
+                 normalize_obs=False, sigma=None, seed=0, precision='fp32', mirrored=False):
+        self.k, self.device = kernels, torch.device(device)
+        self.d0, self.H, self.A, self.clip = int(state_dim), int(hidden), int(action_dim), float(clip)
+        self.repetitions, self.normalize_obs = int(repetitions), bool(normalize_obs)
+        self.sigma, self.seed, self.precision, self.mirrored = sigma, int(seed), precision, bool(mirrored)
+        self.obs_stats = torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device) if self.normalize_obs else None
+        self.obs_totals = self.obs_raw = self.T = self.eval_ws = None
+        self.set_tape(obs, target)
+
+    def set_tape(self, obs, target):
+        """Returns whether the buffers moved: a tape of the current shape is copied in place (stable for a graph)."""
+        obs = torch.as_tensor(obs, dtype=torch.float32)
+        target = torch.as_tensor(target, dtype=torch.float32)
+        if obs.dim() != 2 or obs.shape[1] != self.d0 or target.dim() != 2 or target.shape[1] != self.A \
+                or target.shape[0] != obs.shape[0]:
+            raise ValueError('tape shapes %r / %r do not match (T,%d) / (T,%d)' %
+                             (tuple(obs.shape), tuple(target.shape), self.d0, self.A))
+        if self.obs_raw is not None and self.obs_raw.shape == obs.shape:
+            self.obs_raw.copy_(obs, non_blocking=True)
+            self.target.copy_(target, non_blocking=True)
+            return False
+        self.obs_raw = obs.to(self.device).contiguous()
+        self.target = target.to(self.device).contiguous()
+        # what the kernels read: the raw tape, or its normalised image refreshed every generation
+        self.obs = torch.empty_like(self.obs_raw) if self.normalize_obs else self.obs_raw
+        if int(obs.shape[0]) != self.T and hasattr(self.k, 'eval_workspace'):
+            # a new tape length may be a multi-pass tensor-core shape: size its tile cache for the new T
+            self.eval_ws = self.k.eval_workspace(self.d0, self.H, self.A, int(obs.shape[0]), self.precision, self.device)
+        self.T = int(obs.shape[0])
+        return True
+
+    def members(self, theta, *, state, generation, offset, n_local, out):
+        if self.normalize_obs:        # utils.py:48-51 with the statistics of the previous generations
+            self.k.obs_normalize(self.obs_raw, self.obs_stats, out=self.obs)
+        if n_local:
+            (self.k.nes_eval_mirrored if self.mirrored else self.k.nes_eval)(
+                theta, self.obs, self.target, hidden=self.H, sigma=self.sigma, clip=self.clip, seed=self.seed,
+                state=state, member_offset=offset, n_local=n_local, precision=self.precision, out=out,
+                workspace=self.eval_ws)
+
+    def solutions(self, solutions, *, offset, generation, out=None):
+        return self.k.pop_eval(solutions, self.obs, self.target, hidden=self.H, clip=self.clip, out=out)
+
+    def test_returns(self, solution, repetitions, generation, state=None):
+        """`repetitions` evaluations of one solution, one launch each as the reference's test() loops run them: NES's
+        through the normaliser with des_nes_eval at sigma = 0, CMA-ES's (no sigma) as one row of des_pop_eval."""
+        out = []
+        for _ in range(repetitions):
+            if self.sigma is None:
+                f = self.solutions(solution.reshape(1, -1), offset=0, generation=generation)
+            else:
+                obs = self.k.obs_normalize(self.obs_raw, self.obs_stats) if self.normalize_obs else self.obs_raw
+                f = self.k.nes_eval(solution, obs, self.target, hidden=self.H, sigma=0.0, clip=self.clip, seed=self.seed,
+                                    generation=0, member_offset=0, n_local=1, precision='fp32')
+            out.append(float(f[0]))
+        return np.asarray(out)
+
+    def share_totals(self, world, pg):
+        pass
+
+    def merge(self, N):
+        if self.normalize_obs:
+            # natural_es.py:85-89: every member saw the whole tape, so every rank merges the same online statistics
+            self.k.obs_stats_merge(self.obs_stats, self.obs_raw, N * self.T * self.repetitions)
+
+    def steps(self, N, world, pg):
+        return N * self.repetitions * self.T
+
+    def capturable(self, world):
+        return True
+
+
+class _Episodes:
+    """The statistics of the states episodes visit: each rank sums its members' raw observations in fp64, and one
+    (2*d0+1)-double all-reduce replaces the per-worker Chan merges of natural_es.py:85-89 / cma_es.py:92-96."""
+
+    def __init__(self, kernels, device, *, state_dim, hidden, clip, action_noise_std, seed, repetitions, normalize_obs,
+                 sigma, mirrored):
+        if int(hidden) not in POLICY_WIDTHS:
+            raise ValueError('%s: hidden must be one of %s (the device policy keeps H/16 units per lane); got %r'
+                             % (type(self).__name__, POLICY_WIDTHS, hidden))
+        self.k, self.device = kernels, torch.device(device)
+        self.d0, self.H, self.clip = int(state_dim), int(hidden), float(clip)
+        self.action_noise_std, self.seed, self.repetitions = float(action_noise_std), int(seed), int(repetitions)
+        self.normalize_obs, self.sigma, self.mirrored = bool(normalize_obs), sigma, bool(mirrored)
+        w = 2 * self.d0 + 1
+        self.obs_stats = torch.zeros(w, dtype=torch.float32, device=self.device) if self.normalize_obs else None
+        self.obs_totals = torch.zeros(w, dtype=torch.float64, device=self.device)
+
+    def set_tape(self, obs, target):
+        raise TypeError('%s steps its environments; there is no tape to set' % type(self).__name__)
+
+    def share_totals(self, world, pg):
+        if world > 1 and self.normalize_obs:
+            dist.all_reduce(self.obs_totals, group=pg)
+
+    def merge(self, N):
+        if self.normalize_obs:
+            self.k.obs_stats_merge_totals(self.obs_stats, self.obs_totals, self.d0)
+
+
+class DeviceRollouts(_Episodes):
+    """Closed-loop episodes stepped on the device (SURVEY 8f row 3): Evaluator.eval utils.py:116-124 runs `repetitions`
+    episodes per member, every member seeing its own observations.  Environment: a DeviceEnv task."""
+
+    def __init__(self, kernels, device, *, task, hidden, repetitions, clip=None, horizon=None, **kw):
+        if task not in DeviceEnv.SPECS:
+            raise ValueError('closed-loop environments available on the device: %s (got %r)' % (sorted(DeviceEnv.SPECS), task))
+        spec = DeviceEnv.SPECS[task]
+        super().__init__(kernels, device, state_dim=spec['state_dim'], hidden=hidden,
+                         clip=spec['clip'] if clip is None else clip, repetitions=repetitions, **kw)
+        self.env_id, self.A, self.horizon = spec['env'], spec['action_dim'], int(horizon or spec['horizon'])
+        self.T, self.test_repetitions = self.horizon, self.repetitions
+        self.roll_ws = None
+
+    def _workspace(self, n):
+        w = 2 * self.d0 + 1
+        if self.roll_ws is None or self.roll_ws.numel() < n * w:
+            self.roll_ws = torch.empty(n * w, dtype=torch.float64, device=self.device)
+        return self.roll_ws
+
+    def _env(self):
+        return dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip,
+                    action_noise_std=self.action_noise_std, seed=self.seed)
+
+    def members(self, theta, *, state, generation, offset, n_local, out):
+        self.obs_totals.zero_()
+        if n_local:
+            (self.k.rollout_eval_mirrored if self.mirrored else self.k.rollout_eval)(
+                theta, repetitions=self.repetitions, sigma=self.sigma, state=state, member_offset=offset, n_local=n_local,
+                obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                workspace=self._workspace(n_local), out=out, **self._env())
+
+    def solutions(self, solutions, *, offset, generation, out=None):
+        n = int(solutions.shape[0])
+        self.obs_totals.zero_()
+        out = out if out is not None else torch.zeros(n, dtype=torch.float32, device=self.device)
+        if n:
+            self.k.rollout_eval_solutions(solutions, repetitions=self.repetitions, generation=generation,
+                                          member_offset=offset, obs_stats=self.obs_stats,
+                                          totals_out=self.obs_totals if self.normalize_obs else None,
+                                          workspace=self._workspace(n), out=out, **self._env())
+        return out
+
+    def test_returns(self, solution, repetitions, generation, state=None):
+        """Noiseless episodes from the test stream, keyed by the generation word in `state` if given, else `generation`."""
+        sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
+        episodes = torch.empty(int(repetitions), dtype=torch.float32, device=self.device)
+        word = dict(state=state) if state is not None else dict(generation=generation)
+        self.k.rollout_eval(sol, repetitions=int(repetitions), sigma=0.0, member_offset=0, n_local=1, noiseless=True,
+                            obs_stats=self.obs_stats, episodes_out=episodes, **word, **self._env())
+        return episodes.cpu().numpy().astype(np.float64)
+
+    def steps(self, N, world, pg):
+        return N * self.repetitions * self.horizon
+
+    def capturable(self, world):
+        return world == 1 or not self.normalize_obs      # sharded, the observation totals travel through NCCL
+
+
+class HostEpisodes:
+    """The bridge between environments stepped on the host and the population's policy on the device: runs the episodes
+    of `n` weight rows x `repetitions` in lockstep until every slot is done (Evaluator.eval / single_run,
+    utils.py:116-139).  Per step: observations -> pinned buffer -> device, des_policy_act, actions -> host, env.step,
+    fp64 return accumulation per slot.  Slot b = i * repetitions + r of the batch environment is episode r of row i.
+
+    `batch_env` implements the protocol of envs.py (num_envs, reset(keys), step(actions, alive)); its num_envs must be
+    n * repetitions."""
+
+    def __init__(self, kernels, device, batch_env, n, repetitions, state_dim, hidden, action_dim, clip, action_noise_std,
+                 seed):
+        self.k, self.device, self.env = kernels, torch.device(device), batch_env
+        self.n, self.reps = int(n), int(repetitions)
+        self.d0, self.H, self.A = int(state_dim), int(hidden), int(action_dim)
+        self.clip, self.action_noise_std, self.seed = float(clip), float(action_noise_std), int(seed)
+        B = self.n * self.reps
+        if int(batch_env.num_envs) != B:
+            raise ValueError('the batch environment has %d slots; %d members x %d repetitions need %d'
+                             % (batch_env.num_envs, self.n, self.reps, B))
+        pin = self.device.type == 'cuda'
+        self.obs_h = torch.empty((B, self.d0), dtype=torch.float32, pin_memory=pin)
+        self.alive_h = torch.empty(B, dtype=torch.uint8, pin_memory=pin)
+        self.act_h = torch.empty((B, self.A), dtype=torch.float32, pin_memory=pin)
+        self.obs_d = torch.empty((B, self.d0), dtype=torch.float32, device=self.device)
+        self.alive_d = torch.empty(B, dtype=torch.uint8, device=self.device)
+        self.act_d = torch.empty((B, self.A), dtype=torch.float32, device=self.device)
+
+    def run(self, rows, *, generation, member_offset=0, key_member=None, obs_stats=None, stat_part=None):
+        """Returns (returns[n, repetitions] fp64, environment steps taken).  Episode (i, r) resets with the key
+        (generation, member_offset + i, r), or (generation, key_member, r) when key_member is given (test episodes,
+        whose action noise then uses member 0 as des_rollout_eval's test episodes do)."""
+        n, reps, B = self.n, self.reps, self.n * self.reps
+        if B == 0:
+            return np.zeros((n, reps)), 0
+        members = (np.full(n, int(key_member), dtype=np.int64) if key_member is not None
+                   else int(member_offset) + np.arange(n, dtype=np.int64))
+        keys = np.stack([np.full(B, int(generation) & 0xFFFFFFFF, dtype=np.int64), np.repeat(members, reps),
+                         np.tile(np.arange(reps, dtype=np.int64), n)], axis=1)
+        noise_offset = 0 if key_member is not None else int(member_offset)
+        obs = self.env.reset(keys)
+        alive = np.ones(B, dtype=bool)
+        returns = np.zeros(B, dtype=np.float64)
+        steps, t = 0, 0
+        cuda = self.device.type == 'cuda'
+        obs_h, alive_h, act_h = self.obs_h.numpy(), self.alive_h.numpy(), self.act_h.numpy()
+        while alive.any():
+            obs_h[:] = obs                                              # fp32 cast: FloatTensor(o), utils.py:42-45
+            alive_h[:] = alive
+            self.obs_d.copy_(self.obs_h, non_blocking=True)
+            self.alive_d.copy_(self.alive_h, non_blocking=True)
+            self.k.policy_act(rows, self.obs_d, self.alive_d, state_dim=self.d0, hidden=self.H, action_dim=self.A,
+                              repetitions=reps, clip=self.clip, action_noise_std=self.action_noise_std, seed=self.seed,
+                              generation=generation, member_offset=noise_offset, t=t, obs_stats=obs_stats,
+                              stat_part=stat_part, out=self.act_d)
+            self.act_h.copy_(self.act_d, non_blocking=True)
+            if cuda:
+                torch.cuda.current_stream(self.device).synchronize()
+            obs, reward, done = self.env.step(act_h, alive)
+            returns[alive] += np.asarray(reward, dtype=np.float64)[alive]      # utils.py:137
+            steps += int(alive.sum())
+            alive &= ~np.asarray(done, dtype=bool)
+            t += 1
+        return returns.reshape(n, reps), steps
+
+
+class HostRollouts(_Episodes):
+    """Episodes stepped on the HOST by the user's own code, the per-step policy on the device (des_policy_act):
+    Evaluator.eval utils.py:116-124.  NES members become rows theta + sigma*eps once per generation (des_nes_perturb,
+    natural_es.py:28-30).  The step count is the episodes' real length, summed over ranks (natural_es.py:75,
+    cma_es.py:73).  batch_env_fn(num_slots) builds a batch environment (envs.py); the default wraps env_fn in
+    envs.GymEnvBatch."""
+
+    def __init__(self, kernels, device, *, env_fn, state_dim, action_dim, hidden, repetitions, test_repetitions=None,
+                 batch_env_fn=None, **kw):
+        super().__init__(kernels, device, state_dim=state_dim, hidden=hidden, repetitions=repetitions, **kw)
+        self.A, self.test_repetitions = int(action_dim), int(test_repetitions or repetitions)
+        if batch_env_fn is None:
+            batch_env_fn = lambda B: GymEnvBatch(env_fn, B, self.seed)      # noqa: E731
+        self.batch_env_fn = batch_env_fn
+        self._bridges = {}            # (rows, repetitions) -> HostEpisodes
+        self.rows = self.stat_part = None
+        self.last_steps = 0           # environment steps of the last evaluation on this rank
+
+    def _bridge(self, n, reps):
+        ep = self._bridges.get((n, reps))
+        if ep is None:
+            ep = HostEpisodes(self.k, self.device, self.batch_env_fn(n * reps), n, reps, self.d0, self.H, self.A,
+                              self.clip, self.action_noise_std, self.seed)
+            self._bridges[(n, reps)] = ep
+        return ep
+
+    def members(self, theta, *, state, generation, offset, n_local, out):
+        self.obs_totals.zero_()
+        self.last_steps = 0
+        if n_local:
+            if self.rows is None:
+                self.rows = torch.empty((n_local, theta.numel()), dtype=torch.float32, device=self.device)
+            (self.k.nes_perturb_mirrored if self.mirrored else self.k.nes_perturb)(theta, n_local, self.sigma, self.seed, generation,
+                                                      member_offset=offset, out=self.rows)
+            self._episodes(self.rows, offset, generation, out)
+
+    def solutions(self, solutions, *, offset, generation, out=None):
+        n = int(solutions.shape[0])
+        self.obs_totals.zero_()
+        self.last_steps = 0
+        out = out if out is not None else torch.zeros(n, dtype=torch.float32, device=self.device)
+        if n:
+            self._episodes(solutions.to(device=self.device, dtype=torch.float32).contiguous(), offset, generation, out)
+        return out
+
+    def _episodes(self, rows, offset, generation, out):
+        n = int(rows.shape[0])
+        if self.stat_part is None or self.stat_part.shape[0] != n:
+            self.stat_part = torch.zeros((n, 2 * self.d0 + 1), dtype=torch.float64, device=self.device)
+        else:
+            self.stat_part.zero_()
+        part = self.stat_part if self.normalize_obs else None
+        ret, self.last_steps = self._bridge(n, self.repetitions).run(rows, generation=generation, member_offset=offset,
+                                                                     obs_stats=self.obs_stats, stat_part=part)
+        out.copy_(torch.from_numpy(ret.mean(axis=1).astype(np.float32)))       # -cost, utils.py:124
+        if part is not None:
+            self.k.obs_parts_reduce(part, self.d0, out=self.obs_totals)
+
+    def test_returns(self, solution, repetitions, generation, state=None):
+        """Episodes keyed (generation, TEST_MEMBER, repetition), which do not feed the statistics; `state` is not read."""
+        row = solution.reshape(1, -1).to(device=self.device, dtype=torch.float32).contiguous()
+        ret, _ = self._bridge(1, int(repetitions)).run(row, generation=generation, key_member=TEST_MEMBER,
+                                                       obs_stats=self.obs_stats)
+        return ret[0]
+
+    def steps(self, N, world, pg):
+        total = torch.tensor([self.last_steps], dtype=torch.int64, device=self.device)
+        if world > 1:
+            dist.all_reduce(total, group=pg)
+        return int(total.item())
+
+    def capturable(self, world):
+        return False
+
+
+def from_config(config, kernels, device):
+    """The source a config describes: `host_env` configs step on the host, `closed_loop` ones on the device, the rest
+    read the tape of config.env_fn() (CMA-ES: without a normaliser)."""
+    kw = dict(hidden=config.hidden_size, clip=config.clip, seed=getattr(config, 'seed', 0), repetitions=config.repetitions)
+    episodes = dict(action_noise_std=config.action_noise_std, normalize_obs=getattr(config, 'normalize_obs', True),
+                    sigma=None, mirrored=False)
+    if getattr(config, 'host_env', False):
+        return HostRollouts(kernels, device, env_fn=config.env_fn, batch_env_fn=getattr(config, 'batch_env_fn', None),
+                            state_dim=config.state_dim, action_dim=config.action_dim, **episodes, **kw)
+    if getattr(config, 'closed_loop', False):
+        return DeviceRollouts(kernels, device, task=config.task, **episodes, **kw)
+    env = config.env_fn()
+    return Tape(kernels, device, env.obs, env.target, state_dim=env.obs.shape[1], action_dim=env.target.shape[1], **kw)

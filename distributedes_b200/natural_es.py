@@ -75,7 +75,6 @@ def train(config, engine=None):
     stats = SharedStats(config.state_dim)
     engine = engine if engine is not None else build_engine(config)
     worker = Worker(engine.rank, None, StaticNormalizer(config.state_dim), None, None, None, config, engine=engine)
-    steps_per_generation = config.pop_size * config.repetitions * engine.T
 
     training_rewards, training_steps, training_timestamps = [], [], []
     initial_time = time.time()
@@ -92,8 +91,7 @@ def train(config, engine=None):
 
         worker.run()                                                           # :62-73 (evaluate + gather)
         rewards = engine.fitness_all
-        # :75 sums the episodes' real lengths: engines that step their environments until done report them
-        total_steps += engine.steps_taken if hasattr(engine, 'steps_taken') else steps_per_generation
+        total_steps += engine.steps_taken                                      # :75, the episodes' real lengths
         r_mean = float(rewards.mean())
         r_std = float(rewards.std(unbiased=False))
         if engine.rank == 0:
@@ -112,10 +110,8 @@ def train(config, engine=None):
 def test(config, solution, stats, engine=None):
     """natural_es.py:101-110: mean and 'ste' of test_repetitions noiseless episodes of `solution`
     (None = the engine's current parameters)."""
-    if engine is not None and hasattr(engine, 'test_returns'):      # closed loop: distinct reset states per episode
+    if engine is not None:
         rewards = engine.test_returns(solution, config.test_repetitions)
-    elif engine is not None:
-        rewards = [engine.noiseless_fitness(solution) for _ in range(config.test_repetitions)]
     else:
         normalizer = StaticNormalizer(config.state_dim)
         normalizer.offline_stats.load_state_dict(stats.state_dict())

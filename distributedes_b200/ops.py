@@ -12,6 +12,7 @@ import torch
 
 from . import _lib
 from ._lib import Dims, Opt, PRECISIONS, State
+from .envs import DeviceEnv
 
 
 def _stream():
@@ -129,7 +130,12 @@ def obs_normalize(obs, stats, out=None):
     return out
 
 
-ENV_DIMS = {0: (3, 1)}      # DES_ENV_PENDULUM: (state_dim, action_dim)
+def _env_dims(env):
+    """(state_dim, action_dim) of the device environment with library id `env` (envs.DeviceEnv.SPECS)."""
+    for spec in DeviceEnv.SPECS.values():
+        if spec['env'] == env:
+            return spec['state_dim'], spec['action_dim']
+    raise RuntimeError('unknown environment id %r' % (env,))
 
 
 def rollout_eval(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, clip, action_noise_std=0.0, seed,
@@ -154,9 +160,7 @@ def rollout_eval_mirrored(theta, *, env=0, hidden, horizon=200, repetitions=10, 
 
 def _rollout(fn, theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed, generation, state,
              member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out, episodes_out):
-    if env not in ENV_DIMS:
-        raise RuntimeError('unknown environment id %r' % (env,))
-    d0, A = ENV_DIMS[env]
+    d0, A = _env_dims(env)
     if out is None:
         out = torch.empty(n_local, dtype=torch.float32, device=theta.device)
     if totals_out is not None and workspace is None:
@@ -178,9 +182,7 @@ def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions
                            episodes_out=None):
     """Closed-loop fitness of explicit solutions[n_local, P] (CMA-ES's ask() rows, cma_es.py:22-29): row i is global
     member member_offset + i, whose episodes reset from the same counter stream as rollout_eval's member."""
-    if env not in ENV_DIMS:
-        raise RuntimeError('unknown environment id %r' % (env,))
-    d0, A = ENV_DIMS[env]
+    d0, A = _env_dims(env)
     if solutions.dim() != 2:
         raise RuntimeError('solutions must be [n_local, P], got shape %r' % (tuple(solutions.shape),))
     n_local, P = solutions.shape

@@ -19,7 +19,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from distributedes_b200 import ops                       # noqa: E402
-from distributedes_b200.engine import HostEpisodes       # noqa: E402
+from distributedes_b200.fitness import HostEpisodes       # noqa: E402
 from oracle import nes_oracle as orc                     # noqa: E402
 from oracle import pendulum_oracle as po                 # noqa: E402
 

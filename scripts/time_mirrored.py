@@ -52,8 +52,9 @@ def time_engine(eng, steps, flush):
         e[2].record()
         eng.k.centered_rank(eng.fitness_all, eng.offset, eng.n_local, workspace=eng.rank_ws, out=eng.shaped)
         e[3].record()
-        eng._op('nes_grad_partial')(eng.shaped, eng.P, seed=eng.seed, state=eng.state, member_offset=eng.offset,
-                                    workspace=eng.grad_ws, out=eng.partial)
+        grad = eng.k.nes_grad_partial_mirrored if eng.mirrored else eng.k.nes_grad_partial
+        grad(eng.shaped, eng.P, seed=eng.seed, state=eng.state, member_offset=eng.offset, workspace=eng.grad_ws,
+             out=eng.partial)
         e[4].record()
         eng.apply()
         e[5].record()
