@@ -26,7 +26,6 @@ constexpr int kActThreads = 128;
 constexpr int kActMaxReps = 16;        // the action-noise counter packs member*16 + repetition
 constexpr int kActMaxD0 = 32;
 constexpr int kActMaxA = 8;
-constexpr uint32_t kStreamActNoiseHost = 3u;   // the rollout kernel's action-noise stream (kStreamActNoise)
 
 struct ActArgs {
     float *actions;                    // [n_local][reps][A]
@@ -184,7 +183,7 @@ __global__ void __launch_bounds__(kActThreads) policy_act_kernel(ActArgs a) {
         float act = p[0] + b3s[c];
         if (a.act_noise != 0.f) {                                            // utils.py:133
             const float4 z = noise_quad(a.t + ((uint32_t)(c >> 2) << 31), member * 16u + (uint32_t)r, a.gen,
-                                        kStreamActNoiseHost, a.key);
+                                        kStreamActNoise, a.key);
             const int cc = c & 3;
             const float zc = cc == 0 ? z.x : cc == 1 ? z.y : cc == 2 ? z.z : z.w;
             act = __fmaf_rn(zc, a.act_noise, act);
@@ -204,8 +203,7 @@ extern "C" DES_API int des_policy_act(float *actions_out_dev, double *stat_part_
     using namespace des;
     const char *who = "des_policy_act";
     const int H = dims.hidden, d0 = dims.state_dim, A = dims.action_dim;
-    DES_REQUIRE(H == 16 || H == 32 || H == 64 || H == 96 || H == 128,
-                "%s: hidden must be 16, 32, 64, 96 or 128 (got %d)", who, H);
+    DES_REQUIRE(policy_width_ok(H), "%s: hidden must be 16, 32, 64, 96 or 128 (got %d)", who, H);
     DES_REQUIRE(d0 >= 1 && d0 <= kActMaxD0, "%s: state_dim must be in [1, %d] (got %d)", who, kActMaxD0, d0);
     DES_REQUIRE(A >= 1 && A <= kActMaxA, "%s: action_dim must be in [1, %d] (got %d)", who, kActMaxA, A);
     DES_REQUIRE(repetitions >= 1 && repetitions <= kActMaxReps,
@@ -213,8 +211,7 @@ extern "C" DES_API int des_policy_act(float *actions_out_dev, double *stat_part_
                 kActMaxReps, repetitions);
     const Layout L(d0, H, A);
     DES_REQUIRE(P == L.P, "%s: rows have P = %lld, the (%d,%d,%d) MLP needs %d", who, (long long)P, d0, H, A, L.P);
-    DES_REQUIRE(n_local >= 0 && member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 28,
-                "%s: bad member range", who);
+    DES_REQUIRE(member_range_ok(member_offset, n_local, 28), "%s: bad member range", who);
     DES_REQUIRE(t >= 0 && t < ((int64_t)1 << 31), "%s: step index must be in [0, 2^31)", who);
     DES_REQUIRE(alive_dev, "%s: NULL alive mask", who);
     if (n_local == 0) return DES_OK;
@@ -227,20 +224,13 @@ extern "C" DES_API int des_policy_act(float *actions_out_dev, double *stat_part_
     a.key = make_philox_key(seed); a.gen = (uint32_t)generation; a.t = (uint32_t)t;
     a.member_offset = (uint64_t)member_offset;
     const size_t smem = sizeof(float) * act_smem_floats(d0, H, A);
-    cudaStream_t st = (cudaStream_t)stream;
-#define DES_ACT_LAUNCH(HH)                                                                                          \
-    do {                                                                                                            \
-        DES_CUDA(cudaFuncSetAttribute(policy_act_kernel<HH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        policy_act_kernel<HH><<<(unsigned)n_local, kActThreads, smem, st>>>(a);                                     \
-    } while (0)
+    void (*kernel)(ActArgs);
     switch (H) {
-        case 16: DES_ACT_LAUNCH(16); break;
-        case 32: DES_ACT_LAUNCH(32); break;
-        case 64: DES_ACT_LAUNCH(64); break;
-        case 96: DES_ACT_LAUNCH(96); break;
-        default: DES_ACT_LAUNCH(128); break;
+        case 16: kernel = policy_act_kernel<16>; break;
+        case 32: kernel = policy_act_kernel<32>; break;
+        case 64: kernel = policy_act_kernel<64>; break;
+        case 96: kernel = policy_act_kernel<96>; break;
+        default: kernel = policy_act_kernel<128>; break;
     }
-#undef DES_ACT_LAUNCH
-    DES_LAUNCH_CHECK("policy_act_kernel");
-    return DES_OK;
+    return launch_smem("policy_act_kernel", kernel, (unsigned)n_local, kActThreads, smem, (cudaStream_t)stream, a);
 }

@@ -21,6 +21,12 @@ int cuda_fail(cudaError_t e, const char *what) {
     return (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver) ? DES_ERR_NO_DEVICE : DES_ERR_CUDA;
 }
 
+int not_whole_pairs(const char *who, const char *count, int64_t member_offset, int64_t n) {
+    set_error("%s: a mirrored shard holds whole pairs: member_offset (%lld) and %s (%lld) must be even", who,
+              (long long)member_offset, count, (long long)n);
+    return DES_ERR_INVALID_ARGUMENT;
+}
+
 int eval_ffma_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                      double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
                      int64_t member_offset, int64_t n_local, const float *solutions, bool mirrored, cudaStream_t st);
@@ -79,10 +85,8 @@ static int nes_eval(const char *who, float *fitness_out_dev, const float *theta_
     DES_REQUIRE(des_param_count(dims.state_dim, dims.hidden, dims.action_dim) < ((int64_t)1 << 31),
                 "%s: parameter count exceeds 2^31", who);
     DES_REQUIRE(n_local >= 0 && n_local < ((int64_t)1 << 31), "%s: bad n_local=%lld", who, (long long)n_local);
-    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32, "%s: member index must fit 32 bits", who);
-    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0),
-                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
-                (long long)member_offset, (long long)n_local);
+    DES_REQUIRE(member_range_ok(member_offset, n_local, 32), "%s: member index must fit 32 bits", who);
+    if (mirrored && !whole_pairs(member_offset, n_local)) return not_whole_pairs(who, "n_local", member_offset, n_local);
     DES_REQUIRE(clip >= 0.0, "%s: clip must be >= 0", who);
     if (n_local == 0) return DES_OK;
     DES_REQUIRE(fitness_out_dev && theta_dev && obs_dev && target_dev, "%s: NULL pointer", who);

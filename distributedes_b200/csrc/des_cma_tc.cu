@@ -237,10 +237,8 @@ int cma_rank_mu_tc(float *out_dev, const float *Y_dev, const float *w_dev, int64
     a.ptiles_per_side = (int)((n + a.ptile - 1) / a.ptile);
     const int64_t tiles = (int64_t)a.tiles * (a.tiles + 1) / 2;
     const size_t smem = 1024 + (size_t)kStages * kStageBytes + sizeof(Bars);
-    DES_CUDA(cudaFuncSetAttribute(cma_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cma_syrk_kernel<<<(unsigned)tiles, kThreads, smem, st>>>(a, maps[0], maps[1], maps[2], maps[3]);
-    DES_LAUNCH_CHECK("cma_syrk_kernel");
-    return DES_OK;
+    return launch_smem("cma_syrk_kernel", cma_syrk_kernel, (unsigned)tiles, kThreads, smem, st, a, maps[0], maps[1], maps[2],
+                       maps[3]);
 }
 
 }  // namespace des

@@ -58,8 +58,14 @@ constexpr uint32_t kPhiloxM0 = 0xD2511F53u;
 constexpr uint32_t kPhiloxM1 = 0xCD9E8D57u;
 constexpr uint32_t kPhiloxW0 = 0x9E3779B9u;
 constexpr uint32_t kPhiloxW1 = 0xBB67AE85u;
+// Counter streams (the fourth counter word): NES perturbations, CMA-ES samples, environment resets, action noise.  The
+// host-stepped policy (des_act.cu) draws its action noise exactly as the device rollout (des_envs.cu) does.
 constexpr uint32_t kStreamNesEps = 0u;
 constexpr uint32_t kStreamCmaZ = 1u;
+constexpr uint32_t kStreamEnvReset = 2u;
+constexpr uint32_t kStreamActNoise = 3u;
+// Member word of the test episodes' resets (test(), natural_es.py:101-110): no member of a population reaches it.
+constexpr uint32_t kTestEpisodeMember = 0x40000000u;
 
 // Round keys k + r*W precomputed on the host (kernel-parameter constant bank): the xor takes them as
 // constant operands, so the key schedule costs no instructions.
@@ -207,9 +213,49 @@ __device__ __forceinline__ float4 noise_quad(uint32_t q, uint32_t member, uint32
     return z;
 }
 
-__device__ __forceinline__ uint64_t load_generation(const des_state *st, uint64_t fallback) {
-    return st ? st->generation : fallback;
+// The generation word of the counters: des_state's generation when the caller passes one (graph replay), else `gen`,
+// which is read only then.
+__device__ __forceinline__ uint32_t generation_word(const des_state *state, const uint32_t &gen) {
+    return state ? (uint32_t)state->generation : gen;
 }
+
+// Mirrored sampling: member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1.  fma(-sigma, eps, theta) is exactly
+// fp32(theta - sigma*eps), and the even member of a pair has the bits of the plain member m >> 1.  `member` keeps the
+// caller's integer type: the shift happens in that width.
+template <typename Member>
+__device__ __forceinline__ uint32_t noise_word(Member member, bool mirrored) {
+    return (uint32_t)(mirrored ? member >> 1 : member);
+}
+template <typename Member>
+__device__ __forceinline__ float member_sigma(Member member, bool mirrored, float sigma) {
+    return mirrored && (member & 1u) ? -sigma : sigma;
+}
+
+// ---- entry-point checks and launches (host) ------------------------------------------------------------------------
+// A shard holds the members [member_offset, member_offset + n).  Their indices fit `bits` bits: 32 for the noise counter
+// word, 28 where the action-noise counter packs member*16 + repetition.
+inline bool member_range_ok(int64_t member_offset, int64_t n, int bits) {
+    return n >= 0 && member_offset >= 0 && member_offset + n <= ((int64_t)1 << bits);
+}
+// A mirrored shard holds whole pairs (members 2p and 2p + 1).
+inline bool whole_pairs(int64_t member_offset, int64_t n) { return member_offset % 2 == 0 && n % 2 == 0; }
+// Reports a shard that whole_pairs rejects (`count` names n's argument): DES_ERR_INVALID_ARGUMENT.
+int not_whole_pairs(const char *who, const char *count, int64_t member_offset, int64_t n);
+// Hidden widths of the closed-loop policy kernels (rollout_pendulum_kernel, policy_act_kernel): H/16 units per lane.
+inline bool policy_width_ok(int H) { return H == 16 || H == 32 || H == 64 || H == 96 || H == 128; }
+
+// Opts `kernel` in to `smem` bytes of dynamic shared memory and launches it; the status of both.
+template <typename... Params, typename... Args>
+int launch_smem(const char *name, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                const Args &...args) {
+    DES_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, block, smem, st>>>(args...);
+    DES_LAUNCH_CHECK(name);
+    return DES_OK;
+}
+
+// totals[c] = sum over the n_local rows of parts[n_local][width] (des_obs.cu), in member order
+int obs_parts_reduce(double *totals, const double *parts, int64_t n_local, int width, cudaStream_t st);
 
 // ---- CMA rank-mu (des_cma.cu: fp32 FFMA kernel and the entry point; des_cma_tc.cu: split-fp16 wgmma SYRK) ----------
 constexpr int64_t kCmaTcMinN = 2048;     // n >= this runs on the tensor cores, smaller n on the FFMA kernel

@@ -14,9 +14,6 @@
 namespace des {
 
 constexpr int kEnvPendulum = 0;
-constexpr int kMaxRollH = 128;         // hidden units (R = H/16 per lane, up to 8)
-constexpr uint32_t kStreamEnvReset = 2u;
-constexpr uint32_t kStreamActNoise = 3u;
 
 struct RollArgs {
     float *fitness;                    // [n_local] mean return over the repetitions (higher is better)
@@ -93,7 +90,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
     double *red = reinterpret_cast<double *>(b3s + 4);      // [10][8] per-episode results
     const Layout L = a.L;
     const int lane = threadIdx.x, rg = lane >> 1, eg = lane & 1;
-    const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
+    const uint32_t gen = generation_word(a.state, a.gen);
     const uint32_t member = (uint32_t)(a.member_offset + blockIdx.x);
 
     // flat parameter j of the member -> its place in shared memory
@@ -110,10 +107,9 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
         const float *row = a.rows + (int64_t)blockIdx.x * L.P;
         for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
     } else {
-        // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30); mirrored, the noise
-        // of counter word member >> 1 with sigma negated for the odd member: fma(-sigma, eps, theta) = fp32(theta - sigma*eps)
-        const uint32_t word = a.mirrored ? member >> 1 : member;
-        const float sigma = a.mirrored && (member & 1u) ? -a.sigma : a.sigma;
+        // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30)
+        const uint32_t word = noise_word(member, a.mirrored);
+        const float sigma = member_sigma(member, a.mirrored, a.sigma);
         for (int q = lane; q < (L.P + 3) / 4; q += 32) {
             float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
             if (!a.noiseless) z = noise_quad((uint32_t)q, word, gen, kStreamNesEps, a.key);
@@ -260,34 +256,6 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
     }
 }
 
-// Chan-merge the per-member observation partials (all members of all ranks, after an all-reduce of the three sums) into
-// the shared statistics (utils.py:85-96).  totals = [sum(3) | sumsq(3) | count] in fp64.
-__global__ void obs_stats_merge_totals_kernel(float *__restrict__ stats, const double *__restrict__ totals, int d0) {
-    const int k = threadIdx.x;
-    if (k >= d0) return;
-    const double nB = totals[2 * d0];
-    if (nB <= 0) return;
-    const double mb = totals[k] / nB, vb = fmax(totals[d0 + k] / nB - mb * mb, 0.0);
-    const double nA = (double)stats[2 * d0], n = nA + nB;
-    const double mA = (double)stats[k], vA = (double)stats[d0 + k];
-    const double delta = mb - mA;
-    const double m = mA + delta * nB / n;
-    const double v = (vA * nA + vb * nB + delta * delta * nA * nB / n) / n;
-    __syncthreads();
-    stats[k] = (float)m;
-    stats[d0 + k] = (float)v;
-    if (k == 0) stats[2 * d0] = (float)n;
-}
-
-__global__ void stat_part_reduce_kernel(double *__restrict__ totals, const double *__restrict__ part, int64_t n_local, int width) {
-    // one thread per column, fixed order over members: deterministic
-    const int c = threadIdx.x;
-    if (c >= width) return;
-    double s = 0.0;
-    for (int64_t i = 0; i < n_local; ++i) s += part[i * width + c];
-    totals[c] = s;
-}
-
 // Shared by both entry points: argument checks (before any CUDA work), workspace, launch.  rows_mode selects the
 // explicit-solution kernels: `weights` is then rows[n_local][P] instead of the theta that sigma*eps perturbs.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
@@ -297,17 +265,14 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, cudaStream_t st) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
-    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0 && member_offset >= 0 && n_local >= 0),
-                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
-                (long long)member_offset, (long long)n_local);
+    if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
+        return not_whole_pairs(who, "n_local", member_offset, n_local);
     DES_REQUIRE(!mirrored || !noiseless, "%s: test episodes (noiseless) have no pairs; use des_rollout_eval", who);
     DES_REQUIRE(dims.state_dim == 3 && dims.action_dim == 1, "%s: Pendulum-v0 has state_dim 3, action_dim 1", who);
-    DES_REQUIRE(dims.hidden == 16 || (dims.hidden > 0 && dims.hidden % 32 == 0 && dims.hidden <= kMaxRollH),
-                "%s: hidden must be 16 or a multiple of 32, <= %d (got %d)", who, kMaxRollH, dims.hidden);
+    DES_REQUIRE(policy_width_ok(dims.hidden), "%s: hidden must be 16 or a multiple of 32, <= 128 (got %d)", who, dims.hidden);
     DES_REQUIRE(repetitions >= 1 && repetitions <= 10, "%s: repetitions must be in [1, 10] (one warp each)", who);
     DES_REQUIRE(dims.tape_len >= 1, "%s: episode length (dims.tape_len) must be >= 1", who);
-    DES_REQUIRE(n_local >= 0 && member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 28,
-                "%s: bad member range", who);
+    DES_REQUIRE(member_range_ok(member_offset, n_local, 28), "%s: bad member range", who);
     if (n_local == 0) return DES_OK;
     DES_REQUIRE(fitness_out_dev && weights_dev, "%s: NULL pointer", who);
     RollArgs a;
@@ -319,7 +284,7 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     a.sigma = noiseless ? 0.f : (float)sigma; a.clip = (float)clip; a.act_noise = (float)action_noise_std;
     a.key = make_philox_key(seed); a.gen = (uint32_t)generation;
     a.member_offset = (uint64_t)member_offset;
-    a.reset_member_base = noiseless ? 0x40000000u : (uint32_t)member_offset;     // test episodes use their own reset stream
+    a.reset_member_base = noiseless ? kTestEpisodeMember : (uint32_t)member_offset;
     a.noiseless = noiseless ? 1 : 0;
     a.mirrored = mirrored ? 1 : 0;
     a.stat_part = nullptr;
@@ -334,26 +299,17 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     const int H = dims.hidden;
     const size_t smem = sizeof(float) * ((size_t)H * H + 2 * (size_t)H * kHS + 8 + 40 + (size_t)H * 4 + 3 * (size_t)H + 4) +
                         sizeof(double) * 80;
-#define DES_ROLL_LAUNCH(R)                                                                                          \
-    do {                                                                                                            \
-        auto k__ = rows_mode ? rollout_pendulum_kernel<R, true> : rollout_pendulum_kernel<R, false>;               \
-        DES_CUDA(cudaFuncSetAttribute(k__, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));               \
-        k__<<<(unsigned)n_local, 32, smem, st>>>(a);                                                                \
-    } while (0)
+    void (*kernel)(RollArgs);
     switch (H / 16) {                    // R = H/16 hidden units per lane
-        case 1: DES_ROLL_LAUNCH(1); break;
-        case 2: DES_ROLL_LAUNCH(2); break;
-        case 4: DES_ROLL_LAUNCH(4); break;
-        case 6: DES_ROLL_LAUNCH(6); break;
-        default: DES_ROLL_LAUNCH(8); break;
+        case 1: kernel = rows_mode ? rollout_pendulum_kernel<1, true> : rollout_pendulum_kernel<1, false>; break;
+        case 2: kernel = rows_mode ? rollout_pendulum_kernel<2, true> : rollout_pendulum_kernel<2, false>; break;
+        case 4: kernel = rows_mode ? rollout_pendulum_kernel<4, true> : rollout_pendulum_kernel<4, false>; break;
+        case 6: kernel = rows_mode ? rollout_pendulum_kernel<6, true> : rollout_pendulum_kernel<6, false>; break;
+        default: kernel = rows_mode ? rollout_pendulum_kernel<8, true> : rollout_pendulum_kernel<8, false>; break;
     }
-#undef DES_ROLL_LAUNCH
-    DES_LAUNCH_CHECK("rollout_pendulum_kernel");
-    if (obs_totals_out_dev) {
-        stat_part_reduce_kernel<<<1, 32, 0, st>>>(obs_totals_out_dev, a.stat_part, n_local, 7);
-        DES_LAUNCH_CHECK("stat_part_reduce_kernel");
-    }
-    return DES_OK;
+    const int rc = launch_smem("rollout_pendulum_kernel", kernel, (unsigned)n_local, 32, smem, st, a);
+    if (rc != DES_OK || !obs_totals_out_dev) return rc;
+    return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
 }
 
 }  // namespace des
@@ -394,23 +350,4 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
                                false, (cudaStream_t)stream);
-}
-
-extern "C" DES_API int des_obs_parts_reduce(double *obs_totals_out_dev, const double *parts_dev, int64_t n_local,
-                                            int32_t state_dim, void *stream) {
-    DES_REQUIRE(state_dim > 0 && state_dim <= 511 && n_local >= 0, "des_obs_parts_reduce: bad arguments");
-    DES_REQUIRE(obs_totals_out_dev && (parts_dev || n_local == 0), "des_obs_parts_reduce: NULL pointer");
-    const int width = 2 * state_dim + 1;
-    des::stat_part_reduce_kernel<<<1, (unsigned)((width + 31) / 32 * 32), 0, (cudaStream_t)stream>>>(
-        obs_totals_out_dev, parts_dev, n_local, width);
-    DES_LAUNCH_CHECK("stat_part_reduce_kernel");
-    return DES_OK;
-}
-
-extern "C" DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,
-                                                  void *stream) {
-    DES_REQUIRE(stats_dev && obs_totals_dev && state_dim > 0 && state_dim <= 1024, "des_obs_stats_merge_totals: bad arguments");
-    des::obs_stats_merge_totals_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(stats_dev, obs_totals_dev, state_dim);
-    DES_LAUNCH_CHECK("obs_stats_merge_totals_kernel");
-    return DES_OK;
 }

@@ -80,10 +80,10 @@ __global__ void __launch_bounds__(kThreads) eval_ffma_kernel(EvalArgs a) {
 
     const Layout L = a.L;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
+    const uint32_t gen = generation_word(a.state, a.gen);
     const uint64_t gm = a.member_offset + blockIdx.x;
-    const uint32_t member = (uint32_t)(a.mirrored ? gm >> 1 : gm);       // the counter word of the noise
-    const float sigma = a.mirrored && (gm & 1u) ? -a.sigma : a.sigma;    // fma(-sigma, eps, theta) = fp32(theta - sigma*eps)
+    const uint32_t member = noise_word(gm, a.mirrored);
+    const float sigma = member_sigma(gm, a.mirrored, a.sigma);
     const float *wsrc = FROM_MATRIX ? a.solutions + (int64_t)blockIdx.x * L.P : a.theta;
     double fit = 0.0;                       // meaningful in thread 0 only
 
@@ -204,15 +204,8 @@ int eval_ffma_launch(float *fitness, const float *theta, const float *obs, const
         set_error("des_nes_eval(FP32): hidden/state_dim %d needs %zu B shared memory (> 227 KB)", kmax, smem);
         return DES_ERR_UNSUPPORTED;
     }
-    if (solutions) {
-        DES_CUDA(cudaFuncSetAttribute(eval_ffma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        eval_ffma_kernel<true><<<(unsigned)n_local, kThreads, smem, st>>>(a);
-    } else {
-        DES_CUDA(cudaFuncSetAttribute(eval_ffma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        eval_ffma_kernel<false><<<(unsigned)n_local, kThreads, smem, st>>>(a);
-    }
-    DES_LAUNCH_CHECK("eval_ffma_kernel");
-    return DES_OK;
+    return launch_smem("eval_ffma_kernel", solutions ? eval_ffma_kernel<true> : eval_ffma_kernel<false>, (unsigned)n_local,
+                       kThreads, smem, st, a);
 }
 
 }  // namespace des

@@ -192,7 +192,7 @@ __device__ __forceinline__ void eval_tc_body(const TcArgs &a) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
     const Layout L = a.L;
-    const uint32_t gen = a.state ? (uint32_t)a.state->generation : a.gen;
+    const uint32_t gen = generation_word(a.state, a.gen);
     const int64_t first = blockIdx.x / CL, stride = gridDim.x / CL;
 
     // A CTA's half of a weight tile in a cluster: rows [32 rank, 32 rank + 32) of every 8 KB atom of a W2' chunk, rows
@@ -295,9 +295,8 @@ __device__ __forceinline__ void eval_tc_body(const TcArgs &a) {
         int i = 0;
         for (int64_t m = first; m < a.n_local; m += stride, ++i) {
             // the counter word of the noise and, mirrored, the sign of the pair member
-            const uint32_t member = kMirror ? (uint32_t)((a.member_offset + (uint64_t)m) >> 1)
-                                            : (uint32_t)(a.member_offset + (uint64_t)m);
-            const float sgn = kMirror && ((a.member_offset + (uint64_t)m) & 1u) ? -1.0f : 1.0f;
+            const uint32_t member = noise_word(a.member_offset + (uint64_t)m, kMirror);
+            const float sgn = member_sigma(a.member_offset + (uint64_t)m, kMirror, 1.0f);
             // ---- small fp32 arrays (whole, in every CTA) into buffer i & 1: b1 | b2 | W3[8][H] | b3[8]
             float *small = small_buf + (i & 1) * C::SMALL_FLOATS;
             if (i >= 2) mbar_wait(bar(C::BAR_SMALL_EMPTY + (i & 1)), ((i >> 1) - 1) & 1);
@@ -318,7 +317,7 @@ __device__ __forceinline__ void eval_tc_body(const TcArgs &a) {
                                          __ldg(reinterpret_cast<const float4 *>(a.theta + L.off_w3) + k), sgn);
             for (int k = L.A * H + ptid; k < H * kMaxA; k += kProdThreads) small[2 * H + k] = 0.f;   // unused action rows
             if (ptid < kMaxA)
-                small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, kMirror ? sgn * a.sigma : a.sigma, member, gen, a.key) : 0.f;
+                small[2 * H + kMaxA * H + ptid] = ptid < L.A ? perturbed1(a.theta, L.off_b3 + ptid, sgn * a.sigma, member, gen, a.key) : 0.f;
             // ---- W1' (this CTA's half of the rows in a cluster), once every consumer has run member i-1's layer 1
             DES_TRACE(TR_GEN);
             if (i >= 1) mbar_wait(bar(C::BAR_W1_EMPTY), (i - 1) & 1);
@@ -342,7 +341,7 @@ __device__ __forceinline__ void eval_tc_body(const TcArgs &a) {
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
                         const int k = c8 * 8 + e;
-                        w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, kMirror ? sgn * a.sigma : a.sigma, member, gen, a.key) : 0.f;
+                        w[e] = (k < L.d0) ? perturbed1(a.theta, L.off_w1 + n * L.d0 + k, sgn * a.sigma, member, gen, a.key) : 0.f;
                     }
                 }
                 uint4 hi, lo;
@@ -555,8 +554,8 @@ static int launch_tc(TcArgs &a, cudaStream_t st) {
     int dev = 0, sms = 132;
     DES_CUDA(cudaGetDevice(&dev));
     DES_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    DES_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     if (CL == 2) {
+        DES_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
         // each cluster accumulates its two halves into the output with atomicAdd: zero it first
         DES_CUDA(cudaMemsetAsync(a.fitness, 0, (size_t)a.n_local * sizeof(float), st));
         const int64_t clusters = a.n_local < sms / 2 ? a.n_local : sms / 2;
@@ -573,12 +572,11 @@ static int launch_tc(TcArgs &a, cudaStream_t st) {
         cfg.attrs = attr;
         cfg.numAttrs = 1;
         DES_CUDA(cudaLaunchKernelEx(&cfg, kernel, a));
-    } else {
-        const int64_t grid = a.n_local < sms ? a.n_local : sms;
-        kernel<<<(unsigned)grid, kTcThreads, C::SMEM, st>>>(a);
+        DES_LAUNCH_CHECK("eval_tc_kernel");
+        return DES_OK;
     }
-    DES_LAUNCH_CHECK("eval_tc_kernel");
-    return DES_OK;
+    const int64_t grid = a.n_local < sms ? a.n_local : sms;
+    return launch_smem("eval_tc_kernel", kernel, (unsigned)grid, kTcThreads, C::SMEM, st, a);
 }
 
 template <int H, bool X3, bool kMirror>

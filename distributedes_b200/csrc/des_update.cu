@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restr
                                                                    uint64_t member_offset) {
     const int64_t q = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
     if (q >= nq) return;
-    const uint32_t gen = state ? (uint32_t)state->generation : gen_arg;
+    const uint32_t gen = generation_word(state, gen_arg);
     const int64_t i0 = (int64_t)blockIdx.y * per_chunk;
     const int64_t i1 = min(n_local, i0 + per_chunk);
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -160,10 +160,8 @@ static int grad_partial(const char *who, float *partial_out_dev, const float *sh
                         void *workspace_dev, size_t workspace_bytes, bool mirrored, cudaStream_t st) {
     DES_REQUIRE(n_local >= 0 && P > 0, "%s: bad sizes n_local=%lld P=%lld", who, (long long)n_local, (long long)P);
     DES_REQUIRE(partial_out_dev, "%s: partial_out_dev is NULL", who);
-    DES_REQUIRE(member_offset >= 0 && member_offset + n_local <= (int64_t)1 << 32, "%s: member index must fit 32 bits", who);
-    DES_REQUIRE(!mirrored || (member_offset % 2 == 0 && n_local % 2 == 0),
-                "%s: a mirrored shard holds whole pairs: member_offset (%lld) and n_local (%lld) must be even", who,
-                (long long)member_offset, (long long)n_local);
+    DES_REQUIRE(member_range_ok(member_offset, n_local, 32), "%s: member index must fit 32 bits", who);
+    if (mirrored && !whole_pairs(member_offset, n_local)) return not_whole_pairs(who, "n_local", member_offset, n_local);
     if (n_local == 0) {
         DES_CUDA(cudaMemsetAsync(partial_out_dev, 0, (size_t)P * sizeof(float), st));
         return DES_OK;
