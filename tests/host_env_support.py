@@ -1,10 +1,8 @@
 """Test support for host-stepped environments (engine.HostEnvEngine, des_policy_act): a numpy stand-in for the
-policy step, a kernels module for the CPU gloo runs (tests/fake_kernels.py plus the host-step ops), a vectorised
-Pendulum-v0 implementing the batch protocol, and the oracle's episode loop."""
+policy step (cpu_ops.policy_act runs it), a vectorised Pendulum-v0 implementing the batch protocol, and the oracle's
+episode loop."""
 import numpy as np
-import torch
 
-from fake_kernels import *          # noqa: F401,F403  the NESEngine ops on CPU tensors
 from oracle import nes_oracle as orc
 from oracle import pendulum_oracle as po
 
@@ -62,50 +60,6 @@ def accumulate_stats(part, obs, alive):
                 part[i, :d0] += o
                 part[i, d0:2 * d0] += o * o
                 part[i, 2 * d0] += 1.0
-
-
-# ---- the host-step ops on CPU tensors (same names and arguments as distributedes_b200.ops) -------------------------------
-def nes_perturb(theta, n_members, sigma, seed, generation, member_offset=0, out=None):
-    P = theta.numel()
-    rows = orc.perturb(theta.numpy(), sigma, orc.noise(seed, generation, member_offset, n_members, P))
-    res = torch.from_numpy(np.asarray(rows, dtype=np.float32).reshape(n_members, P))
-    if out is None:
-        return res
-    out.copy_(res)
-    return out
-
-
-def policy_act(rows, obs, alive, *, state_dim, hidden, action_dim, repetitions, clip, action_noise_std=0.0, seed,
-               generation, member_offset=0, t, obs_stats=None, stat_part=None, out=None):
-    n, d0, A, reps = rows.shape[0], state_dim, action_dim, repetitions
-    o = obs.numpy().reshape(n, reps, d0)
-    al = alive.numpy().reshape(n, reps).astype(bool)
-    stats = None
-    if obs_stats is not None:
-        a = obs_stats.numpy()
-        stats = (a[:d0], a[d0:2 * d0], a[2 * d0])
-    if stat_part is not None:
-        part = stat_part.numpy().reshape(n, 2 * d0 + 1)
-        accumulate_stats(part, o, al)
-    act = policy_actions(rows.numpy(), o, al, d0, hidden, A, clip, stats, action_noise_std, seed, generation,
-                         member_offset, t)
-    res = torch.from_numpy(act.astype(np.float32).reshape(n, reps, A))
-    if out is None:
-        return res
-    out.copy_(res.reshape(out.shape))
-    return out
-
-
-def obs_parts_reduce(parts, state_dim, out=None):
-    p = parts.numpy().reshape(-1, 2 * state_dim + 1)
-    tot = np.zeros(2 * state_dim + 1)
-    for row in p:
-        tot += row
-    res = torch.from_numpy(tot)
-    if out is None:
-        return res
-    out.copy_(res)
-    return out
 
 
 # ---- environments ------------------------------------------------------------------------------------------------------

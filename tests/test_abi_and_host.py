@@ -7,6 +7,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from lib_fixture import lib  # noqa: F401
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(REPO, 'include', 'des_b200.h')
 
@@ -14,14 +16,6 @@ HEADER = os.path.join(REPO, 'include', 'des_b200.h')
 def header_symbols():
     txt = open(HEADER).read()
     return sorted(set(re.findall(r'DES_API\s+[\w\s\*]+?\b(des_\w+)\s*\(', txt)))
-
-
-@pytest.fixture(scope='module')
-def lib():
-    from distributedes_b200 import _lib, build
-    if not os.path.exists(_lib.LIB_PATH):
-        build.build_library()
-    return _lib.load()
 
 
 def test_header_declares_the_expected_surface():

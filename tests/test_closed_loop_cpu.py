@@ -2,16 +2,13 @@
 verbatim on its PendulumConfig (tests/golden/train_closed_pend.npz, oracle/make_golden.py::golden_train_closed), and
 the world_size-2 host logic of engine.RolloutEngine under gloo."""
 import os
-import sys
-import tempfile
 
 import numpy as np
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
+import cpu_ops
 from oracle import nes_oracle as orc
 from oracle import pendulum_oracle as po
+from ranks import spawn
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(REPO, 'tests', 'golden', 'train_closed_pend.npz')
@@ -57,33 +54,22 @@ def test_reset_states_are_in_range_and_distinct():
     assert not np.any(th == th2)
 
 
-def _worker(rank, world, port, N, gens, outdir):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    import fake_kernels
+def _worker(N, gens):
     from distributedes_b200.engine import RolloutEngine
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        theta0 = orc.synthetic_theta(3, 32, 1)
-        eng = RolloutEngine(hidden=32, pop_size=N, theta0=theta0, sigma=0.1, learning_rate=0.1, repetitions=2, horizon=20,
-                            seed=13, device='cpu', kernels=fake_kernels)
-        tests = []
-        for _ in range(gens):
-            tests.append(eng.test_returns())
-            eng.generation()
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), theta=eng.theta.numpy(), stats=eng.obs_stats.numpy(),
-                 fit=eng.fitness_all.numpy(), tests=np.stack(tests))
-    finally:
-        dist.destroy_process_group()
+    theta0 = orc.synthetic_theta(3, 32, 1)
+    eng = RolloutEngine(hidden=32, pop_size=N, theta0=theta0, sigma=0.1, learning_rate=0.1, repetitions=2, horizon=20,
+                        seed=13, device='cpu', kernels=cpu_ops)
+    tests = []
+    for _ in range(gens):
+        tests.append(eng.test_returns())
+        eng.generation()
+    return dict(theta=eng.theta.numpy(), stats=eng.obs_stats.numpy(), fit=eng.fitness_all.numpy(), tests=np.stack(tests))
 
 
 def test_rollout_engine_sharded_equals_single_process():
     """Ragged 2-rank split: fitness all-gather, fp64 observation-total all-reduce, identical update on both ranks."""
     N, world, gens = 7, 2, 2
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_worker, args=(world, 29671, N, gens, outdir), nprocs=world, join=True)
-        res = [np.load(os.path.join(outdir, 'rank%d.npz' % r)) for r in range(world)]
+    res = spawn(world, _worker, N, gens)
     for k in ('theta', 'stats', 'fit', 'tests'):
         assert np.array_equal(res[0][k], res[1][k]), k
     recs = list(oracle_chain(orc.synthetic_theta(3, 32, 1), 32, N, 2, 13, 0.1, 0.1, 0.005, gens, horizon=20))
@@ -93,36 +79,25 @@ def test_rollout_engine_sharded_equals_single_process():
     assert np.max(np.abs(res[0]['theta'] - recs[-1]['theta'])) <= 2e-6
 
 
-def _train_worker(rank, world, port, outdir):
+def _train_worker():
     """natural_es.train() — the reference-facing loop — on two ranks under gloo, closed loop, oracle-backed kernels."""
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    import fake_kernels
     from distributedes_b200 import natural_es
     from distributedes_b200.config import ClosedLoopPendulumConfig
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        g = np.load(GOLD)
-        cfg = ClosedLoopPendulumConfig(hidden_size=int(g['H']))
-        cfg.initial_weight = g['theta0'].copy()
-        cfg.pop_size, cfg.sigma, cfg.learning_rate, cfg.seed = int(g['N']), float(g['sigma']), float(g['lr']), int(g['seed'])
-        cfg.max_steps = (int(g['gens']) + 1) * cfg.pop_size * cfg.repetitions * 200 - 1
-        eng = natural_es.build_engine(cfg, device='cpu', kernels=fake_kernels)
-        rewards, steps, stamps = natural_es.train(cfg, engine=eng)
-        np.savez(os.path.join(outdir, 'train%d.npz' % rank), rewards=np.asarray(rewards), steps=np.asarray(steps),
-                 theta=eng.theta.numpy(), n_stamps=len(stamps))
-    finally:
-        dist.destroy_process_group()
+    g = np.load(GOLD)
+    cfg = ClosedLoopPendulumConfig(hidden_size=int(g['H']))
+    cfg.initial_weight = g['theta0'].copy()
+    cfg.pop_size, cfg.sigma, cfg.learning_rate, cfg.seed = int(g['N']), float(g['sigma']), float(g['lr']), int(g['seed'])
+    cfg.max_steps = (int(g['gens']) + 1) * cfg.pop_size * cfg.repetitions * 200 - 1
+    eng = natural_es.build_engine(cfg, device='cpu', kernels=cpu_ops)
+    rewards, steps, stamps = natural_es.train(cfg, engine=eng)
+    return dict(rewards=np.asarray(rewards), steps=np.asarray(steps), theta=eng.theta.numpy(), n_stamps=len(stamps))
 
 
 def test_train_surface_on_two_ranks_reproduces_the_reference_golden():
     """BASELINE configs[0] through natural_es.train(ClosedLoopPendulumConfig) on 2 ranks (8 members each): the returned
     [rewards, steps, timestamps] triple and the final parameters equal the reference's verbatim run."""
     g = np.load(GOLD)
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_train_worker, args=(2, 29683, outdir), nprocs=2, join=True)
-        r = [np.load(os.path.join(outdir, 'train%d.npz' % k)) for k in range(2)]
+    r = spawn(2, _train_worker)
     for k in ('rewards', 'steps', 'theta'):
         assert np.array_equal(r[0][k], r[1][k]), k
     assert list(r[0]['steps']) == list(g['train_steps']) and int(r[0]['n_stamps']) == len(g['train_steps'])

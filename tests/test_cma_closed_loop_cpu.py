@@ -2,19 +2,17 @@
 PendulumConfig(hidden_size=16) (tests/golden/train_cma_closed_pend.npz, oracle/make_golden_cma.py), the
 sharded host logic of cma_es.train under gloo, and the C ABI's argument checks for des_rollout_eval_solutions."""
 import os
-import sys
-import tempfile
-import types
 
 import numpy as np
 import pytest
-import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
+import cpu_ops
+from lib_fixture import lib  # noqa: F401
 from oracle import cma_oracle as cma
 from oracle import nes_oracle as orc
 from oracle import pendulum_oracle as po
+from ranks import spawn
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(REPO, 'tests', 'golden', 'train_cma_closed_pend.npz')
@@ -77,73 +75,37 @@ def test_oracle_chain_matches_verbatim_reference_cma_train():
         assert np.max(np.abs(r['ps'] - g['ps'][k])) <= 1e-6 * np.max(np.abs(g['ps'][k]))
 
 
-def _closed_loop_kernels():
-    """tests/fake_kernels plus the explicit-row rollout (oracle-backed), as a module the host code can take as `kernels`."""
-    import fake_kernels
-    kn = types.ModuleType('fake_closed_loop_cma_kernels')
-    kn.__dict__.update({k: v for k, v in fake_kernels.__dict__.items() if not k.startswith('__')})
-
-    def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions=10, clip, action_noise_std=0.0,
-                               seed, generation=0, member_offset=0, obs_stats=None, totals_out=None, workspace=None,
-                               out=None, episodes_out=None):
-        stats = None
-        if obs_stats is not None:
-            a = obs_stats.numpy()
-            stats = (a[:3], a[3:6], a[6])
-        n = solutions.shape[0]
-        ret, osum, osq, cnt = po.rollouts(solutions.numpy(), hidden, seed, generation,
-                                          np.arange(member_offset, member_offset + n), repetitions, stats, horizon, clip,
-                                          action_noise_std)
-        out.copy_(torch.from_numpy(ret.mean(1).astype(np.float32)))
-        if totals_out is not None:
-            totals_out.copy_(torch.from_numpy(np.concatenate([osum, osq, [cnt]])))
-        return out
-
-    kn.rollout_eval_solutions = rollout_eval_solutions
-    return kn
-
-
-def _train_worker(rank, world, port, outdir):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
+def _train_worker():
     from distributedes_b200 import cma_es
     from distributedes_b200.config import ClosedLoopPendulumConfig
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        g = np.load(GOLD)
-        cfg = ClosedLoopPendulumConfig(16)
-        cfg.initial_weight = g['theta0'].copy()
-        cfg.pop_size, cfg.sigma, cfg.seed = int(g['lam']), float(g['sigma']), int(g['seed'])
-        cfg.max_steps = (int(g['gens']) + 1) * cfg.pop_size * cfg.repetitions * 200 - 1
-        kn = _closed_loop_kernels()
-        worker = cma_es.Worker(rank, None, None, None, None, cfg, device='cpu', kernels=kn)
-        es = cma_es.CMAEvolutionStrategy(cfg.initial_weight, cfg.sigma, cfg.pop_size, seed=cfg.seed, device='cpu',
-                                         kernels=kn)
-        told = []
-        real_tell = es.tell
+    g = np.load(GOLD)
+    cfg = ClosedLoopPendulumConfig(16)
+    cfg.initial_weight = g['theta0'].copy()
+    cfg.pop_size, cfg.sigma, cfg.seed = int(g['lam']), float(g['sigma']), int(g['seed'])
+    cfg.max_steps = (int(g['gens']) + 1) * cfg.pop_size * cfg.repetitions * 200 - 1
+    worker = cma_es.Worker(dist.get_rank(), None, None, None, None, cfg, device='cpu', kernels=cpu_ops)
+    es = cma_es.CMAEvolutionStrategy(cfg.initial_weight, cfg.sigma, cfg.pop_size, seed=cfg.seed, device='cpu',
+                                     kernels=cpu_ops)
+    told = []
+    real_tell = es.tell
 
-        def spy_tell(solutions, cost):
-            told.append(np.asarray(cost, dtype=np.float64).copy())
-            return real_tell(solutions, cost)
-        es.tell = spy_tell
-        rewards, steps, stamps = cma_es.train(cfg, worker=worker, es=es)
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), rewards=np.asarray(rewards), steps=np.asarray(steps),
-                 n_stamps=len(stamps), m=es.m.numpy(), C=es.C.numpy(), sigma=es.sigma, pc=es.pc.numpy(),
-                 stats=worker.obs_stats.numpy(), shaped=np.stack(told), n_local=es.n_local)
-    finally:
-        dist.destroy_process_group()
+    def spy_tell(solutions, cost):
+        told.append(np.asarray(cost, dtype=np.float64).copy())
+        return real_tell(solutions, cost)
+    es.tell = spy_tell
+    rewards, steps, stamps = cma_es.train(cfg, worker=worker, es=es)
+    return dict(rewards=np.asarray(rewards), steps=np.asarray(steps), n_stamps=len(stamps), m=es.m.numpy(),
+                C=es.C.numpy(), sigma=es.sigma, pc=es.pc.numpy(), stats=worker.obs_stats.numpy(), shaped=np.stack(told),
+                n_local=es.n_local)
 
 
-@pytest.mark.parametrize('world,port', [(2, 29713), (3, 29727)])
-def test_cma_train_closed_loop_sharded_packed_reproduces_the_reference_golden(world, port):
+@pytest.mark.parametrize('world', [2, 3])
+def test_cma_train_closed_loop_sharded_packed_reproduces_the_reference_golden(world):
     """cma_es.train(ClosedLoopPendulumConfig(16)) on gloo ranks (8 + 8 members, and the ragged 6 + 5 + 5): every rank returns
     the same triple and holds the same strategy state, equal to the reference's verbatim run.  tell() all-reduces the
     rank-mu partials in the packed form sharded GPU runs use."""
     g = np.load(GOLD)
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_train_worker, args=(world, port, outdir), nprocs=world, join=True)
-        r = [np.load(os.path.join(outdir, 'rank%d.npz' % k)) for k in range(world)]
+    r = spawn(world, _train_worker)
     assert sum(int(x['n_local']) for x in r) == int(g['lam'])
     for x in r[1:]:
         for k in ('rewards', 'steps', 'm', 'C', 'sigma', 'pc', 'stats', 'shaped'):
@@ -172,14 +134,6 @@ def test_hidden_16_is_accepted_on_the_closed_loop_path():
     assert ClosedLoopPendulumConfig().hidden_size == 64
     with pytest.raises(ValueError, match='hidden_size'):
         ClosedLoopPendulumConfig(48)
-
-
-@pytest.fixture(scope='module')
-def lib():
-    from distributedes_b200 import _lib, build
-    if not os.path.exists(_lib.LIB_PATH):
-        build.build_library()
-    return _lib.load()
 
 
 def test_rollout_eval_solutions_validates_before_cuda(lib):

@@ -1,48 +1,34 @@
 """world_size=2 on CPU with gloo: cma_es.CMAEvolutionStrategy sharded over the ranks (members split, z regenerated per
 shard, all-reduce of the packed rank-mu partials — the sharded path the GPUs run — and of sum_i w_i y_i) must reproduce the single-process fp64 restatement
 (oracle/cma_oracle.CMAState) given the same counter noise."""
-import os
-import sys
-import tempfile
-
 import numpy as np
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cpu_ops
+from ranks import spawn
+
 N, LAM, GENS, SEED = 12, 9, 3, 4          # ragged: 5 + 4 members
 
 
-def _worker(rank, world, port, outdir):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    import fake_kernels
+def _worker():
     from distributedes_b200.cma_es import CMAEvolutionStrategy
     from oracle import cma_oracle as cma
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        m0 = np.random.RandomState(0).randn(N)
-        es = CMAEvolutionStrategy(m0, 1.0, LAM, seed=SEED, device='cpu', kernels=fake_kernels)
-        Xs = []
-        for _ in range(GENS):
-            X = es.ask()
-            Xs.append(X.numpy().copy())
-            cost = es.gather_cost(torch.from_numpy(cma.sphere(X.numpy()).astype(np.float32)))
-            es.tell(X, cost)
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), m=es.m.numpy(), C=es.C.numpy(), sigma=es.sigma,
-                 offset=es.offset, n_local=es.n_local, pc=es.pc.numpy(), X=np.stack(Xs))
-    finally:
-        dist.destroy_process_group()
+    m0 = np.random.RandomState(0).randn(N)
+    es = CMAEvolutionStrategy(m0, 1.0, LAM, seed=SEED, device='cpu', kernels=cpu_ops)
+    Xs = []
+    for _ in range(GENS):
+        X = es.ask()
+        Xs.append(X.numpy().copy())
+        cost = es.gather_cost(torch.from_numpy(cma.sphere(X.numpy()).astype(np.float32)))
+        es.tell(X, cost)
+    return dict(m=es.m.numpy(), C=es.C.numpy(), sigma=es.sigma, offset=es.offset, n_local=es.n_local, pc=es.pc.numpy(),
+                X=np.stack(Xs))
 
 
 def test_sharded_cma_with_packed_partials_equals_single_process_restatement():
     from oracle import cma_oracle as cma
     from oracle import nes_oracle as orc
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_worker, args=(2, 29691, outdir), nprocs=2, join=True)
-        r = [np.load(os.path.join(outdir, 'rank%d.npz' % k)) for k in range(2)]
+    r = spawn(2, _worker)
     assert int(r[0]['offset']) == 0 and int(r[0]['n_local']) + int(r[1]['n_local']) == LAM
     for k in ('m', 'C', 'sigma', 'pc'):                       # identical update on every rank, no broadcast
         assert np.array_equal(r[0][k], r[1][k]), k

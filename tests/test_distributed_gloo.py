@@ -1,61 +1,40 @@
 """world_size=2 on CPU with gloo: the sharded generation (engine.NESEngine host logic) must produce exactly the
 single-process result: members split across ranks (even and ragged), fitness gathered by the zero-padded
 all-reduce, partial sums all-reduced, identical update on every rank."""
-import os
-import sys
-
 import numpy as np
 import pytest
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cpu_ops
+from ranks import spawn
 
 
-def _worker(rank, world, port, N, gens, outdir, normalize=False):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    import fake_kernels
+def _worker(N, gens, normalize=False):
     from distributedes_b200.engine import NESEngine
     from oracle import nes_oracle as orc
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        d0, H, A, T = 3, 8, 1, 6
-        obs, target = orc.synthetic_tape(T, d0, A)
-        theta0 = orc.synthetic_theta(d0, H, A)
-        eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=theta0, obs=obs, target=target,
-                        sigma=0.1, learning_rate=0.1, clip=2.0, seed=11, device='cpu', kernels=fake_kernels,
-                        normalize_obs=normalize)
-        fits = []
-        for _ in range(gens):
-            eng.generation()
-            fits.append(eng.fitness_all.numpy().copy())
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), offset=eng.offset, n_local=eng.n_local,
-                 theta=eng.theta.numpy(), fits=np.stack(fits))
-    finally:
-        dist.destroy_process_group()
+    d0, H, A, T = 3, 8, 1, 6
+    obs, target = orc.synthetic_tape(T, d0, A)
+    theta0 = orc.synthetic_theta(d0, H, A)
+    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=theta0, obs=obs, target=target,
+                    sigma=0.1, learning_rate=0.1, clip=2.0, seed=11, device='cpu', kernels=cpu_ops,
+                    normalize_obs=normalize)
+    fits = []
+    for _ in range(gens):
+        eng.generation()
+        fits.append(eng.fitness_all.numpy().copy())
+    return dict(offset=eng.offset, n_local=eng.n_local, theta=eng.theta.numpy(), fits=np.stack(fits))
 
 
 @pytest.mark.parametrize('N,world', [(10, 2), (11, 2), (3, 2)])
 def test_sharded_generation_equals_single_process(N, world):
     from oracle import nes_oracle as orc
-    import tempfile
-    port = 29600 + N
     gens = 2
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_worker, args=(world, port, N, gens, outdir), nprocs=world, join=True)
-        results = []
-        for r in range(world):
-            z = np.load(os.path.join(outdir, 'rank%d.npz' % r))
-            results.append((r, int(z['offset']), int(z['n_local']), z['theta'], z['fits']))
+    res = spawn(world, _worker, N, gens)
     # shards tile the population
-    assert results[0][1] == 0 and sum(r[2] for r in results) == N
+    assert res[0]['offset'] == 0 and sum(r['n_local'] for r in res) == N
     # every rank ends with bit-identical parameters (no broadcast needed)
-    for r in results[1:]:
-        assert np.array_equal(r[3], results[0][3])
-        assert np.array_equal(r[4], results[0][4])
+    for r in res[1:]:
+        assert np.array_equal(r['theta'], res[0]['theta'])
+        assert np.array_equal(r['fits'], res[0]['fits'])
     # and they equal the single-process oracle chain
     d0, H, A, T = 3, 8, 1, 6
     obs, target = orc.synthetic_tape(T, d0, A)
@@ -64,21 +43,17 @@ def test_sharded_generation_equals_single_process(N, world):
     for gen in range(gens):
         out = orc.nes_generation(theta, opt, obs, target, sigma=0.1, clip=2.0, seed=11, gen=gen, N=N, d0=d0, H=H, A=A,
                                  weight_decay=0.005, learning_rate=0.1)
-        assert np.allclose(results[0][4][gen], out['fitness'], rtol=1e-6)
+        assert np.allclose(res[0]['fits'][gen], out['fitness'], rtol=1e-6)
         theta = out['theta']
-    assert np.max(np.abs(results[0][3] - theta)) <= 2e-6
+    assert np.max(np.abs(res[0]['theta'] - theta)) <= 2e-6
 
 
 def test_sharded_generation_with_observation_normaliser():
     """normalize_obs=True under gloo: every rank merges identical online statistics (no collective), so the two ranks
     stay bit-identical and equal the single-process chain with the oracle's ObsStats."""
-    import tempfile
     from oracle import nes_oracle as orc
     N, world, gens = 9, 2, 3
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_worker, args=(world, 29650, N, gens, outdir, True), nprocs=world, join=True)
-        res = [np.load(os.path.join(outdir, 'rank%d.npz' % r)) for r in range(world)]
-        thetas = [r['theta'] for r in res]
+    thetas = [r['theta'] for r in spawn(world, _worker, N, gens, True)]
     assert np.array_equal(thetas[0], thetas[1])
     d0, H, A, T = 3, 8, 1, 6
     obs, target = orc.synthetic_tape(T, d0, A)

@@ -3,9 +3,10 @@ pairs of a mirrored shard, NULL pointers and policy widths.  Every input here is
 library answers it on any machine.  Each case pins the status code and the exact message; where several checks fail
 at once the pin also fixes which one is reported."""
 import ctypes as C
-import os
 
 import pytest
+
+from lib_fixture import lib  # noqa: F401
 
 D = C.c_void_p(256)          # never dereferenced: every case returns before any CUDA work
 NULL = None
@@ -151,14 +152,6 @@ PINS = {
     ('des_policy_act', 'null_count'): (-1, 'des_policy_act: NULL alive mask'),
     ('des_policy_act', 'bad_width'): (-1, 'des_policy_act: hidden must be 16, 32, 64, 96 or 128 (got 48)'),
 }
-
-
-@pytest.fixture(scope='module')
-def lib():
-    from distributedes_b200 import _lib, build
-    if not os.path.exists(_lib.LIB_PATH):
-        build.build_library()
-    return _lib.load()
 
 
 @pytest.mark.parametrize('entry,case', sorted(PINS))

@@ -1,66 +1,22 @@
 """The host logic around the kernels, pinned without a GPU: which device ops every NES and CMA-ES mode launches per
 generation, in which order and with which arguments, and which collectives it issues on tensors of which size — one
-process and each rank of a 2-rank gloo run.  The kernels are the oracle-backed CPU stand-ins (tests/fake_kernels.py,
-host_env_support.py, mirrored_support.py) behind a recording proxy.  Also: CMA-ES on a host-stepped environment
-sharded over 2 and 3 gloo ranks against the single-process run."""
+process and each rank of a 2-rank gloo run.  The kernels are the oracle-backed CPU stand-ins (cpu_ops.py) behind a
+recording proxy.  Also: CMA-ES on a host-stepped environment sharded over 2 and 3 gloo ranks against the
+single-process run."""
 import hashlib
 import inspect
-import os
-import sys
-import tempfile
 import types
 
 import numpy as np
 import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, 'tests'))
-
-from oracle import nes_oracle as orc      # noqa: E402
-from oracle import pendulum_oracle as po  # noqa: E402
-from oracle import synth_walk as sw       # noqa: E402
-
-
-def _stand_ins():
-    """One module with every CPU stand-in: the NES ops, the host-step ops, the mirrored twins, and the two
-    explicit-row evaluations CMA-ES needs (des_pop_eval on the tape, des_rollout_eval_solutions on the device)."""
-    import host_env_support
-    import mirrored_support
-    kn = types.ModuleType('fake_fitness_kernels')
-    for mod in (host_env_support, mirrored_support):
-        kn.__dict__.update({k: v for k, v in mod.__dict__.items() if not k.startswith('__')})
-
-    def pop_eval(solutions, obs, target, *, hidden, clip, out=None):
-        T, d0 = obs.shape
-        A = target.shape[1]
-        f = [orc.tape_fitness(orc.forward(s, obs.numpy(), d0, hidden, A), target.numpy(), clip) for s in solutions.numpy()]
-        res = torch.tensor(f, dtype=torch.float32)
-        if out is None:
-            return res
-        out.copy_(res)
-        return out
-
-    def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions=10, clip, action_noise_std=0.0,
-                               seed, generation=0, member_offset=0, obs_stats=None, totals_out=None, workspace=None,
-                               out=None, episodes_out=None):
-        stats = None
-        if obs_stats is not None:
-            a = obs_stats.numpy()
-            stats = (a[:3], a[3:6], a[6])
-        n = solutions.shape[0]
-        ret, osum, osq, cnt = po.rollouts(solutions.numpy(), hidden, seed, generation,
-                                          np.arange(member_offset, member_offset + n), repetitions, stats, horizon, clip,
-                                          action_noise_std)
-        out.copy_(torch.from_numpy(ret.mean(1).astype(np.float32)))
-        if totals_out is not None:
-            totals_out.copy_(torch.from_numpy(np.concatenate([osum, osq, [cnt]])))
-        return out
-
-    kn.pop_eval, kn.rollout_eval_solutions = pop_eval, rollout_eval_solutions
-    return kn
+import cpu_ops
+import host_env_support as hs
+from oracle import nes_oracle as orc
+from oracle import synth_walk as sw
+from ranks import spawn
 
 
 def _canon(v):
@@ -104,7 +60,7 @@ class record:
 
     def __init__(self):
         self.log = []
-        self.kernels = Recorder(_stand_ins(), self.log)
+        self.kernels = Recorder(cpu_ops, self.log)
 
     def __enter__(self):
         self.saved = {n: getattr(dist, n) for n in self.COLLECTIVES}
@@ -135,18 +91,16 @@ class record:
 
 
 # ---- the modes ---------------------------------------------------------------------------------------------------------
-class Cfg:
+class Cfg(types.SimpleNamespace):
     """The attributes natural_es.train / cma_es.train read."""
 
     def __init__(self, **kw):
-        self.__dict__.update(dict(state_dim=3, pop_size=6, repetitions=1, test_repetitions=2, max_steps=0,
-                                  max_generations=1, seed=7))
-        self.__dict__.update(kw)
+        super().__init__(**{**dict(state_dim=3, pop_size=6, repetitions=1, test_repetitions=2, max_steps=0,
+                                   max_generations=1, seed=7), **kw})
 
 
 def _nes(mode, kernels):
     from distributedes_b200.engine import HostEnvEngine, NESEngine, RolloutEngine
-    import host_env_support as hs
     mirrored = mode.endswith('mirrored')
     common = dict(pop_size=6, sigma=0.1, learning_rate=0.1, seed=7, device='cpu', kernels=kernels, mirrored=mirrored)
     if mode.startswith('tape'):
@@ -174,7 +128,6 @@ class PendulumProbe:
 def _cma_config(mode, seed=7):
     from distributedes_b200.config import ClosedLoopPendulumConfig, HostEnvConfig, SynthTapeConfig
     from distributedes_b200.envs import GymEnvBatch
-    import host_env_support as hs
     if mode == 'tape':
         cfg = SynthTapeConfig(hidden_size=8, state_dim=3, action_dim=2, tape_len=5)
         cfg.test_repetitions = 2
@@ -230,24 +183,6 @@ def _traces():
 
 NES_MODES = ('tape', 'tape_mirrored', 'tape_norm', 'device', 'device_mirrored', 'host', 'host_mirrored')
 CMA_MODES = ('tape', 'device', 'host')
-
-
-def _gloo(rank, world, port, outdir, fn):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        np.save(os.path.join(outdir, 'rank%d.npy' % rank), np.asarray([fn()], dtype=object), allow_pickle=True)
-    finally:
-        dist.destroy_process_group()
-
-
-def _spawn(world, port, fn):
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_gloo, args=(world, port, outdir, fn), nprocs=world, join=True)
-        return [np.load(os.path.join(outdir, 'rank%d.npy' % r), allow_pickle=True)[0] for r in range(world)]
-
 
 
 # per mode, recorded from the host layer as it was before the fitness sources (fitness.py) took over the evaluation:
@@ -376,7 +311,7 @@ def test_every_mode_issues_the_pinned_ops_and_collectives_in_one_process():
 
 
 def test_every_mode_issues_the_pinned_ops_and_collectives_on_each_of_two_gloo_ranks():
-    r = _spawn(2, 29853, _traces)
+    r = spawn(2, _traces)
     for key, (_, r0, r1) in EXPECTED.items():
         assert (r[0][key], r[1][key]) == (r0, r1), key
 
@@ -384,16 +319,16 @@ def test_every_mode_issues_the_pinned_ops_and_collectives_on_each_of_two_gloo_ra
 def _walk_cma():
     cfg = _cma_config('walk', seed=5)
     cfg.pop_size, cfg.max_generations = 5, 3
-    return _run_cma('walk', cfg=cfg, kernels=_stand_ins())
+    return _run_cma('walk', cfg=cfg, kernels=cpu_ops)
 
 
-@pytest.mark.parametrize('world,port', [(2, 29855), (3, 29857)])
-def test_host_stepped_cma_sharded_over_gloo_ranks_equals_the_single_process_run(world, port):
+@pytest.mark.parametrize('world', [2, 3])
+def test_host_stepped_cma_sharded_over_gloo_ranks_equals_the_single_process_run(world):
     """cma_es.train on SynthWalk (episodes of 40-160 steps) with ragged shards (3 + 2, 2 + 2 + 1): each rank steps its
     own solutions' environments; the costs, the step counts summed over ranks, the observation totals and the test
     episodes of the best solution give the single-process run's results."""
     one = _walk_cma()
-    res = _spawn(world, port, _walk_cma)
+    res = spawn(world, _walk_cma)
     for r in res[1:]:
         for k in one:
             assert np.array_equal(r[k], res[0][k]), k

@@ -3,20 +3,19 @@ on SynthWalk-v0 (tests/golden/train_host_walk.npz, oracle/make_golden_host.py), 
 envs.GymEnvBatch, des_policy_act's argument checks, GymConfig without gym, and engine.HostEnvEngine on two gloo ranks."""
 import os
 import sys
-import tempfile
 
 import numpy as np
 import pytest
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
+import cpu_ops
+import host_env_support as hs
+from lib_fixture import lib  # noqa: F401
+from oracle import nes_oracle as orc
 from oracle import synth_walk as sw
+from ranks import spawn
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(REPO, 'tests', 'golden', 'train_host_walk.npz')
-sys.path.insert(0, os.path.join(REPO, 'tests'))
-import host_env_support as hs          # noqa: E402
 
 
 def walk_batch(seed):
@@ -123,14 +122,6 @@ def test_episode_seed_is_a_pure_function_of_the_key():
     assert list(episode_seed(11, k[:, 0], k[:, 1], k[:, 2])) == seeds
 
 
-@pytest.fixture(scope='module')
-def lib():
-    from distributedes_b200 import _lib, build
-    if not os.path.exists(_lib.LIB_PATH):
-        build.build_library()
-    return _lib.load()
-
-
 @pytest.mark.parametrize('d0,H,A,reps,alive,P,match', [
     (24, 48, 4, 10, True, None, 'hidden must be 16, 32, 64, 96 or 128'),
     (33, 64, 4, 10, True, None, 'state_dim must be in'),
@@ -172,11 +163,13 @@ def test_host_env_config_probes_the_environment():
 def _engine(N, seed, device='cpu'):
     from distributedes_b200.engine import HostEnvEngine
     return HostEnvEngine(env_fn=sw.SynthWalkEnv, batch_env_fn=walk_batch(seed), hidden=16, pop_size=N,
-                         theta0=np.asarray(hs.orc.synthetic_theta(24, 16, 4), dtype=np.float32), sigma=0.1,
-                         learning_rate=0.1, repetitions=3, test_repetitions=2, seed=seed, device=device, kernels=hs)
+                         theta0=np.asarray(orc.synthetic_theta(24, 16, 4), dtype=np.float32), sigma=0.1,
+                         learning_rate=0.1, repetitions=3, test_repetitions=2, seed=seed, device=device,
+                         kernels=cpu_ops)
 
 
-def _run(eng, gens):
+def _run(N, gens):
+    eng = _engine(N, 5)
     out = dict(fit=[], steps=[], stats=[], tests=[])
     for _ in range(gens):
         out['tests'].append(eng.test_returns())
@@ -188,27 +181,13 @@ def _run(eng, gens):
     return {k: np.asarray(v) for k, v in out.items()}
 
 
-def _gloo_worker(rank, world, port, N, gens, outdir):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        res = _run(_engine(N, 5), gens)
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), **res)
-    finally:
-        dist.destroy_process_group()
-
-
 def test_host_env_engine_on_two_ranks_equals_the_single_process_run():
     """Ragged 2-rank split: each rank steps only its own members' environments; the fitness all-gather, the fp64
     observation totals and the step count summed over ranks give the single-process run's fitness, steps, statistics
     and parameters."""
     N, gens = 5, 2
-    one = _run(_engine(N, 5), gens)
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_gloo_worker, args=(2, 29707, N, gens, outdir), nprocs=2, join=True)
-        res = [np.load(os.path.join(outdir, 'rank%d.npz' % r)) for r in range(2)]
+    one = _run(N, gens)
+    res = spawn(2, _run, N, gens)
     for k in ('fit', 'steps', 'stats', 'tests', 'theta'):
         assert np.array_equal(res[0][k], res[1][k]), k
     for k in ('fit', 'steps', 'stats', 'tests'):

@@ -4,22 +4,17 @@ pair-form gradient, the evenness rules of the engines and the C entry points, ch
 under gloo with 2 and 3 ranks against the single-process chain."""
 import ctypes as C
 import os
-import sys
-import tempfile
 
 import numpy as np
 import pytest
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
+import cpu_ops
+import mirrored_support as ms
+from lib_fixture import lib  # noqa: F401
 from oracle import mirrored_oracle as mo
 from oracle import nes_oracle as orc
 from oracle import pendulum_oracle as po
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, 'tests'))
-import mirrored_support as ms      # noqa: E402
+from ranks import spawn
 
 
 def test_noise_mirrored_rows_are_signed_plain_rows():
@@ -78,7 +73,7 @@ def _tape_engine(N, mirrored=True, **kw):
     d0, H, A, T = 3, 8, 1, 6
     obs, target = orc.synthetic_tape(T, d0, A)
     return NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
-                     target=target, sigma=0.1, learning_rate=0.1, clip=2.0, seed=11, device='cpu', kernels=ms,
+                     target=target, sigma=0.1, learning_rate=0.1, clip=2.0, seed=11, device='cpu', kernels=cpu_ops,
                      mirrored=mirrored, **kw)
 
 
@@ -88,7 +83,7 @@ def test_odd_population_is_rejected():
     from distributedes_b200.engine import RolloutEngine
     with pytest.raises(ValueError, match='even pop_size'):
         RolloutEngine(hidden=16, pop_size=9, theta0=orc.synthetic_theta(3, 16, 1), sigma=0.1, learning_rate=0.1,
-                      device='cpu', kernels=ms, mirrored=True)
+                      device='cpu', kernels=cpu_ops, mirrored=True)
     e = _tape_engine(8)
     assert (e.offset, e.n_local, e.mirrored) == (0, 8, True)
 
@@ -96,14 +91,6 @@ def test_odd_population_is_rejected():
 def test_config_defaults_to_plain_sampling():
     from distributedes_b200.config import ClosedLoopPendulumConfig, SynthTapeConfig
     assert SynthTapeConfig().mirrored is False and ClosedLoopPendulumConfig(16).mirrored is False
-
-
-@pytest.fixture(scope='module')
-def lib():
-    from distributedes_b200 import _lib, build
-    if not os.path.exists(_lib.LIB_PATH):
-        build.build_library()
-    return _lib.load()
 
 
 def test_mirrored_entry_points_reject_odd_shards_before_any_cuda_work(lib):
@@ -155,30 +142,20 @@ def test_checkpoint_records_the_sampling_mode(tmp_path):
         natural_es.load_checkpoint(mirrored, path)
 
 
-def _worker(rank, world, port, N, gens, outdir):
-    sys.path.insert(0, REPO)
-    sys.path.insert(0, os.path.join(REPO, 'tests'))
-    torch.set_num_threads(1)
-    dist.init_process_group('gloo', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        eng = _tape_engine(N)
-        fits = []
-        for _ in range(gens):
-            eng.generation()
-            fits.append(eng.fitness_all.numpy().copy())
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), offset=eng.offset, n_local=eng.n_local, theta=eng.theta.numpy(),
-                 fits=np.stack(fits))
-    finally:
-        dist.destroy_process_group()
+def _worker(N, gens):
+    eng = _tape_engine(N)
+    fits = []
+    for _ in range(gens):
+        eng.generation()
+        fits.append(eng.fitness_all.numpy().copy())
+    return dict(offset=eng.offset, n_local=eng.n_local, theta=eng.theta.numpy(), fits=np.stack(fits))
 
 
-@pytest.mark.parametrize('N,world,port', [(22, 2, 29811), (22, 3, 29812), (8, 3, 29813)])
-def test_sharded_mirrored_generation_equals_single_process(N, world, port):
+@pytest.mark.parametrize('N,world', [(22, 2), (22, 3), (8, 3)])
+def test_sharded_mirrored_generation_equals_single_process(N, world):
     """Shards are whole pairs (shard_bounds over N/2 pairs, scaled by 2), also when the pairs do not split evenly."""
     gens = 2
-    with tempfile.TemporaryDirectory() as outdir:
-        mp.spawn(_worker, args=(world, port, N, gens, outdir), nprocs=world, join=True)
-        res = [np.load(os.path.join(outdir, 'rank%d.npz' % r)) for r in range(world)]
+    res = spawn(world, _worker, N, gens)
     offs = [(int(r['offset']), int(r['n_local'])) for r in res]
     assert all(o % 2 == 0 and n % 2 == 0 for o, n in offs) and sum(n for _, n in offs) == N
     assert all(offs[k][0] + offs[k][1] == offs[k + 1][0] for k in range(world - 1))
