@@ -1,6 +1,6 @@
 """Minimal stand-in for the third-party ``cma`` package (pycma) so the reference's cma_es.py imports and runs verbatim
-in this container, where pycma is not installed.  TEST INFRASTRUCTURE ONLY: oracle/make_golden_cma.py puts this directory on
-sys.path; the product package never imports it.
+where pycma is not installed.  TEST INFRASTRUCTURE ONLY: oracle/make_golden.py puts this directory on sys.path; the
+product package never imports it.
 
 Only what cma_es.py:43-49, :62 and :90 touch exists: ``CMAOptions`` (a dict; only 'popsize' is read) and
 ``CMAEvolutionStrategy(x0, sigma, opts)`` whose ask() / tell() wrap oracle/cma_oracle.CMAState, the fp64 restatement of

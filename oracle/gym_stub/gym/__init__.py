@@ -1,14 +1,28 @@
-"""Minimal stand-in for the ``gym`` package so the reference's config.py / natural_es.py import and run
-verbatim in this container (``gym`` is not installed; config.py:1 imports it).  TEST INFRASTRUCTURE ONLY —
-used by oracle/make_golden.py and oracle/ref_cpu_baseline.py, never by the product package.
+"""Minimal stand-in for the ``gym`` package so the reference's config.py, natural_es.py and cma_es.py import and run
+verbatim here (``gym`` is not installed; config.py:1 imports it).  TEST INFRASTRUCTURE ONLY — used by
+oracle/make_golden.py and oracle/ref_cpu_baseline.py, never by the product package.
 
-``gym.make('Pendulum-v0')`` returns the restated Pendulum (see PendulumEnv).
-``gym.make('SynthTape-d<d0>-a<A>-T<T>-v0')`` returns the synthetic observation-tape environment of
-SURVEY.md §8d: a fixed tape X[T,d0], targets a*[T,A]; reward r_t = -||a_t - a*_t||^2 for the (already
-clipped, utils.py:134) action the agent passes; the episode ends after T steps.
+``gym.make(task)`` knows three tasks:
+  'Pendulum-v0'                    the restated Pendulum (PendulumEnv)
+  'SynthWalk-v0'                   oracle/synth_walk.py's host-stepped test environment
+  'SynthTape-d<d0>-a<A>-T<T>-v0'   the synthetic observation tape of SURVEY.md §8d: a fixed tape X[T,d0], targets
+                                   a*[T,A]; reward r_t = -||a_t - a*_t||^2 for the (already clipped, utils.py:134)
+                                   action the agent passes; the episode ends after T steps.
+The oracle modules are imported only when a task needs them, so the tape task runs with nothing but numpy.
+
+Episode keys: make() numbers every instance it returns from the counter ``instances``; a run that keys its episodes
+installs a fresh ``itertools.count()`` first, so that in a one-worker train() 0 = the config probe, 1 = the worker and
+2 + g = test() number g.  ``reset_hook(instance, episode)`` (module attribute), when set, gives the start of every
+Pendulum and SynthWalk episode: (theta, theta_dot) for Pendulum, the episode seed for SynthWalk.  Unset, Pendulum draws
+uniform(-[pi, 1], [pi, 1]) and SynthWalk resets from its current seed.
 """
+import itertools
 import re
+
 import numpy as np
+
+reset_hook = None
+instances = itertools.count()
 
 
 class _Box:
@@ -41,12 +55,9 @@ class SynthTapeEnv:
 
 
 class PendulumEnv:
-    """'Pendulum-v0' of OpenAI gym (classic_control/pendulum.py + the 200-step TimeLimit wrapper), restated from its
-    published dynamics: state (theta, theta_dot) in float64, torque clipped to +-2, speed to +-8, dt 0.05, g 10.
-
-    ``reset_hook(instance_index, episode_index) -> (theta, theta_dot)`` (module attribute ``pendulum_reset_hook``) lets
-    oracle/make_golden.py feed the counter-RNG reset states; without it reset() draws uniform(-[pi,1], [pi,1])."""
-    max_speed, max_torque, dt, horizon = 8.0, 2.0, 0.05, 200
+    """'Pendulum-v0' of OpenAI gym (classic_control/pendulum.py + the 200-step TimeLimit wrapper): state (theta,
+    theta_dot) in float64, stepped by oracle.pendulum_oracle.pendulum_step, the one restatement of its dynamics."""
+    horizon = 200
 
     def __init__(self, instance):
         self.instance = instance
@@ -60,8 +71,8 @@ class PendulumEnv:
         return np.array([np.cos(th), np.sin(th), thdot])
 
     def reset(self):
-        if pendulum_reset_hook is not None:
-            self.state = np.asarray(pendulum_reset_hook(self.instance, self.episode), dtype=np.float64)
+        if reset_hook is not None:
+            self.state = np.asarray(reset_hook(self.instance, self.episode), dtype=np.float64)
         else:
             high = np.array([np.pi, 1.0])
             self.state = self.np_random.uniform(low=-high, high=high)
@@ -70,27 +81,41 @@ class PendulumEnv:
         return self._obs()
 
     def step(self, u):
+        from oracle.pendulum_oracle import pendulum_step
         th, thdot = self.state
-        u = np.clip(u, -self.max_torque, self.max_torque)[0]
-        norm = ((th + np.pi) % (2 * np.pi)) - np.pi
-        costs = norm ** 2 + 0.1 * thdot ** 2 + 0.001 * (u ** 2)
-        newthdot = thdot + (-3 * 10.0 / 2 * np.sin(th + np.pi) + 3.0 * u) * self.dt
-        newth = th + newthdot * self.dt
-        newthdot = np.clip(newthdot, -self.max_speed, self.max_speed)
-        self.state = np.array([newth, newthdot])
+        th, thdot, reward = pendulum_step(th, thdot, u[0])
+        self.state = np.array([th, thdot])
         self.t += 1
-        return self._obs(), -costs, self.t >= self.horizon, {}
+        return self._obs(), reward, self.t >= self.horizon, {}
 
 
-pendulum_reset_hook = None
-_pendulum_instances = [0]
+class SeededEpisodes:
+    """A seed()-able environment (SynthWalk-v0) whose episodes are numbered like PendulumEnv's: reset_hook, when set,
+    gives each episode's seed."""
+
+    def __init__(self, env, instance):
+        self.env, self.instance, self.episode = env, instance, 0
+        self.observation_space, self.action_space = env.observation_space, env.action_space
+
+    def reset(self):
+        if reset_hook is not None:
+            self.env.seed(reset_hook(self.instance, self.episode))
+        self.episode += 1
+        return self.env.reset()
+
+    def step(self, action):
+        return self.env.step(action)
 
 
 def make(task):
+    instance = next(instances)
     if task == 'Pendulum-v0':
-        _pendulum_instances[0] += 1
-        return PendulumEnv(_pendulum_instances[0] - 1)
+        return PendulumEnv(instance)
+    if task == 'SynthWalk-v0':
+        from oracle import synth_walk
+        return SeededEpisodes(synth_walk.SynthWalkEnv(), instance)
     m = re.fullmatch(r'SynthTape-d(\d+)-a(\d+)-T(\d+)-v0', task)
     if m is None:
-        raise ValueError('gym stub only knows Pendulum-v0 and SynthTape-d<d0>-a<A>-T<T>-v0, got %r' % (task,))
+        raise ValueError('gym stand-in only knows Pendulum-v0, SynthWalk-v0 and SynthTape-d<d0>-a<A>-T<T>-v0, got %r'
+                         % (task,))
     return SynthTapeEnv(int(m.group(1)), int(m.group(2)), int(m.group(3)))

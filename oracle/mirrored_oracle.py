@@ -8,7 +8,8 @@ eps: the contract of the *_mirrored entry points of include/des_b200.h is
 so members 2p and 2p+1 are theta + sigma*eps_p and theta - sigma*eps_p.  Everything else of a generation (forward,
 fitness, fitness_shift over all N members, Adam) is the plain chain of nes_oracle.py; environment reset states and
 action noise stay keyed by the global member index.  Pinned by tests/golden/train_b64_mirrored.npz and
-train_closed_mirrored_pend.npz, written by oracle/make_golden_mirrored.py from the reference's own natural_es.train().
+train_closed_mirrored_pend.npz, written by oracle/make_golden.py from the reference's own natural_es.train() with
+np.random.randn serving noise_mirrored's rows.
 """
 import numpy as np
 

@@ -6,9 +6,10 @@ Restates, for the reference's PendulumConfig (config.py:26-31), what ``Evaluator
 
 The environment is a third-party dependency that is absent here: OpenAI ``gym`` (imported at config.py:1; the reference
 pins no version — 'Pendulum-v0' with a 200-step TimeLimit exists in gym 0.9-0.17).  Its published dynamics are restated
-in ``pendulum_step`` below; this part is therefore "parity unpinned" against gym itself.  What IS pinned: the rollout loop
-around it — tests/golden/train_closed_pend.npz is produced by the reference's own natural_es.train() running verbatim
-over oracle/gym_stub's Pendulum-v0 (the same restated dynamics), see oracle/make_golden.py.
+in ``pendulum_step`` below, the only restatement: oracle/gym_stub's Pendulum-v0 steps through it too.  This part is
+therefore "parity unpinned" against gym itself.  What IS pinned: the rollout loop around it —
+tests/golden/train_closed_pend.npz is produced by the reference's own natural_es.train() running verbatim over
+oracle/gym_stub's Pendulum-v0, see oracle/make_golden.py.
 
 Reset states come from the counter RNG (stream 2) so every process can regenerate them:
   Philox(counter = (repetition, member, generation, 2), key = seed) -> u = (low 23 bits + 0.5) / 2^23,

@@ -1,8 +1,8 @@
 """'SynthWalk-v0': a BipedalWalker-shaped test environment (obs 24, action 4) — TEST INFRASTRUCTURE ONLY.
 
-The host-stepped training path (engine.HostEnvEngine) is pinned with it: oracle/make_golden_host.py runs the reference's
-natural_es.train() verbatim on it, and the tests step the same dynamics through distributedes_b200.envs.GymEnvBatch.
-Its dynamics live here only.
+The host-stepped training path (engine.HostEnvEngine) is pinned with it: oracle/make_golden.py runs the reference's
+natural_es.train() verbatim on it (the stand-in gym's make('SynthWalk-v0')), and the tests step the same dynamics
+through distributedes_b200.envs.GymEnvBatch.  Its dynamics live here only.
 
   state s in R^24, fp64; reset state: 24 uniforms in (-1, 1) from the episode seed (below)
   s' = 0.8 s + 0.2 tanh(M s) + B a                       a = the (clipped) action, 4 entries

@@ -223,8 +223,8 @@ def test_bench_reference_arm_contract():
 
 def test_host_normaliser_matches_reference_arithmetic():
     """utils.SharedStats.feed / merge and StaticNormalizer.__call__ restate utils.py:37-96 in the reference's fp32
-    operation order: the fixture values below were produced by the reference classes on the same inputs
-    (RandomState(0), 5-dim observations) — see the inline generator in the docstring of oracle/make_golden.py."""
+    operation order: the expected values below are that arithmetic (StaticNormalizer's pass-through and scaling,
+    utils.py:48-51, and the Chan merge, utils.py:85-96) written out on 5-dim RandomState(0) observations."""
     from distributedes_b200.utils import SharedStats, StaticNormalizer
     rs = np.random.RandomState(0)
     a = StaticNormalizer(5)

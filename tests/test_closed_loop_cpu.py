@@ -1,5 +1,5 @@
 """Closed-loop rollouts (SURVEY 8f row 3) on CPU: the oracle against the reference's own natural_es.train() run
-verbatim on its PendulumConfig (tests/golden/train_closed_pend.npz, oracle/make_golden.py::golden_train_closed), and
+verbatim on its PendulumConfig (tests/golden/train_closed_pend.npz, oracle/make_golden.py::train_env), and
 the world_size-2 host logic of engine.RolloutEngine under gloo."""
 import os
 

@@ -1,5 +1,5 @@
 """Closed-loop CMA-ES on CPU: the oracle chain against the reference's own cma_es.train() run verbatim on its
-PendulumConfig(hidden_size=16) (tests/golden/train_cma_closed_pend.npz, oracle/make_golden_cma.py), the
+PendulumConfig(hidden_size=16) (tests/golden/train_cma_closed_pend.npz, oracle/make_golden.py::train_cma), the
 sharded host logic of cma_es.train under gloo, and the C ABI's argument checks for des_rollout_eval_solutions."""
 import os
 

@@ -1,5 +1,5 @@
 """Host-stepped environments on CPU: the oracle's host loop against the reference's own natural_es.train() run verbatim
-on SynthWalk-v0 (tests/golden/train_host_walk.npz, oracle/make_golden_host.py), the batch protocol adapter
+on SynthWalk-v0 (tests/golden/train_host_walk.npz, oracle/make_golden.py::train_env), the batch protocol adapter
 envs.GymEnvBatch, des_policy_act's argument checks, GymConfig without gym, and engine.HostEnvEngine on two gloo ranks."""
 import os
 import sys

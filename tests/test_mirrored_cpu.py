@@ -1,5 +1,5 @@
 """Mirrored (antithetic) sampling without a GPU: the oracle against the reference's own natural_es.train() run on explicit
-+-eps pairs (tests/golden/train_b64_mirrored.npz, train_closed_mirrored_pend.npz, oracle/make_golden_mirrored.py), the
++-eps pairs (tests/golden/train_b64_mirrored.npz, train_closed_mirrored_pend.npz, oracle/make_golden.py), the
 pair-form gradient, the evenness rules of the engines and the C entry points, checkpoints, and sharded NESEngine runs
 under gloo with 2 and 3 ranks against the single-process chain."""
 import ctypes as C
