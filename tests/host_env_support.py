@@ -63,6 +63,14 @@ def accumulate_stats(part, obs, alive):
 
 
 # ---- environments ------------------------------------------------------------------------------------------------------
+class PendulumProbe:
+    """The shapes of Pendulum-v0 with the classic gym API, for the configs' probe (PendulumBatch does the stepping)."""
+    class _Box:
+        def __init__(self, n):
+            self.shape = (n,)
+    observation_space, action_space = _Box(3), _Box(1)
+
+
 class PendulumBatch:
     """Pendulum-v0 (oracle/pendulum_oracle.py's dynamics) as a vectorised environment of the batch protocol: slot b
     resets from the counter stream of des_rollout_eval, Philox(repetition, member, generation, 2)."""

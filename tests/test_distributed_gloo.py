@@ -1,6 +1,9 @@
 """world_size=2 on CPU with gloo: the sharded generation (engine.NESEngine host logic) must produce exactly the
 single-process result: members split across ranks (even and ragged), fitness gathered by the zero-padded
-all-reduce, partial sums all-reduced, identical update on every rank."""
+all-reduce, partial sums all-reduced, identical update on every rank.  Also the launcher's timeout."""
+import multiprocessing
+import time
+
 import numpy as np
 import pytest
 
@@ -64,3 +67,15 @@ def test_sharded_generation_with_observation_normaliser():
                                    weight_decay=0.005, learning_rate=0.1)['theta']
         stats.merge_tape(obs, N * T)
     assert np.max(np.abs(thetas[0] - theta)) <= 2e-6
+
+
+def _sleep(seconds):
+    time.sleep(seconds)
+
+
+def test_spawn_kills_every_rank_after_its_timeout():
+    """A rank that never returns fails spawn with TimeoutError instead of hanging the suite, and leaves no process."""
+    before = set(multiprocessing.active_children())
+    with pytest.raises(TimeoutError):
+        spawn(2, _sleep, 300, timeout=10)
+    assert not set(multiprocessing.active_children()) - before

@@ -117,14 +117,6 @@ def _nes(mode, kernels):
                          clip=2.0, **common), Cfg(repetitions=2, test_repetitions=3)
 
 
-class PendulumProbe:
-    """The shapes of Pendulum-v0 with the classic gym API (the batch environment does the stepping)."""
-    class _Box:
-        def __init__(self, n):
-            self.shape = (n,)
-    observation_space, action_space = _Box(3), _Box(1)
-
-
 def _cma_config(mode, seed=7):
     from distributedes_b200.config import ClosedLoopPendulumConfig, HostEnvConfig, SynthTapeConfig
     from distributedes_b200.envs import GymEnvBatch
@@ -135,7 +127,7 @@ def _cma_config(mode, seed=7):
         cfg = ClosedLoopPendulumConfig(16)
         cfg.repetitions = cfg.test_repetitions = 2
     elif mode == 'host':
-        cfg = HostEnvConfig(PendulumProbe, hidden_size=16, clip=2.0, task='Pendulum-v0',
+        cfg = HostEnvConfig(hs.PendulumProbe, hidden_size=16, clip=2.0, task='Pendulum-v0',
                             batch_env_fn=lambda B: hs.PendulumBatch(B, seed, horizon=9))
         cfg.repetitions, cfg.test_repetitions = 2, 3
     else:       # episodes of varying length

@@ -134,36 +134,6 @@ def test_c_session_generation_host(precision, ftol):
     assert rc == -1 and b'shard' in lib.des_last_error()
 
 
-@pytest.mark.parametrize('tag', ['pend', 'b64'])
-def test_observation_normaliser_matches_reference_train(golden_dir, tag):
-    """NESEngine(normalize_obs=True) against natural_es.train() run verbatim WITH its StaticNormalizer/SharedStats
-    (tests/golden/train_norm_*.npz): gradient after weight decay, update and parameters, three generations."""
-    from distributedes_b200.engine import NESEngine
-    from distributedes_b200 import ops
-    g = np.load(os.path.join(golden_dir, 'train_norm_%s.npz' % tag))
-    d0, H, A, T = (int(v) for v in g['dims'])
-    N, seed = int(g['N']), int(g['seed'])
-    obs, target = orc.synthetic_tape(T, d0, A)
-    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=g['theta0'], obs=obs, target=target,
-                    sigma=float(g['sigma']), learning_rate=float(g['lr']), weight_decay=float(g['wd']), clip=float(g['clip']),
-                    seed=seed, precision='fp32', device='cuda:0', normalize_obs=True)
-    stats = orc.ObsStats(d0)
-    for gen in range(int(g['gens'])):
-        rew = eng.noiseless_fitness()                                   # test(), natural_es.py:54
-        assert abs(rew - g['test_rewards'][gen]) < 2e-5 * abs(g['test_rewards'][gen])
-        eng.generation()
-        grad = eng.partial.cpu().numpy().astype(np.float64) / N / float(g['sigma']) * (1 - float(g['wd']))
-        assert relnorm(grad, g['grad_after_wd'][gen]) <= 2e-5, gen      # N <= 24: no rank flips; noise/forward fp32 error
-        assert np.max(np.abs(eng.theta_numpy() - g['theta'][gen])) <= 2e-5
-        stats.merge_tape(obs, N * T)
-        sd = eng.stats_state_dict()
-        assert np.allclose(sd['m'], stats.m, atol=1e-6) and np.allclose(sd['v'], stats.v, rtol=1e-5) and sd['n'][0] == stats.n
-    # the normalised tape the kernels read is (o - m)/sqrt(v + 1e-6)
-    ref = np.stack([stats.normalize(o) for o in obs])
-    got = ops.obs_normalize(eng.obs_raw, eng.obs_stats).cpu().numpy()
-    assert np.max(np.abs(got - ref)) <= 1e-5
-
-
 def test_multi_runs_files_and_checkpoint_resume(tmp_path):
     """natural_es.py:113-124 bookkeeping: pickle of [[rewards, steps, timestamps], ...] + log file; and a checkpoint
     taken mid-run resumes to bit-identical parameters."""

@@ -4,10 +4,8 @@
   single-CTA and multi-pass tapes, with and without the tile workspace); member 2p+1 matches the fp32 forward of the
   des_nes_perturb_mirrored rows within the per-precision tolerances of test_gpu_ops.py.
 * Rows, the pair-form reduction (against an fp64 sum over the device's own normals), closed-loop and host-stepped
-  Pendulum, natural_es.train against the reference's verbatim run on explicit +-eps pairs (tests/golden/*_mirrored*),
-  graph capture and two GPUs."""
-import os
-
+  Pendulum and graph capture.  natural_es.train against the reference's verbatim run on explicit +-eps pairs is in
+  tests/test_gpu_goldens.py, two GPUs in tests/test_gpu_multi.py."""
 import numpy as np
 import pytest
 
@@ -19,7 +17,6 @@ from oracle import pendulum_oracle as po
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = {'fp32': 2e-5, 'f16x3': 3e-5, 'f16': 4e-3}
 RTOL = 2e-4
 
@@ -122,8 +119,6 @@ def test_closed_loop_equals_explicit_rows(H):
 def test_host_stepped_pendulum_equals_closed_loop():
     """HostEnvEngine(mirrored=True) stepping Pendulum-v0 on the host evaluates the members RolloutEngine(mirrored=True)
     evaluates on the device, and both match the oracle's mirrored closed-loop fitness."""
-    import sys
-    sys.path.insert(0, HERE)
     import host_env_support as hs
     from distributedes_b200.engine import HostEnvEngine, RolloutEngine
     H, N, reps, seed = 32, 12, 3, 5
@@ -141,72 +136,6 @@ def test_host_stepped_pendulum_equals_closed_loop():
     assert np.array_equal(host.rows[0::2].cpu().numpy(), ops().nes_perturb(dev(theta0), N // 2, 0.1, seed, 0).cpu().numpy())
 
 
-def relnorm(a, b):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.linalg.norm(a - b) / np.linalg.norm(b)
-
-
-def test_tape_train_matches_reference_golden():
-    """NESEngine(mirrored=True) against natural_es.train() run verbatim on explicit +-eps pairs: test rewards, gradient
-    after weight decay, Adam update and parameters for three generations (no rank flips at N = 24)."""
-    from distributedes_b200.engine import NESEngine
-    g = np.load(os.path.join(HERE, 'golden', 'train_b64_mirrored.npz'))
-    d0, H, A, T = (int(v) for v in g['dims'])
-    N, seed = int(g['N']), int(g['seed'])
-    obs, target = orc.synthetic_tape(T, d0, A)
-    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=N, theta0=g['theta0'], obs=obs, target=target,
-                    sigma=float(g['sigma']), learning_rate=float(g['lr']), weight_decay=float(g['wd']),
-                    clip=float(g['clip']), seed=seed, precision='fp32', device=DEV, mirrored=True)
-    for gen in range(int(g['gens'])):
-        rew = eng.noiseless_fitness()
-        assert abs(rew - g['test_rewards'][gen]) < 2e-5 * abs(g['test_rewards'][gen])
-        eng.generation()
-        grad = eng.partial.cpu().numpy().astype(np.float64) / N / float(g['sigma']) * (1 - float(g['wd']))
-        assert relnorm(grad, g['grad_after_wd'][gen]) <= 2e-5, gen
-        if gen >= 1:
-            assert relnorm(eng.update.cpu().numpy(), g['update'][gen]) <= 2e-5, gen
-        assert np.max(np.abs(eng.theta_numpy() - g['theta'][gen])) <= 2e-5
-
-
-def test_closed_loop_train_matches_reference_golden():
-    """natural_es.train(ClosedLoopPendulumConfig) with config.mirrored = True against the reference's verbatim run
-    (layered: the gradient chain on the device's own fitness, then against the golden when no rank flipped)."""
-    from distributedes_b200 import natural_es
-    from distributedes_b200.config import ClosedLoopPendulumConfig
-    g = np.load(os.path.join(HERE, 'golden', 'train_closed_mirrored_pend.npz'))
-    H, N, reps, seed, gens = int(g['H']), int(g['N']), int(g['reps']), int(g['seed']), int(g['gens'])
-    cfg = ClosedLoopPendulumConfig(hidden_size=H)
-    cfg.initial_weight = g['theta0'].copy()
-    cfg.pop_size, cfg.sigma, cfg.learning_rate, cfg.seed = N, float(g['sigma']), float(g['lr']), seed
-    cfg.repetitions = cfg.test_repetitions = reps
-    cfg.max_steps = (gens + 1) * N * reps * 200 - 1
-    cfg.mirrored = True
-    eng = natural_es.build_engine(cfg)
-    assert eng.mirrored
-    fits, stats = [], []
-    real_rank, real_apply = eng.rank_and_reduce, eng.apply
-
-    def spy_rank():
-        fits.append(eng.fitness_all.cpu().numpy().astype(np.float64))
-        return real_rank()
-
-    def spy_apply():
-        real_apply()
-        stats.append(eng.obs_stats.cpu().numpy().copy())
-    eng.rank_and_reduce, eng.apply = spy_rank, spy_apply
-    rewards, steps, _ = natural_es.train(cfg, engine=eng)
-    assert steps == list(g['train_steps'])
-    assert np.allclose(rewards, g['test_rewards'], rtol=RTOL)
-    theta, opt, P = g['theta0'].copy(), orc.Adam(), g['theta0'].size
-    for gen in range(gens):
-        assert np.allclose(stats[gen], g['stats'][gen], rtol=5e-4, atol=5e-5)
-        grad = mo.nes_gradient_streamed(orc.fitness_shift(fits[gen]), float(g['sigma']), seed, gen, P)
-        theta, _ = orc.nes_update(theta, grad, opt, float(g['wd']), float(g['lr']))
-    assert np.max(np.abs(eng.theta_numpy() - theta)) <= 1e-5 * np.max(np.abs(theta - g['theta0']))
-    if np.max(np.abs(theta - g['theta'][-1])) <= 2e-6:
-        assert np.max(np.abs(eng.theta_numpy() - g['theta'][-1])) <= 1e-5 * np.max(np.abs(g['theta'][-1] - g['theta0']))
-
-
 @pytest.mark.parametrize('precision', ['f16x3', 'f16'])
 def test_graph_captured_generation_equals_eager(precision):
     from distributedes_b200.engine import NESEngine
@@ -220,40 +149,3 @@ def test_graph_captured_generation_equals_eager(precision):
         b.generation()
         assert torch.equal(a.fitness_all, b.fitness_all) and torch.equal(a.theta, b.theta)
     assert not torch.equal(a.theta, torch.from_numpy(kw['theta0']).to(DEV))
-
-
-def _two_gpu_worker(rank, world, port, outdir):
-    import torch.distributed as dist
-    from distributedes_b200.engine import NESEngine
-    torch.cuda.set_device(rank)
-    dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world)
-    try:
-        d0, H, A, T = 24, 64, 4, 256
-        obs, target = orc.synthetic_tape(T, d0, A)
-        eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=22, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
-                        target=target, sigma=0.1, learning_rate=0.05, seed=3, precision='f16x3',
-                        device=torch.device('cuda', rank), mirrored=True)
-        for _ in range(2):
-            eng.generation()
-        np.savez(os.path.join(outdir, 'rank%d.npz' % rank), theta=eng.theta_numpy(), fit=eng.fitness_all.cpu().numpy(),
-                 offset=eng.offset, n_local=eng.n_local)
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason='needs 2 GPUs')
-def test_two_gpu_mirrored_equals_one_gpu(tmp_path):
-    import torch.multiprocessing as mp
-    from distributedes_b200.engine import NESEngine
-    mp.spawn(_two_gpu_worker, args=(2, 29871, str(tmp_path)), nprocs=2, join=True)
-    r = [np.load(str(tmp_path / ('rank%d.npz' % k))) for k in range(2)]
-    assert (int(r[0]['n_local']), int(r[1]['offset'])) == (12, 12)
-    assert np.array_equal(r[0]['theta'], r[1]['theta']) and np.array_equal(r[0]['fit'], r[1]['fit'])
-    d0, H, A, T = 24, 64, 4, 256
-    obs, target = orc.synthetic_tape(T, d0, A)
-    eng = NESEngine(state_dim=d0, hidden=H, action_dim=A, pop_size=22, theta0=orc.synthetic_theta(d0, H, A), obs=obs,
-                    target=target, sigma=0.1, learning_rate=0.05, seed=3, precision='f16x3', device=DEV, mirrored=True)
-    for _ in range(2):
-        eng.generation()
-    assert np.array_equal(eng.fitness_all.cpu().numpy(), r[0]['fit'])
-    assert np.max(np.abs(eng.theta_numpy() - r[0]['theta'])) <= 1e-6
