@@ -12,6 +12,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
+from .ops import _ptr
 
 
 class _DevArray:
@@ -52,8 +53,9 @@ class PeerComm:
                    'des_comm_allgather_fitness')
 
     def allreduce_partial(self, partial_local, out):
-        assert partial_local.is_cuda and out.is_cuda and partial_local.dtype == torch.float32 and out.dtype == torch.float32
-        _lib.check(self.lib.des_comm_allreduce_partial(self._h, C.c_void_p(out.data_ptr()), C.c_void_p(partial_local.data_ptr()),
+        dev = self.fitness_all.device
+        _lib.check(self.lib.des_comm_allreduce_partial(self._h, _ptr(out, 'out', torch.float32, self.P, dev),
+                                                       _ptr(partial_local, 'partial_local', torch.float32, self.P, dev),
                                                        self.P, self._stream()), 'des_comm_allreduce_partial')
 
     def close(self):

@@ -2,11 +2,13 @@
 
 PyTorch is plumbing here: it owns device memory and the stream; every op below passes raw
 pointers to libdes_b200.so, which enqueues hand-written sm_90a kernels on the current stream.
-CPU tensors are an error (there is no CPU fallback).
+The entry points cannot see how large an allocation is, so every tensor argument goes through _ptr first: dtype,
+contiguity, element count and device.  CPU tensors are an error (there is no CPU fallback).
 """
 from __future__ import annotations
 
 import ctypes as C
+import functools
 
 import torch
 
@@ -14,32 +16,52 @@ from . import _lib
 from ._lib import Dims, Opt, PRECISIONS, State
 from .envs import DeviceEnv
 
+F32, F64, U8, I32 = torch.float32, torch.float64, torch.uint8, torch.int32
+STATE_BYTES = C.sizeof(State)
+
 
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _ptr(t, dtype, name, allow_none=False):
-    if t is None:
-        if allow_none:
-            return C.c_void_p(0)
-        raise RuntimeError('%s is None' % name)
+def _ptr(t, name, dtype, n=None, dev=None, optional=False, need='needs'):
+    """The device pointer of tensor argument `name` (None for an omitted optional one), after checking in this order:
+    a tensor, of `dtype` (None: any), contiguous, `n` entries where the op fixes its shape, on the op's device `dev`
+    (None for the anchor, the tensor that selects the device)."""
+    if t is None and optional:
+        return None
     if not isinstance(t, torch.Tensor):
-        raise RuntimeError('%s must be a torch.Tensor' % name)
-    if not t.is_cuda:
-        raise RuntimeError('%s is a CPU tensor: distributedes_b200 has no CPU path' % name)
-    if t.dtype != dtype:
+        raise RuntimeError('%s must be a torch.Tensor, got %s' % (name, type(t).__name__))
+    if dtype is not None and t.dtype != dtype:
         raise RuntimeError('%s must be %s, got %s' % (name, dtype, t.dtype))
     if not t.is_contiguous():
         raise RuntimeError('%s must be contiguous' % name)
-    return C.c_void_p(t.data_ptr())
+    if n is not None and t.numel() != n:
+        raise RuntimeError('%s has %d entries, %s %d' % (name, t.numel(), need, n))
+    if dev is not None and t.device != dev:
+        raise RuntimeError('%s is on %s, the op runs on %s' % (name, t.device, dev))
+    return t.data_ptr()
 
 
-def _on(t, name):
-    """Device guard for the tensor that selects the GPU; CPU tensors are an error, not a fallback."""
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+def _ws(t, dev):
+    """(pointer, bytes) of a caller's workspace: any contiguous tensor on `dev`; the library judges its size."""
+    return _ptr(t, 'workspace', None, None, dev, True), 0 if t is None else t.numel() * t.element_size()
+
+
+def _launch(fn, anchor, name, *args):
+    """Entry point `fn` on the anchor's device and current stream, its arguments bound by _ptr.  The CPU check comes
+    after every argument is bound, so every check above runs without a GPU."""
+    if not anchor.is_cuda:
         raise RuntimeError('%s is a CPU tensor: distributedes_b200 has no CPU path' % name)
-    return torch.cuda.device(t.device)
+    with torch.cuda.device(anchor.device):
+        _lib.check(getattr(_lib.load(), fn)(*args, _stream()), fn)
+
+
+def _rows(t, name):
+    """n of a 2-D table t[n, P]."""
+    if not isinstance(t, torch.Tensor) or t.dim() != 2:
+        raise RuntimeError('%s must be a 2-D tensor [n, P], got shape %r' % (name, tuple(getattr(t, 'shape', ()))))
+    return t.shape[0]
 
 
 def _precision(p):
@@ -57,18 +79,21 @@ def param_count(state_dim, hidden, action_dim):
     return int(n)
 
 
+@functools.lru_cache(maxsize=None)
+def _mlp(d0, H, A):
+    """(P, how a count error about the weights of the (d0, H, A) MLP reads), cached: policy_act runs once per step."""
+    return param_count(d0, H, A), 'the (%d,%d,%d) MLP needs' % (d0, H, A)
+
+
 def new_state(device, generation=0):
     """Device-resident des_state {generation, adam_t, beta1_t, beta2_t} as a 32-byte tensor."""
-    st = torch.empty(C.sizeof(State), dtype=torch.uint8, device=device)
-    with torch.cuda.device(st.device):
-        _lib.check(_lib.load().des_state_init(C.c_void_p(st.data_ptr()), generation, _stream()), 'des_state_init')
+    st = torch.empty(STATE_BYTES, dtype=U8, device=device)
+    _launch('des_state_init', st, 'state', st.data_ptr(), generation)
     return st
 
 
 def state_advance(state, beta1=0.9, beta2=0.999):
-    with torch.cuda.device(state.device):
-        _lib.check(_lib.load().des_state_advance(_ptr(state, torch.uint8, 'state'), beta1, beta2, _stream()),
-                   'des_state_advance')
+    _launch('des_state_advance', state, 'state', _ptr(state, 'state', U8, STATE_BYTES), beta1, beta2)
 
 
 def read_state(state):
@@ -79,10 +104,8 @@ def read_state(state):
 
 def noise_fill(n_members, P, seed, generation, member_offset=0, stream_tag=0, device='cuda'):
     """eps[n_members, P] fp32 — debug/parity op (natural_es.py:29)."""
-    out = torch.empty((n_members, P), dtype=torch.float32, device=device)
-    with torch.cuda.device(out.device):
-        _lib.check(_lib.load().des_noise_fill(_ptr(out, torch.float32, 'out'), n_members, P, seed, generation,
-                                              member_offset, stream_tag, _stream()), 'des_noise_fill')
+    out = torch.empty((n_members, P), dtype=F32, device=device)
+    _launch('des_noise_fill', out, 'out', out.data_ptr(), n_members, P, seed, generation, member_offset, stream_tag)
     return out
 
 
@@ -99,34 +122,29 @@ def nes_perturb_mirrored(theta, n_members, sigma, seed, generation, member_offse
 
 
 def _perturb(fn, theta, n_members, sigma, seed, generation, member_offset, out):
-    P = theta.numel()
+    P, dev = theta.numel(), theta.device
     if out is None:
-        out = torch.empty((n_members, P), dtype=torch.float32, device=theta.device)
-    elif out.numel() != n_members * P:
-        raise RuntimeError('out has %d entries, need %d x %d' % (out.numel(), n_members, P))
-    with _on(theta, 'theta'):
-        _lib.check(getattr(_lib.load(), fn)(_ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'),
-                                            n_members, P, sigma, seed, generation, member_offset, _stream()), fn)
+        out = torch.empty((n_members, P), dtype=F32, device=dev)
+    _launch(fn, theta, 'theta', _ptr(out, 'out', F32, n_members * P, dev), _ptr(theta, 'theta', F32), n_members, P,
+            sigma, seed, generation, member_offset)
     return out
 
 
 def obs_stats_merge(stats, obs, n_feed):
     """SharedStats.merge of one generation's online statistics on the tape env (utils.py:85-96), in place."""
     T, d0 = obs.shape
-    with _on(obs, 'obs'):
-        _lib.check(_lib.load().des_obs_stats_merge(_ptr(stats, torch.float32, 'stats'), _ptr(obs, torch.float32, 'obs'),
-                                                   T, d0, float(n_feed), _stream()), 'des_obs_stats_merge')
+    _launch('des_obs_stats_merge', obs, 'obs', _ptr(stats, 'stats', F32, 2 * d0 + 1, obs.device), _ptr(obs, 'obs', F32),
+            T, d0, float(n_feed))
     return stats
 
 
 def obs_normalize(obs, stats, out=None):
     """StaticNormalizer.__call__ (utils.py:42-57) over the whole tape: identity while stats are empty."""
-    T, d0 = obs.shape
+    (T, d0), dev = obs.shape, obs.device
     if out is None:
-        out = torch.empty_like(obs)
-    with _on(obs, 'obs'):
-        _lib.check(_lib.load().des_obs_normalize(_ptr(out, torch.float32, 'out'), _ptr(obs, torch.float32, 'obs'),
-                                                 _ptr(stats, torch.float32, 'stats'), T, d0, _stream()), 'des_obs_normalize')
+        out = torch.empty((T, d0), dtype=F32, device=dev)
+    _launch('des_obs_normalize', obs, 'obs', _ptr(out, 'out', F32, T * d0, dev), _ptr(obs, 'obs', F32),
+            _ptr(stats, 'stats', F32, 2 * d0 + 1, dev), T, d0)
     return out
 
 
@@ -143,9 +161,9 @@ def rollout_eval(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, cl
                  workspace=None, out=None, episodes_out=None):
     """Closed-loop fitness of members [member_offset, member_offset + n_local): mean return over `repetitions`
     episodes stepped on the device (Evaluator.eval utils.py:116-124 over single_run utils.py:126-139)."""
-    return _rollout('des_rollout_eval', theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed,
-                    generation, state, member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out,
-                    episodes_out)
+    return _rollout('des_rollout_eval', theta, 'theta', (sigma, state, noiseless), env, hidden, horizon, repetitions,
+                    clip, action_noise_std, seed, generation, member_offset, n_local, obs_stats, totals_out, workspace,
+                    out, episodes_out)
 
 
 def rollout_eval_mirrored(theta, *, env=0, hidden, horizon=200, repetitions=10, sigma, clip, action_noise_std=0.0, seed,
@@ -153,28 +171,9 @@ def rollout_eval_mirrored(theta, *, env=0, hidden, horizon=200, repetitions=10, 
                           totals_out=None, workspace=None, out=None, episodes_out=None):
     """rollout_eval with mirrored noise: member m's weights are theta + (-1)^(m & 1) sigma*eps[m >> 1] (member_offset and
     n_local even; noiseless is rejected: test episodes use rollout_eval).  Episodes stay keyed by the global member."""
-    return _rollout('des_rollout_eval_mirrored', theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std,
-                    seed, generation, state, member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out,
-                    episodes_out)
-
-
-def _rollout(fn, theta, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed, generation, state,
-             member_offset, n_local, noiseless, obs_stats, totals_out, workspace, out, episodes_out):
-    d0, A = _env_dims(env)
-    if out is None:
-        out = torch.empty(n_local, dtype=torch.float32, device=theta.device)
-    if totals_out is not None and workspace is None:
-        workspace = torch.empty(max(n_local, 1) * (2 * d0 + 1), dtype=torch.float64, device=theta.device)
-    ws_bytes = workspace.numel() * workspace.element_size() if workspace is not None else 0
-    with _on(theta, 'theta'):
-        _lib.check(getattr(_lib.load(), fn)(
-            _ptr(out, torch.float32, 'out'), _ptr(episodes_out, torch.float32, 'episodes_out', True),
-            _ptr(totals_out, torch.float64, 'totals_out', True), _ptr(theta, torch.float32, 'theta'),
-            _ptr(obs_stats, torch.float32, 'obs_stats', True), int(env), Dims(d0, hidden, A, horizon), int(repetitions),
-            float(sigma), float(clip), float(action_noise_std), int(seed), int(generation),
-            _ptr(state, torch.uint8, 'state', True), int(member_offset), int(n_local), 1 if noiseless else 0,
-            C.c_void_p(workspace.data_ptr()) if workspace is not None else C.c_void_p(0), ws_bytes, _stream()), fn)
-    return out
+    return _rollout('des_rollout_eval_mirrored', theta, 'theta', (sigma, state, noiseless), env, hidden, horizon,
+                    repetitions, clip, action_noise_std, seed, generation, member_offset, n_local, obs_stats, totals_out,
+                    workspace, out, episodes_out)
 
 
 def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions=10, clip, action_noise_std=0.0, seed,
@@ -182,36 +181,42 @@ def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions
                            episodes_out=None):
     """Closed-loop fitness of explicit solutions[n_local, P] (CMA-ES's ask() rows, cma_es.py:22-29): row i is global
     member member_offset + i, whose episodes reset from the same counter stream as rollout_eval's member."""
+    return _rollout('des_rollout_eval_solutions', solutions, 'solutions', None, env, hidden, horizon, repetitions, clip,
+                    action_noise_std, seed, generation, member_offset, _rows(solutions, 'solutions'), obs_stats,
+                    totals_out, workspace, out, episodes_out)
+
+
+def _rollout(fn, weights, name, noise, env, hidden, horizon, repetitions, clip, action_noise_std, seed, generation,
+             member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out):
+    """The launch of rollout_eval[_mirrored] (weights = theta[P], noise = (sigma, state, noiseless)) and of
+    rollout_eval_solutions (weights = solutions[n_local, P], noise = None)."""
     d0, A = _env_dims(env)
-    if solutions.dim() != 2:
-        raise RuntimeError('solutions must be [n_local, P], got shape %r' % (tuple(solutions.shape),))
-    n_local, P = solutions.shape
-    if P != param_count(d0, hidden, A):
-        raise RuntimeError('solutions have %d entries, the (%d,%d,%d) MLP needs %d' % (P, d0, hidden, A, param_count(d0, hidden, A)))
+    P, mlp = _mlp(d0, int(hidden), A)
+    n_local, reps, w, dev = int(n_local), int(repetitions), 2 * d0 + 1, weights.device
     if out is None:
-        out = torch.empty(n_local, dtype=torch.float32, device=solutions.device)
-    elif out.numel() != n_local:
-        raise RuntimeError('out has %d entries, need n_local=%d' % (out.numel(), n_local))
+        out = torch.empty(n_local, dtype=F32, device=dev)
     if totals_out is not None and workspace is None:
-        workspace = torch.empty(max(n_local, 1) * (2 * d0 + 1), dtype=torch.float64, device=solutions.device)
-    ws_bytes = workspace.numel() * workspace.element_size() if workspace is not None else 0
-    with _on(solutions, 'solutions'):
-        _lib.check(_lib.load().des_rollout_eval_solutions(
-            _ptr(out, torch.float32, 'out'), _ptr(episodes_out, torch.float32, 'episodes_out', True),
-            _ptr(totals_out, torch.float64, 'totals_out', True), _ptr(solutions, torch.float32, 'solutions'),
-            _ptr(obs_stats, torch.float32, 'obs_stats', True), int(env), Dims(d0, hidden, A, horizon), int(repetitions),
-            float(clip), float(action_noise_std), int(seed), int(generation), int(member_offset), int(n_local),
-            C.c_void_p(workspace.data_ptr()) if workspace is not None else C.c_void_p(0), ws_bytes, _stream()),
-            'des_rollout_eval_solutions')
+        workspace = torch.empty(max(n_local, 1) * w, dtype=F64, device=dev)
+    head = (_ptr(out, 'out', F32, n_local, dev), _ptr(episodes_out, 'episodes_out', F32, n_local * reps, dev, True),
+            _ptr(totals_out, 'totals_out', F64, w, dev, True),
+            _ptr(weights, name, F32, P, need=mlp) if noise else _ptr(weights, name, F32, n_local * P, need=mlp + ' n x P ='),
+            _ptr(obs_stats, 'obs_stats', F32, w, dev, True), int(env), Dims(d0, hidden, A, horizon), reps)
+    tail = (float(clip), float(action_noise_std), int(seed), int(generation))
+    if noise:     # des_rollout_eval[_mirrored]: sigma before clip, state after the generation, noiseless after n_local
+        sigma, state, noiseless = noise
+        args = head + (float(sigma),) + tail + (_ptr(state, 'state', U8, STATE_BYTES, dev, True), int(member_offset),
+                                                n_local, 1 if noiseless else 0)
+    else:
+        args = head + tail + (int(member_offset), n_local)
+    _launch(fn, weights, name, *args, *_ws(workspace, dev))
     return out
 
 
 def obs_stats_merge_totals(stats, totals, state_dim):
     """Chan merge of a batch given by fp64 [sum | sum of squares | count] into stats [m|v|n] (utils.py:85-96)."""
-    with _on(stats, 'stats'):
-        _lib.check(_lib.load().des_obs_stats_merge_totals(_ptr(stats, torch.float32, 'stats'),
-                                                          _ptr(totals, torch.float64, 'totals'), int(state_dim), _stream()),
-                   'des_obs_stats_merge_totals')
+    w = 2 * int(state_dim) + 1
+    _launch('des_obs_stats_merge_totals', stats, 'stats', _ptr(stats, 'stats', F32, w),
+            _ptr(totals, 'totals', F64, w, stats.device), int(state_dim))
     return stats
 
 
@@ -221,40 +226,29 @@ def policy_act(rows, obs, alive, *, state_dim, hidden, action_dim, repetitions, 
     actions[n_local, repetitions, A] of rows[n_local, P] for raw obs[n_local, repetitions, d0] and alive (uint8) of the
     same leading shape; dead slots get 0.  stat_part (fp64 [n_local, 2*d0+1]) accumulates the raw observation
     statistics of the alive slots."""
-    if rows.dim() != 2:
-        raise RuntimeError('rows must be [n_local, P], got shape %r' % (tuple(rows.shape),))
-    n_local, P = rows.shape
+    n_local, dev = _rows(rows, 'rows'), rows.device
     d0, A, reps = int(state_dim), int(action_dim), int(repetitions)
-    if obs.numel() != n_local * reps * d0 or alive.numel() != n_local * reps:
-        raise RuntimeError('obs / alive have %d / %d entries, need %d x %d x %d / %d x %d'
-                           % (obs.numel(), alive.numel(), n_local, reps, d0, n_local, reps))
-    if stat_part is not None and stat_part.numel() != n_local * (2 * d0 + 1):
-        raise RuntimeError('stat_part has %d entries, need %d x %d' % (stat_part.numel(), n_local, 2 * d0 + 1))
+    P, mlp = _mlp(d0, int(hidden), A)
     if out is None:
-        out = torch.empty((n_local, reps, A), dtype=torch.float32, device=rows.device)
-    elif out.numel() != n_local * reps * A:
-        raise RuntimeError('out has %d entries, need %d x %d x %d' % (out.numel(), n_local, reps, A))
-    with _on(rows, 'rows'):
-        _lib.check(_lib.load().des_policy_act(
-            _ptr(out, torch.float32, 'out'), _ptr(stat_part, torch.float64, 'stat_part', True),
-            _ptr(rows, torch.float32, 'rows'), int(P), _ptr(obs, torch.float32, 'obs'), _ptr(alive, torch.uint8, 'alive'),
-            _ptr(obs_stats, torch.float32, 'obs_stats', True), Dims(d0, int(hidden), A, 0), reps, float(clip),
-            float(action_noise_std), int(seed), int(generation), int(member_offset), int(n_local), int(t), _stream()),
-            'des_policy_act')
+        out = torch.empty((n_local, reps, A), dtype=F32, device=dev)
+    _launch('des_policy_act', rows, 'rows', _ptr(out, 'out', F32, n_local * reps * A, dev),
+            _ptr(stat_part, 'stat_part', F64, n_local * (2 * d0 + 1), dev, True),
+            _ptr(rows, 'rows', F32, n_local * P, need=mlp + ' n x P ='), P, _ptr(obs, 'obs', F32, n_local * reps * d0, dev),
+            _ptr(alive, 'alive', U8, n_local * reps, dev), _ptr(obs_stats, 'obs_stats', F32, 2 * d0 + 1, dev, True),
+            Dims(d0, int(hidden), A, 0), reps, float(clip), float(action_noise_std), int(seed), int(generation),
+            int(member_offset), n_local, int(t))
     return out
 
 
 def obs_parts_reduce(parts, state_dim, out=None):
     """totals[2*d0+1] fp64 = sum of the stat_part rows [n_local, 2*d0+1] in member order."""
-    w = 2 * int(state_dim) + 1
+    w, pp = 2 * int(state_dim) + 1, _ptr(parts, 'parts', F64)
     n_local = parts.numel() // w
     if parts.numel() != n_local * w:
         raise RuntimeError('parts has %d entries, not a multiple of 2*d0+1 = %d' % (parts.numel(), w))
     if out is None:
-        out = torch.empty(w, dtype=torch.float64, device=parts.device)
-    with _on(parts, 'parts'):
-        _lib.check(_lib.load().des_obs_parts_reduce(_ptr(out, torch.float64, 'out'), _ptr(parts, torch.float64, 'parts'),
-                                                    int(n_local), int(state_dim), _stream()), 'des_obs_parts_reduce')
+        out = torch.empty(w, dtype=F64, device=parts.device)
+    _launch('des_obs_parts_reduce', parts, 'parts', _ptr(out, 'out', F64, w, parts.device), pp, n_local, int(state_dim))
     return out
 
 
@@ -283,42 +277,37 @@ def nes_eval_mirrored(theta, obs, target, *, hidden, sigma, clip, seed, generati
                      member_offset, n_local, precision, out, workspace)
 
 
+def _tape(obs, target, dev):
+    """(T, d0, A) and the pointers of the tape obs[T, d0], target[T, A] of nes_eval and pop_eval."""
+    po, pt = _ptr(obs, 'obs', F32, None, dev), _ptr(target, 'target', F32, None, dev)
+    if obs.dim() != 2 or target.dim() != 2 or target.shape[0] != obs.shape[0]:
+        raise RuntimeError('the tape is obs[T, d0] and target[T, A]: obs has shape %r, target %r'
+                           % (tuple(obs.shape), tuple(target.shape)))
+    return obs.shape[0], obs.shape[1], target.shape[1], po, pt
+
+
 def _nes_eval(fn, theta, obs, target, hidden, sigma, clip, seed, generation, state, member_offset, n_local, precision,
               out, workspace):
-    T, d0 = obs.shape
-    A = target.shape[1]
-    if target.shape[0] != T:
-        raise RuntimeError('obs has %d rows but target has %d' % (T, target.shape[0]))
-    if theta.numel() != param_count(d0, hidden, A):
-        raise RuntimeError('theta has %d entries, the (%d,%d,%d) MLP needs %d' %
-                           (theta.numel(), d0, hidden, A, param_count(d0, hidden, A)))
+    dev = theta.device
+    T, d0, A, po, pt = _tape(obs, target, dev)
+    P, mlp = _mlp(d0, int(hidden), A)
     if out is None:
-        out = torch.empty(n_local, dtype=torch.float32, device=theta.device)
-    elif out.numel() != n_local:
-        raise RuntimeError('out has %d entries, need n_local=%d' % (out.numel(), n_local))
-    with _on(theta, 'theta'):
-        _lib.check(getattr(_lib.load(), fn)(
-            _ptr(out, torch.float32, 'out'), _ptr(theta, torch.float32, 'theta'), _ptr(obs, torch.float32, 'obs'),
-            _ptr(target, torch.float32, 'target'), Dims(d0, hidden, A, T), sigma, clip, seed, generation,
-            _ptr(state, torch.uint8, 'state', allow_none=True), member_offset, n_local, _precision(precision),
-            _ptr(workspace, torch.uint8, 'workspace', allow_none=True), workspace.numel() if workspace is not None else 0,
-            _stream()), fn)
+        out = torch.empty(n_local, dtype=F32, device=dev)
+    _launch(fn, theta, 'theta', _ptr(out, 'out', F32, n_local, dev), _ptr(theta, 'theta', F32, P, need=mlp), po, pt,
+            Dims(d0, hidden, A, T), sigma, clip, seed, generation, _ptr(state, 'state', U8, STATE_BYTES, dev, True),
+            member_offset, n_local, _precision(precision), *_ws(workspace, dev))
     return out
 
 
 def pop_eval(solutions, obs, target, *, hidden, clip, out=None):
     """Tape fitness of explicit weight vectors solutions[n, P] (what CMA-ES evaluates, cma_es.py:62-75)."""
-    T, d0 = obs.shape
-    A = target.shape[1]
-    n, P = solutions.shape
-    if P != param_count(d0, hidden, A):
-        raise RuntimeError('solutions have %d entries, the (%d,%d,%d) MLP needs %d' % (P, d0, hidden, A, param_count(d0, hidden, A)))
+    n, dev = _rows(solutions, 'solutions'), solutions.device
+    T, d0, A, po, pt = _tape(obs, target, dev)
+    P, mlp = _mlp(d0, int(hidden), A)
     if out is None:
-        out = torch.empty(n, dtype=torch.float32, device=solutions.device)
-    with _on(solutions, 'solutions'):
-        _lib.check(_lib.load().des_pop_eval(_ptr(out, torch.float32, 'out'), _ptr(solutions, torch.float32, 'solutions'),
-                                            _ptr(obs, torch.float32, 'obs'), _ptr(target, torch.float32, 'target'),
-                                            Dims(d0, hidden, A, T), clip, n, _stream()), 'des_pop_eval')
+        out = torch.empty(n, dtype=F32, device=dev)
+    _launch('des_pop_eval', solutions, 'solutions', _ptr(out, 'out', F32, n, dev),
+            _ptr(solutions, 'solutions', F32, n * P, need=mlp + ' n x P ='), po, pt, Dims(d0, hidden, A, T), clip, n)
     return out
 
 
@@ -329,21 +318,17 @@ def rank_workspace(n_local, device, N):
 
 def centered_rank(fitness_all, member_offset=0, n_local=None, *, workspace=None, return_ranks=False, out=None):
     """fitness_shift (utils.py:142-148) for a shard of the global fitness vector."""
-    _on(fitness_all, 'fitness_all')
-    N = fitness_all.numel()
+    pf = _ptr(fitness_all, 'fitness_all', F32)
+    N, dev = fitness_all.numel(), fitness_all.device
     if n_local is None:
         n_local = N - member_offset
-    dev = fitness_all.device
     if out is None:
-        out = torch.empty(n_local, dtype=torch.float32, device=dev)
-    ranks = torch.empty(n_local, dtype=torch.int32, device=dev) if return_ranks else None
+        out = torch.empty(n_local, dtype=F32, device=dev)
+    ranks = torch.empty(n_local, dtype=I32, device=dev) if return_ranks else None
     if workspace is None:
         workspace = rank_workspace(n_local, dev, N)
-    with _on(fitness_all, 'fitness_all'):
-        _lib.check(_lib.load().des_centered_rank(
-            _ptr(out, torch.float32, 'out'), _ptr(ranks, torch.int32, 'ranks', allow_none=True),
-            _ptr(fitness_all, torch.float32, 'fitness_all'), N, member_offset, n_local,
-            _ptr(workspace, torch.uint8, 'workspace'), workspace.numel(), _stream()), 'des_centered_rank')
+    _launch('des_centered_rank', fitness_all, 'fitness_all', _ptr(out, 'out', F32, n_local, dev),
+            _ptr(ranks, 'ranks', I32, n_local, dev, True), pf, N, member_offset, n_local, *_ws(workspace, dev))
     return (out, ranks) if return_ranks else out
 
 
@@ -366,33 +351,26 @@ def nes_grad_partial_mirrored(shaped_local, P, *, seed, generation=0, state=None
 
 
 def _grad_partial(fn, shaped_local, P, seed, generation, state, member_offset, workspace, out):
-    _on(shaped_local, 'shaped_local')
-    n_local = shaped_local.numel()
-    dev = shaped_local.device
+    ps = _ptr(shaped_local, 'shaped_local', F32)
+    n_local, dev = shaped_local.numel(), shaped_local.device
     if out is None:
-        out = torch.empty(P, dtype=torch.float32, device=dev)
+        out = torch.empty(P, dtype=F32, device=dev)
     if workspace is None:
         workspace = grad_workspace(n_local, P, dev)
-    with _on(shaped_local, 'shaped_local'):
-        _lib.check(getattr(_lib.load(), fn)(
-            _ptr(out, torch.float32, 'out'), _ptr(shaped_local, torch.float32, 'shaped_local'), n_local, P, seed,
-            generation, _ptr(state, torch.uint8, 'state', allow_none=True), member_offset,
-            _ptr(workspace, torch.uint8, 'workspace'), workspace.numel(), _stream()), fn)
+    _launch(fn, shaped_local, 'shaped_local', _ptr(out, 'out', F32, P, dev), ps, n_local, P, seed, generation,
+            _ptr(state, 'state', U8, STATE_BYTES, dev, True), member_offset, *_ws(workspace, dev))
     return out
 
 
 def nes_apply(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learning_rate, weight_decay=0.005,
               beta1=0.9, beta2=0.999, epsilon=1e-8, update_out=None, grad_out=None):
     """natural_es.py:92-96 + utils.py:159-166, in place on theta / adam_m / adam_v (fp64 Adam state)."""
-    P = theta.numel()
-    with _on(theta, 'theta'):
-        _lib.check(_lib.load().des_nes_apply(
-            _ptr(theta, torch.float32, 'theta'), _ptr(adam_m, torch.float64, 'adam_m'),
-            _ptr(adam_v, torch.float64, 'adam_v'), _ptr(update_out, torch.float32, 'update_out', allow_none=True),
-            _ptr(grad_out, torch.float64, 'grad_out', allow_none=True),
-            _ptr(partial_sum, torch.float32, 'partial_sum'), P, N,
-            Opt(sigma, learning_rate, weight_decay, beta1, beta2, epsilon), _ptr(state, torch.uint8, 'state'),
-            _stream()), 'des_nes_apply')
+    pt = _ptr(theta, 'theta', F32)
+    P, dev = theta.numel(), theta.device
+    _launch('des_nes_apply', theta, 'theta', pt, _ptr(adam_m, 'adam_m', F64, P, dev), _ptr(adam_v, 'adam_v', F64, P, dev),
+            _ptr(update_out, 'update_out', F32, P, dev, True), _ptr(grad_out, 'grad_out', F64, P, dev, True),
+            _ptr(partial_sum, 'partial_sum', F32, P, dev), P, N,
+            Opt(sigma, learning_rate, weight_decay, beta1, beta2, epsilon), _ptr(state, 'state', U8, STATE_BYTES, dev))
 
 
 _CMA_WS = {}      # (device, n, lambda) -> workspace tensor of des_cma_rank_mu (tensor-core shapes only)
@@ -400,41 +378,32 @@ CMA_TC_MIN_N = 2048      # des_cma_rank_mu runs n >= this on the tensor cores, s
 
 
 def _cma_rank_mu(Y, w, out, packed):
-    lam, n = Y.shape
-    if w.numel() != lam:
-        raise RuntimeError('w has %d entries, Y has %d rows' % (w.numel(), lam))
+    lam, n, dev = _rows(Y, 'Y'), Y.shape[1], Y.device
+    size = cma_packed_elems(n) if packed else n * n
+    if out is None:
+        out = torch.empty(size if packed else (n, n), dtype=F32, device=dev)
     lib = _lib.load()
-    key = (str(Y.device), int(n), int(lam))
+    key = (str(dev), int(n), int(lam))
     ws = _CMA_WS.get(key)
     if ws is None:
-        ws = torch.empty(int(lib.des_cma_rank_mu_workspace_bytes(int(n), int(lam))), dtype=torch.uint8, device=Y.device)
+        ws = torch.empty(int(lib.des_cma_rank_mu_workspace_bytes(int(n), int(lam))), dtype=torch.uint8, device=dev)
         if len(_CMA_WS) > 8:
             _CMA_WS.clear()
         _CMA_WS[key] = ws
-    with _on(Y, 'Y'):
-        _lib.check(lib.des_cma_rank_mu(_ptr(out, torch.float32, 'out'), _ptr(Y, torch.float32, 'Y'),
-                                       _ptr(w, torch.float32, 'w'), lam, n, 1 if packed else 0,
-                                       C.c_void_p(ws.data_ptr()), ws.numel(), _stream()), 'des_cma_rank_mu')
+    _launch('des_cma_rank_mu', Y, 'Y', _ptr(out, 'out', F32, size, dev), _ptr(Y, 'Y', F32), _ptr(w, 'w', F32, lam, dev),
+            lam, n, 1 if packed else 0, ws.data_ptr(), ws.numel())
     return out
 
 
 def cma_rank_mu(Y, w, out=None):
     """dC[n,n] = sum_i w_i y_i y_i^T for Y[lambda_local, n] (rank-mu term of es.tell, cma_es.py:90).
     Tensor cores (split-fp16 wgmma SYRK) for n >= CMA_TC_MIN_N, fp32 FFMA below."""
-    lam, n = Y.shape
-    if out is None:
-        out = torch.empty((n, n), dtype=torch.float32, device=Y.device)
     return _cma_rank_mu(Y, w, out, False)
 
 
 def cma_cov_apply(Cmat, dC, pc, *, decay, c1, cmu):
     """C <- decay*C + c1*pc pc^T + cmu*dC, in place."""
-    n = Cmat.shape[0]
-    with _on(Cmat, 'C'):
-        _lib.check(_lib.load().des_cma_cov_apply(_ptr(Cmat, torch.float32, 'C'), _ptr(dC, torch.float32, 'dC'),
-                                                 _ptr(pc, torch.float32, 'pc', allow_none=True), n, decay, c1, cmu,
-                                                 _stream()), 'des_cma_cov_apply')
-    return Cmat
+    return _cov_apply('des_cma_cov_apply', Cmat, dC, 'dC', False, pc, decay, c1, cmu)
 
 
 def cma_packed_elems(n):
@@ -443,17 +412,16 @@ def cma_packed_elems(n):
 
 def cma_rank_mu_packed(Y, w, out=None):
     """The rank-mu partial as packed upper-triangular tiles (the multi-GPU all-reduce payload: half of [n, n])."""
-    n = Y.shape[1]
-    if out is None:
-        out = torch.empty(cma_packed_elems(n), dtype=torch.float32, device=Y.device)
     return _cma_rank_mu(Y, w, out, True)
 
 
 def cma_cov_apply_packed(Cmat, tiles, pc, *, decay, c1, cmu):
     """C <- decay*C + c1*pc pc^T + cmu*dC with dC as packed upper tiles, in place."""
-    n = Cmat.shape[0]
-    with _on(Cmat, 'C'):
-        _lib.check(_lib.load().des_cma_cov_apply_packed(_ptr(Cmat, torch.float32, 'C'), _ptr(tiles, torch.float32, 'tiles'),
-                                                        _ptr(pc, torch.float32, 'pc', allow_none=True), n, decay, c1, cmu,
-                                                        _stream()), 'des_cma_cov_apply_packed')
+    return _cov_apply('des_cma_cov_apply_packed', Cmat, tiles, 'tiles', True, pc, decay, c1, cmu)
+
+
+def _cov_apply(fn, Cmat, dC, name, packed, pc, decay, c1, cmu):
+    n, dev = Cmat.shape[0], Cmat.device
+    _launch(fn, Cmat, 'Cmat', _ptr(Cmat, 'Cmat', F32, n * n), _ptr(dC, name, F32, cma_packed_elems(n) if packed else n * n, dev),
+            _ptr(pc, 'pc', F32, n, dev, True), n, decay, c1, cmu)
     return Cmat
