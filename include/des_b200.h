@@ -304,10 +304,15 @@ DES_API int des_state_advance(des_state *state_dev, double beta1, double beta2, 
  * already sorted/weighted by the caller), written to out_dev as the full symmetric [n][n] matrix (packed == 0) or as
  * packed upper-triangular tiles (packed != 0, layout below).  lambda_local == 0 writes zeros.  The library picks the
  * kernel from n: below 2048 fp32 FFMA (fp32 accumulation per k-panel); from 2048 on the tensor cores
- * (csrc/des_cma_tc.cu: dC = Zs^T Z with Z = diag(sqrt|w|) Y, operands split into fp16 hi + lo, three wgmma MMAs per
- * k-step, fp32 accumulation, TMA-fed; |sqrt|w_k| * y| must stay below 65504).  Both stay within 1e-5 of the fp64
- * restatement in both norms.  workspace: des_cma_rank_mu_workspace_bytes(n, lambda_local) bytes (0 where the FFMA
- * kernel runs: workspace_dev may then be NULL), or DES_ERR_WORKSPACE. */
+ * (csrc/des_cma_tc.cu: dC = Zs^T Z with Z = diag(sqrt|w|) Y, each column of Z scaled by a power of two, operands split
+ * into fp16 hi + lo, three wgmma MMAs per k-step, fp32 accumulation, TMA-fed).  Accuracy is stated per entry against
+ * the exact sum of the fp32 inputs, with S_ij = sum_k |w_k y_ki y_kj|: the FFMA kernel within about (lambda + 1) 2^-24
+ * S_ij; the tensor cores within about 2^-21 S_ij of operand rounding plus 2^-22 S_ij per wgmma of the longer K half
+ * (3 per 16 members), at any scale of Y's columns as long as dC stays in fp32's normal range (the worst case, term by
+ * term: oracle/rank_mu_error.py).  Scaling column j of Y by 2^s scales row and column j of dC by 2^s exactly, and a
+ * NaN or inf in column j reaches only row and column j.
+ * workspace: des_cma_rank_mu_workspace_bytes(n, lambda_local) bytes (0 where the FFMA kernel runs: workspace_dev may
+ * then be NULL), or DES_ERR_WORKSPACE. */
 DES_API size_t des_cma_rank_mu_workspace_bytes(int64_t n, int64_t lambda_local);
 DES_API int des_cma_rank_mu(float *out_dev, const float *Y_dev, const float *w_dev, int64_t lambda_local, int64_t n,
                             int packed, void *workspace_dev, size_t workspace_bytes, void *stream);
