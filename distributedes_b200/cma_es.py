@@ -15,10 +15,9 @@ import time
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
-from . import fitness, ops
-from .engine import shard_bounds
+from . import fitness
+from .engine import RankGroup, kernels_and_device
 from .utils import StaticNormalizer, logger
 
 
@@ -51,20 +50,11 @@ class CMAEvolutionStrategy:
     test-suite with an oracle-backed stand-in; the product never runs without the CUDA library."""
 
     def __init__(self, x0, sigma0, popsize, seed=0, device=None, process_group=None, kernels=None):
-        if kernels is None:
-            self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
-            if self.device.type != 'cuda':
-                raise RuntimeError('distributedes_b200.cma_es needs a CUDA device: there is no CPU fallback')
-            kernels = ops
-        else:
-            self.device = torch.device(device if device is not None else 'cpu')
-        self.kn = kernels
-        self.pg = process_group
-        distributed = dist.is_available() and dist.is_initialized()
-        self.world = dist.get_world_size(process_group) if distributed else 1
-        self.rank = dist.get_rank(process_group) if distributed else 0
+        self.kn, self.device = kernels_and_device(kernels, device)
+        self.group = RankGroup(process_group)
+        self.world, self.rank = self.group.world, self.group.rank
         self.n, self.lam, self.seed = len(x0), int(popsize), int(seed)
-        self.offset, self.n_local = shard_bounds(self.lam, self.world, self.rank)
+        self.offset, self.n_local = self.group.shard(self.lam)
         k = cma_constants(self.n, self.lam)
         self.k = k
         dev, f64 = self.device, torch.float64
@@ -101,12 +91,7 @@ class CMAEvolutionStrategy:
     def gather_cost(self, cost_local):
         """[lambda] costs from the ranks' shards: all-reduce of the zero-padded vector (== all-gather, ragged allowed)."""
         cost_local = torch.as_tensor(cost_local, device=self.device, dtype=torch.float32).reshape(-1)
-        if self.world == 1:
-            return cost_local
-        full = torch.zeros(self.lam, dtype=torch.float32, device=self.device)
-        full[self.offset:self.offset + self.n_local] = cost_local
-        dist.all_reduce(full, group=self.pg)
-        return full
+        return self.group.gather(cost_local, self.offset, self.lam)
 
     def tell(self, solutions, cost):
         """cma_es.py:90.  solutions: the rank's [n_local, n] (as returned by ask; all lambda on a single GPU),
@@ -140,14 +125,13 @@ class CMAEvolutionStrategy:
                 self.kn.cma_rank_mu_packed(Y32, w32, out=self.dC_tiles)
             else:
                 self.dC_tiles.zero_()
-            dist.all_reduce(self.dC_tiles, group=self.pg)                     # the CMA collective of north_star
+            self.group.sum_(self.dC_tiles)                                    # the CMA collective of north_star
         else:
             if self.n_local:
                 self.kn.cma_rank_mu(Y32, w32, out=self.dC)
             else:
                 self.dC.zero_()
-        if self.world > 1:
-            dist.all_reduce(yw, group=self.pg)
+        self.group.sum_(yw)
         self.m = self.m + self.sigma * yw
         cs, ds, cc, c1, cmu, mu_eff = k['cs'], k['ds'], k['cc'], k['c1'], k['cmu'], k['mu_eff']
         cinv_yw = self.B @ ((self.B.T @ yw) / self.D)
@@ -179,13 +163,8 @@ class Worker:
 
     def __init__(self, id, state_normalizer, task_q, result_q, stop, config, device=None, kernels=None):
         self.id, self.config = id, config
-        if kernels is None:
-            self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
-            kernels = ops
-        else:
-            self.device = torch.device(device if device is not None else 'cpu')
-        self.kn = kernels
-        self.source = fitness.from_config(config, kernels, self.device)
+        self.kn, self.device = kernels_and_device(kernels, device)
+        self.source = fitness.from_config(config, self.kn, self.device)
         self.obs_stats, self.obs_totals = self.source.obs_stats, self.source.obs_totals
         self.tests_run = 0            # test() calls so far: the generation word of the next test episodes
 
@@ -196,7 +175,7 @@ class Worker:
 
     def steps_over_ranks(self, es):
         """Environment steps of the last run(), summed over ranks (cma_es.py:73 sums the episodes' real lengths)."""
-        return self.source.steps(es.lam, es.world, es.pg)
+        return self.source.steps(es.lam, es.group)
 
     def test_returns(self, solution, repetitions):
         """Returns of `repetitions` noiseless episodes of one solution (cma_es.py:102-111) with the current statistics.
@@ -207,7 +186,7 @@ class Worker:
 
     def merge_obs_stats(self, es):
         """cma_es.py:92-96: the statistics of this generation's observations, summed over ranks, merged into [m|v|n]."""
-        self.source.share_totals(es.world, es.pg)
+        self.source.share_totals(es.group)
         self.source.merge(es.lam)
 
 
@@ -217,8 +196,8 @@ def train(config, worker=None, es=None):
     if worker is None:
         worker = Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
     if es is None:
-        es = CMAEvolutionStrategy(config.initial_weight, config.sigma, config.pop_size, seed=getattr(config, 'seed', 0),
-                                  device=worker.device, kernels=None if worker.kn is ops else worker.kn)
+        es = CMAEvolutionStrategy(config.initial_weight, config.sigma, config.pop_size, seed=config.seed,
+                                  device=worker.device, kernels=worker.kn)
     total_steps = 0
     initial_time = time.time()
     training_rewards, training_steps, training_timestamps = [], [], []
@@ -255,14 +234,10 @@ def train(config, worker=None, es=None):
 
 
 def _fetch_member(es, solutions_local, index):
-    """Solution `index` of the global population on every rank (the owner contributes it, the others zeros)."""
-    if es.world == 1:
-        return solutions_local[index]
-    row = torch.zeros(es.n, dtype=torch.float32, device=es.device)
-    if es.offset <= index < es.offset + es.n_local:
-        row.copy_(solutions_local[index - es.offset])
-    dist.all_reduce(row, group=es.pg)
-    return row
+    """Solution `index` of the global population on every rank: a gather of one row, which its owner holds."""
+    i = index - es.offset
+    mine = solutions_local[i:i + 1] if 0 <= i < es.n_local else solutions_local[:0]
+    return es.group.gather(mine, 0, 1)[0]
 
 
 def test(config, solution, stats, worker=None):

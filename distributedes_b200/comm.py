@@ -24,11 +24,11 @@ class _DevArray:
 
 
 class PeerComm:
-    def __init__(self, N, P, device, process_group=None):
+    """The exchange among the ranks of `group` (an engine.RankGroup)."""
+
+    def __init__(self, N, P, device, group):
         self.lib = _lib.load()
-        self.pg = process_group
-        self.rank = dist.get_rank(process_group)
-        self.world = dist.get_world_size(process_group)
+        self.rank, self.world = group.rank, group.world
         self.device = torch.device(device)
         self.N, self.P = int(N), int(P)
         self._h = C.c_void_p()
@@ -37,13 +37,13 @@ class PeerComm:
             _lib.check(self.lib.des_comm_create(C.byref(self._h), self.rank, self.world, self.N, self.P, handle), 'des_comm_create')
             mine = torch.tensor(list(bytes(handle)), dtype=torch.uint8, device=self.device)
             every = [torch.empty_like(mine) for _ in range(self.world)]
-            dist.all_gather(every, mine, group=process_group)
+            dist.all_gather(every, mine, group=group.pg)
             blob = b''.join(bytes(t.cpu().numpy().tobytes()) for t in every)
             buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
             _lib.check(self.lib.des_comm_connect(self._h, buf), 'des_comm_connect')
             ptr = self.lib.des_comm_fitness_all_dev(self._h)
             self.fitness_all = torch.as_tensor(_DevArray(ptr, self.N, self), device=self.device)
-            dist.barrier(group=process_group)            # every block is mapped before anyone stores into a peer
+            dist.barrier(group=group.pg)                 # every block is mapped before anyone stores into a peer
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)

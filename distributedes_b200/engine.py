@@ -23,6 +23,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from . import ops
 from .fitness import DeviceRollouts, HostEpisodes, HostRollouts, Tape  # noqa: F401  (engine.HostEpisodes stays public)
 
 
@@ -35,41 +36,79 @@ def shard_bounds(N, world_size, rank):
     return start, base + (1 if rank < rem else 0)
 
 
-def _kernels_and_device(kernels, device):
-    if kernels is None:
-        from . import ops as kernels          # loads libdes_b200.so; raises if it is missing
-    return kernels, torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
+class RankGroup:
+    """This process among the ranks of `process_group`: its `world`, `rank` and `pg` (1, 0 and None when
+    torch.distributed is not initialised), its shard of a population and the two collectives the trainers issue."""
+
+    def __init__(self, process_group=None):
+        self.pg = process_group
+        distributed = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(process_group) if distributed else 1
+        self.rank = dist.get_rank(process_group) if distributed else 0
+
+    def shard(self, N, pairs=False):
+        """(offset, count) of this rank's members of N; with `pairs`, whole +-eps pairs (members 2p and 2p+1)."""
+        if pairs:
+            offset, n = shard_bounds(N // 2, self.world, self.rank)
+            return 2 * offset, 2 * n
+        return shard_bounds(N, self.world, self.rank)
+
+    def sum_(self, t):
+        """t summed over the ranks, in place; a single process has nothing to add."""
+        if self.world > 1:
+            dist.all_reduce(t, group=self.pg)
+        return t
+
+    def gather(self, part, offset, N, out=None):
+        """[N, ...] on every rank from each rank's `part`, its rows [offset, offset + len(part)): the sum over the ranks
+        of the zero-padded parts, which is an all-gather that allows ragged shards.  A single process returns `part` (or
+        `out`).  `out`, when given, is the [N, ...] result with `part` already its slice: the gather is then in place,
+        with no copy and no allocation."""
+        if self.world == 1:
+            return part if out is None else out
+        if out is None:
+            out = part.new_zeros((N,) + tuple(part.shape[1:]))
+            out[offset:offset + len(part)] = part
+        else:
+            out[:offset].zero_()
+            out[offset + len(part):].zero_()
+        dist.all_reduce(out, group=self.pg)
+        return out
+
+
+def kernels_and_device(kernels=None, device=None):
+    """The device ops and the device of a trainer: `kernels` None is distributedes_b200.ops (libdes_b200.so), `device`
+    None the current CUDA device.  The library has no CPU path, so it is refused a CPU device here, at construction."""
+    kernels = ops if kernels is None else kernels
+    device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if kernels is ops and device.type != 'cuda':
+        raise RuntimeError('distributedes_b200 needs a CUDA device, got %s: there is no CPU fallback' % device)
+    return kernels, device
 
 
 class NESEngine:
     """One rank's NES generation.  `obs`, `target`, `normalize_obs` and `repetitions` build the tape source unless a
-    `source` is given; the source's buffers (tape, eval workspace, statistics, host rows) read through the engine."""
+    `source` is given; the source's buffers (tape, eval workspace, statistics, host rows) and its precision read through
+    the engine."""
 
     def __init__(self, *, state_dim, hidden, action_dim, pop_size, theta0, obs=None, target=None, sigma, learning_rate,
                  weight_decay=0.005, clip=1.0, seed=0, precision='fp32', beta1=0.9, beta2=0.999, epsilon=1e-8,
                  device=None, process_group=None, kernels=None, use_graph=False, normalize_obs=False, repetitions=1,
                  mirrored=False, source=None):
-        self.k, self.device = _kernels_and_device(kernels, device)
-        self.pg = process_group
-        distributed = dist.is_available() and dist.is_initialized()
-        self.world = dist.get_world_size(process_group) if distributed else 1
-        self.rank = dist.get_rank(process_group) if distributed else 0
+        self.k, self.device = kernels_and_device(kernels, device)
+        self.group = RankGroup(process_group)
+        self.world, self.rank = self.group.world, self.group.rank
         self.d0, self.H, self.A = int(state_dim), int(hidden), int(action_dim)
         self.N = int(pop_size)
         if self.N < 2:
             raise ValueError('pop_size must be >= 2 (fitness_shift divides by N-1, utils.py:146)')
         # mirrored sampling: members 2p and 2p+1 are theta +- sigma*eps_p; a shard holds whole pairs
         self.mirrored = bool(mirrored)
-        if self.mirrored:
-            if self.N % 2:
-                raise ValueError('mirrored sampling needs an even pop_size (members come in +-eps pairs); got %d' % self.N)
-            pair_offset, pairs = shard_bounds(self.N // 2, self.world, self.rank)
-            self.offset, self.n_local = 2 * pair_offset, 2 * pairs
-        else:
-            self.offset, self.n_local = shard_bounds(self.N, self.world, self.rank)
+        if self.mirrored and self.N % 2:
+            raise ValueError('mirrored sampling needs an even pop_size (members come in +-eps pairs); got %d' % self.N)
+        self.offset, self.n_local = self.group.shard(self.N, pairs=self.mirrored)
         self.sigma, self.lr, self.wd, self.clip = float(sigma), float(learning_rate), float(weight_decay), float(clip)
         self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
-        self.precision = precision
         theta0 = np.ascontiguousarray(theta0, dtype=np.float32).reshape(-1)
         self.P = self.k.param_count(self.d0, self.H, self.A)
         if theta0.size != self.P:
@@ -85,14 +124,14 @@ class NESEngine:
         if self.world > 1 and self.k.__name__.endswith('.ops') and dev.type == 'cuda' and os.environ.get('DES_COMM', 'peer') != 'nccl':
             try:
                 from .comm import PeerComm
-                self.comm = PeerComm(self.N, self.P, dev, process_group)
+                self.comm = PeerComm(self.N, self.P, dev, self.group)
             except RuntimeError as e:
                 import warnings
                 warnings.warn('distributedes_b200: peer-memory exchange unavailable (%s); using NCCL all-reduces' % e)
                 self.comm = None
             # every rank must take the same path
             ok = torch.tensor([1 if self.comm is not None else 0], device=dev)
-            dist.all_reduce(ok, op=dist.ReduceOp.MIN, group=process_group)
+            dist.all_reduce(ok, op=dist.ReduceOp.MIN, group=self.group.pg)
             if int(ok.item()) == 0 and self.comm is not None:
                 self.comm.close()
                 self.comm = None
@@ -137,13 +176,11 @@ class NESEngine:
 
     # -- the three phases around the two collectives -------------------------------------------------------
     def evaluate(self):
-        if self.world > 1 and self.comm is None:
-            self.fitness_all.zero_()
         self.source.members(self.theta, state=self.state, generation=self.generation_index, offset=self.offset,
                             n_local=self.n_local, out=self.fitness_shard_out)
         self._gather_fitness()
-        self.source.share_totals(self.world, self.pg)
-        self.steps_taken = self.source.steps(self.N, self.world, self.pg)
+        self.source.share_totals(self.group)
+        self.steps_taken = self.source.steps(self.N, self.group)
         return self.fitness_all
 
     @property
@@ -152,23 +189,21 @@ class NESEngine:
         return self._fitness_xchg[self.offset:self.offset + self.n_local]
 
     def _gather_fitness(self):
-        if self.world > 1:
-            if self.comm is not None:
-                self.comm.allgather_fitness(self.offset, self.n_local)     # shard -> every peer's exchange block, flag barrier
-                self.fitness_all.copy_(self._fitness_xchg)                 # the stable private copy (a 4N-byte device copy)
-            else:
-                dist.all_reduce(self.fitness_all, group=self.pg)
+        if self.comm is not None:
+            self.comm.allgather_fitness(self.offset, self.n_local)     # shard -> every peer's exchange block, flag barrier
+            self.fitness_all.copy_(self._fitness_xchg)                 # the stable private copy (a 4N-byte device copy)
+        else:
+            self.group.gather(self.fitness_shard_out, self.offset, self.N, out=self.fitness_all)
 
     def rank_and_reduce(self):
         self.k.centered_rank(self.fitness_all, self.offset, self.n_local, workspace=self.rank_ws, out=self.shaped)
         grad = self.k.nes_grad_partial_mirrored if self.mirrored else self.k.nes_grad_partial
         grad(self.shaped, self.P, seed=self.seed, state=self.state, member_offset=self.offset, workspace=self.grad_ws,
              out=self.partial_local if self.comm is not None else self.partial)
-        if self.world > 1:
-            if self.comm is not None:
-                self.comm.allreduce_partial(self.partial_local, self.partial)   # slots over NVLink, summed in rank order
-            else:
-                dist.all_reduce(self.partial, group=self.pg)
+        if self.comm is not None:
+            self.comm.allreduce_partial(self.partial_local, self.partial)   # slots over NVLink, summed in rank order
+        else:
+            self.group.sum_(self.partial)
         return self.partial
 
     def apply(self):
@@ -259,17 +294,15 @@ class RolloutEngine(NESEngine):
     Environment: 'Pendulum-v0' (config.py:26-31).  Sharded with the normaliser on, the generation stays eager."""
 
     def __init__(self, *, task='Pendulum-v0', hidden, pop_size, theta0, sigma, learning_rate, repetitions=10,
-                 horizon=None, action_noise_std=0.0, normalize_obs=True, clip=None, seed=0, mirrored=False, **kw):
-        if not (1 <= int(repetitions) <= 10):
-            raise ValueError('RolloutEngine: repetitions must be in [1, 10] (one warp steps them in lockstep); got %r'
-                             % (repetitions,))
-        kw.pop('precision', None)
-        kw['kernels'], kw['device'] = _kernels_and_device(kw.get('kernels'), kw.get('device'))
-        src = DeviceRollouts(kw['kernels'], kw['device'], task=task, hidden=hidden, repetitions=repetitions,
-                             horizon=horizon, clip=clip, action_noise_std=action_noise_std, seed=seed,
-                             normalize_obs=normalize_obs, sigma=float(sigma), mirrored=mirrored)
+                 horizon=None, action_noise_std=0.0, normalize_obs=True, clip=None, seed=0, mirrored=False, kernels=None,
+                 device=None, **kw):
+        k, dev = kernels_and_device(kernels, device)
+        src = DeviceRollouts(k, dev, task=task, hidden=hidden, repetitions=repetitions, horizon=horizon, clip=clip,
+                             action_noise_std=action_noise_std, seed=seed, normalize_obs=normalize_obs, sigma=float(sigma),
+                             mirrored=mirrored)
         super().__init__(state_dim=src.d0, hidden=hidden, action_dim=src.A, pop_size=pop_size, theta0=theta0, sigma=sigma,
-                         learning_rate=learning_rate, clip=src.clip, mirrored=mirrored, source=src, **kw)
+                         learning_rate=learning_rate, clip=src.clip, mirrored=mirrored, source=src, kernels=k, device=dev,
+                         **kw)
 
 
 class HostEnvEngine(NESEngine):
@@ -278,22 +311,12 @@ class HostEnvEngine(NESEngine):
 
     def __init__(self, *, env_fn, hidden, pop_size, theta0, sigma, learning_rate, state_dim=None, action_dim=None,
                  repetitions=10, test_repetitions=None, action_noise_std=0.0, normalize_obs=True, batch_env_fn=None,
-                 clip=1.0, seed=0, mirrored=False, **kw):
-        if state_dim is None or action_dim is None:
-            probe = env_fn()
-            state_dim, action_dim = probe.observation_space.shape[0], probe.action_space.shape[0]
-        if not (1 <= int(state_dim) <= 32 and 1 <= int(action_dim) <= 8):
-            raise ValueError('HostEnvEngine: des_policy_act takes state_dim <= 32 and action_dim <= 8; got %r, %r'
-                             % (state_dim, action_dim))
-        for name, r in (('repetitions', repetitions), ('test_repetitions', test_repetitions or repetitions)):
-            if not (1 <= int(r) <= 16):
-                raise ValueError('HostEnvEngine: %s must be in [1, 16]; got %r' % (name, r))
-        kw.pop('precision', None)
-        kw.pop('use_graph', None)
-        kw['kernels'], kw['device'] = _kernels_and_device(kw.get('kernels'), kw.get('device'))
-        src = HostRollouts(kw['kernels'], kw['device'], env_fn=env_fn, batch_env_fn=batch_env_fn, state_dim=state_dim,
-                           action_dim=action_dim, hidden=hidden, repetitions=repetitions,
-                           test_repetitions=test_repetitions, clip=clip, action_noise_std=action_noise_std, seed=seed,
-                           normalize_obs=normalize_obs, sigma=float(sigma), mirrored=mirrored)
-        super().__init__(state_dim=state_dim, hidden=hidden, action_dim=action_dim, pop_size=pop_size, theta0=theta0,
-                         sigma=sigma, learning_rate=learning_rate, clip=clip, mirrored=mirrored, source=src, **kw)
+                 clip=1.0, seed=0, mirrored=False, kernels=None, device=None, **kw):
+        k, dev = kernels_and_device(kernels, device)
+        src = HostRollouts(k, dev, env_fn=env_fn, batch_env_fn=batch_env_fn, state_dim=state_dim, action_dim=action_dim,
+                           hidden=hidden, repetitions=repetitions, test_repetitions=test_repetitions, clip=clip,
+                           action_noise_std=action_noise_std, seed=seed, normalize_obs=normalize_obs, sigma=float(sigma),
+                           mirrored=mirrored)
+        super().__init__(state_dim=src.d0, hidden=hidden, action_dim=src.A, pop_size=pop_size, theta0=theta0, sigma=sigma,
+                         learning_rate=learning_rate, clip=clip, mirrored=mirrored, source=src, kernels=k, device=dev,
+                         **kw)

@@ -2,12 +2,12 @@
 episodes stepped on the host (HostRollouts).  engine.NESEngine and cma_es.Worker evaluate through one and never ask
 which.  A source evaluates NES members theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
 holds the normaliser statistics `obs_stats` [m | v | n] (or None) and the fp64 observation totals `obs_totals` of its
-last evaluation, shares and merges them, counts its environment steps and says whether a CUDA graph may capture it."""
+last evaluation, shares and merges them over an engine.RankGroup, counts its environment steps and says whether a CUDA
+graph may capture it.  from_config builds the source a config describes, for both trainers."""
 from __future__ import annotations
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 from .envs import TEST_MEMBER, DeviceEnv, GymEnvBatch
 
@@ -16,8 +16,9 @@ POLICY_WIDTHS = (16, 32, 64, 96, 128)     # hidden widths des_rollout_eval and d
 
 class Tape:
     """Fitness on the observation tape.  NES members go through des_nes_eval (after des_obs_normalize of the tape with
-    the statistics of the previous generations, when normalising); explicit rows through des_pop_eval, without a
-    normaliser.  Every member sees the whole tape, so the statistics merge needs no collective."""
+    the statistics of the previous generations, when normalising); explicit rows through des_pop_eval on the raw tape.
+    A tape without a `sigma` evaluates explicit rows only (CMA-ES), so it keeps no normaliser and no eval workspace.
+    Every member sees the whole tape, so the statistics merge needs no collective."""
 
     test_repetitions = 1          # the tape is deterministic
 
@@ -25,7 +26,7 @@ class Tape:
                  normalize_obs=False, sigma=None, seed=0, precision='fp32', mirrored=False):
         self.k, self.device = kernels, torch.device(device)
         self.d0, self.H, self.A, self.clip = int(state_dim), int(hidden), int(action_dim), float(clip)
-        self.repetitions, self.normalize_obs = int(repetitions), bool(normalize_obs)
+        self.repetitions, self.normalize_obs = int(repetitions), bool(normalize_obs) and sigma is not None
         self.sigma, self.seed, self.precision, self.mirrored = sigma, int(seed), precision, bool(mirrored)
         self.obs_stats = torch.zeros(2 * self.d0 + 1, dtype=torch.float32, device=self.device) if self.normalize_obs else None
         self.obs_totals = self.obs_raw = self.T = self.eval_ws = None
@@ -47,7 +48,7 @@ class Tape:
         self.target = target.to(self.device).contiguous()
         # what the kernels read: the raw tape, or its normalised image refreshed every generation
         self.obs = torch.empty_like(self.obs_raw) if self.normalize_obs else self.obs_raw
-        if int(obs.shape[0]) != self.T and hasattr(self.k, 'eval_workspace'):
+        if int(obs.shape[0]) != self.T and self.sigma is not None and hasattr(self.k, 'eval_workspace'):
             # a new tape length may be a multi-pass tensor-core shape: size its tile cache for the new T
             self.eval_ws = self.k.eval_workspace(self.d0, self.H, self.A, int(obs.shape[0]), self.precision, self.device)
         self.T = int(obs.shape[0])
@@ -63,7 +64,7 @@ class Tape:
                 workspace=self.eval_ws)
 
     def solutions(self, solutions, *, offset, generation, out=None):
-        return self.k.pop_eval(solutions, self.obs, self.target, hidden=self.H, clip=self.clip, out=out)
+        return self.k.pop_eval(solutions, self.obs_raw, self.target, hidden=self.H, clip=self.clip, out=out)
 
     def test_returns(self, solution, repetitions, generation, state=None):
         """`repetitions` evaluations of one solution, one launch each as the reference's test() loops run them: NES's
@@ -79,7 +80,7 @@ class Tape:
             out.append(float(f[0]))
         return np.asarray(out)
 
-    def share_totals(self, world, pg):
+    def share_totals(self, group):
         pass
 
     def merge(self, N):
@@ -87,7 +88,7 @@ class Tape:
             # natural_es.py:85-89: every member saw the whole tape, so every rank merges the same online statistics
             self.k.obs_stats_merge(self.obs_stats, self.obs_raw, N * self.T * self.repetitions)
 
-    def steps(self, N, world, pg):
+    def steps(self, N, group):
         return N * self.repetitions * self.T
 
     def capturable(self, world):
@@ -97,6 +98,8 @@ class Tape:
 class _Episodes:
     """The statistics of the states episodes visit: each rank sums its members' raw observations in fp64, and one
     (2*d0+1)-double all-reduce replaces the per-worker Chan merges of natural_es.py:85-89 / cma_es.py:92-96."""
+
+    precision = 'fp32'            # the device policy of des_rollout_eval and des_policy_act
 
     def __init__(self, kernels, device, *, state_dim, hidden, clip, action_noise_std, seed, repetitions, normalize_obs,
                  sigma, mirrored):
@@ -114,9 +117,9 @@ class _Episodes:
     def set_tape(self, obs, target):
         raise TypeError('%s steps its environments; there is no tape to set' % type(self).__name__)
 
-    def share_totals(self, world, pg):
-        if world > 1 and self.normalize_obs:
-            dist.all_reduce(self.obs_totals, group=pg)
+    def share_totals(self, group):
+        if self.normalize_obs:
+            group.sum_(self.obs_totals)
 
     def merge(self, N):
         if self.normalize_obs:
@@ -130,6 +133,9 @@ class DeviceRollouts(_Episodes):
     def __init__(self, kernels, device, *, task, hidden, repetitions, clip=None, horizon=None, **kw):
         if task not in DeviceEnv.SPECS:
             raise ValueError('closed-loop environments available on the device: %s (got %r)' % (sorted(DeviceEnv.SPECS), task))
+        if not (1 <= int(repetitions) <= 10):
+            raise ValueError('DeviceRollouts: repetitions must be in [1, 10] (one warp steps them in lockstep); got %r'
+                             % (repetitions,))
         spec = DeviceEnv.SPECS[task]
         super().__init__(kernels, device, state_dim=spec['state_dim'], hidden=hidden,
                          clip=spec['clip'] if clip is None else clip, repetitions=repetitions, **kw)
@@ -175,7 +181,7 @@ class DeviceRollouts(_Episodes):
                             obs_stats=self.obs_stats, episodes_out=episodes, **word, **self._env())
         return episodes.cpu().numpy().astype(np.float64)
 
-    def steps(self, N, world, pg):
+    def steps(self, N, group):
         return N * self.repetitions * self.horizon
 
     def capturable(self, world):
@@ -252,10 +258,19 @@ class HostRollouts(_Episodes):
     Evaluator.eval utils.py:116-124.  NES members become rows theta + sigma*eps once per generation (des_nes_perturb,
     natural_es.py:28-30).  The step count is the episodes' real length, summed over ranks (natural_es.py:75,
     cma_es.py:73).  batch_env_fn(num_slots) builds a batch environment (envs.py); the default wraps env_fn in
-    envs.GymEnvBatch."""
+    envs.GymEnvBatch.  env_fn is probed for the dimensions when they are not given."""
 
-    def __init__(self, kernels, device, *, env_fn, state_dim, action_dim, hidden, repetitions, test_repetitions=None,
-                 batch_env_fn=None, **kw):
+    def __init__(self, kernels, device, *, env_fn, hidden, repetitions, state_dim=None, action_dim=None,
+                 test_repetitions=None, batch_env_fn=None, **kw):
+        if state_dim is None or action_dim is None:
+            probe = env_fn()
+            state_dim, action_dim = probe.observation_space.shape[0], probe.action_space.shape[0]
+        if not (1 <= int(state_dim) <= 32 and 1 <= int(action_dim) <= 8):
+            raise ValueError('HostRollouts: des_policy_act takes state_dim <= 32 and action_dim <= 8; got %r, %r'
+                             % (state_dim, action_dim))
+        for name, r in (('repetitions', repetitions), ('test_repetitions', test_repetitions or repetitions)):
+            if not (1 <= int(r) <= 16):
+                raise ValueError('HostRollouts: %s must be in [1, 16]; got %r' % (name, r))
         super().__init__(kernels, device, state_dim=state_dim, hidden=hidden, repetitions=repetitions, **kw)
         self.A, self.test_repetitions = int(action_dim), int(test_repetitions or repetitions)
         if batch_env_fn is None:
@@ -312,26 +327,25 @@ class HostRollouts(_Episodes):
                                                        obs_stats=self.obs_stats)
         return ret[0]
 
-    def steps(self, N, world, pg):
-        total = torch.tensor([self.last_steps], dtype=torch.int64, device=self.device)
-        if world > 1:
-            dist.all_reduce(total, group=pg)
-        return int(total.item())
+    def steps(self, N, group):
+        return int(group.sum_(torch.tensor([self.last_steps], dtype=torch.int64, device=self.device)).item())
 
     def capturable(self, world):
         return False
 
 
-def from_config(config, kernels, device):
-    """The source a config describes: `host_env` configs step on the host, `closed_loop` ones on the device, the rest
-    read the tape of config.env_fn() (CMA-ES: without a normaliser)."""
-    kw = dict(hidden=config.hidden_size, clip=config.clip, seed=getattr(config, 'seed', 0), repetitions=config.repetitions)
-    episodes = dict(action_noise_std=config.action_noise_std, normalize_obs=getattr(config, 'normalize_obs', True),
-                    sigma=None, mirrored=False)
+def from_config(config, kernels, device, *, sigma=None, mirrored=False):
+    """The source a config describes, for either trainer: `host_env` configs step on the host, `closed_loop` ones on the
+    device, the rest read the tape of config.env_fn().  `sigma` and `mirrored` are NES's sampling of members; without a
+    sigma the source evaluates explicit rows (CMA-ES)."""
+    kw = dict(hidden=config.hidden_size, clip=config.clip, seed=config.seed, repetitions=config.repetitions,
+              normalize_obs=config.normalize_obs, sigma=sigma, mirrored=mirrored)
     if getattr(config, 'host_env', False):
         return HostRollouts(kernels, device, env_fn=config.env_fn, batch_env_fn=getattr(config, 'batch_env_fn', None),
-                            state_dim=config.state_dim, action_dim=config.action_dim, **episodes, **kw)
+                            state_dim=config.state_dim, action_dim=config.action_dim,
+                            test_repetitions=config.test_repetitions, action_noise_std=config.action_noise_std, **kw)
     if getattr(config, 'closed_loop', False):
-        return DeviceRollouts(kernels, device, task=config.task, **episodes, **kw)
+        return DeviceRollouts(kernels, device, task=config.task, action_noise_std=config.action_noise_std, **kw)
     env = config.env_fn()
-    return Tape(kernels, device, env.obs, env.target, state_dim=env.obs.shape[1], action_dim=env.target.shape[1], **kw)
+    return Tape(kernels, device, env.obs, env.target, state_dim=env.obs.shape[1], action_dim=env.target.shape[1],
+                precision=config.precision, **kw)

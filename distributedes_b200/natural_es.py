@@ -17,7 +17,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .engine import HostEnvEngine, NESEngine, RolloutEngine
+from .engine import NESEngine, kernels_and_device
+from .fitness import from_config
 from .utils import Evaluator, SharedStats, StaticNormalizer, logger
 
 
@@ -40,34 +41,16 @@ class Worker:
         return e.fitness_all[e.offset:e.offset + e.n_local]
 
 
-def build_engine(config, param=None, **kw):
-    theta0 = config.initial_weight if param is None else np.asarray(param, dtype=np.float32)
-    if getattr(config, 'host_env', False):            # environments stepped on the host, policy step on the device
-        return HostEnvEngine(env_fn=config.env_fn, batch_env_fn=getattr(config, 'batch_env_fn', None),
-                             state_dim=config.state_dim, action_dim=config.action_dim, hidden=config.hidden_size,
-                             pop_size=config.pop_size, theta0=theta0, sigma=config.sigma,
-                             learning_rate=config.learning_rate, weight_decay=config.weight_decay, clip=config.clip,
-                             seed=getattr(config, 'seed', 0), beta1=config.opt.beta1, beta2=config.opt.beta2,
-                             epsilon=config.opt.epsilon, repetitions=config.repetitions,
-                             test_repetitions=config.test_repetitions, action_noise_std=config.action_noise_std,
-                             normalize_obs=getattr(config, 'normalize_obs', True),
-                             mirrored=getattr(config, 'mirrored', False), **kw)
-    env = config.env_fn()
-    if getattr(config, 'closed_loop', False):         # environment stepped on the device (SURVEY 8f row 3)
-        return RolloutEngine(task=config.task, hidden=config.hidden_size, pop_size=config.pop_size, theta0=theta0,
-                             sigma=config.sigma, learning_rate=config.learning_rate, weight_decay=config.weight_decay,
-                             clip=config.clip, seed=getattr(config, 'seed', 0), beta1=config.opt.beta1,
-                             beta2=config.opt.beta2, epsilon=config.opt.epsilon, repetitions=config.repetitions,
-                             action_noise_std=config.action_noise_std,
-                             normalize_obs=getattr(config, 'normalize_obs', True),
-                             mirrored=getattr(config, 'mirrored', False), **kw)
-    return NESEngine(state_dim=config.state_dim, hidden=config.hidden_size, action_dim=config.action_dim,
-                     pop_size=config.pop_size, theta0=theta0, obs=env.obs, target=env.target, sigma=config.sigma,
-                     learning_rate=config.learning_rate, weight_decay=config.weight_decay, clip=config.clip,
-                     seed=getattr(config, 'seed', 0), precision=getattr(config, 'precision', 'fp32'),
-                     beta1=config.opt.beta1, beta2=config.opt.beta2, epsilon=config.opt.epsilon,
-                     normalize_obs=getattr(config, 'normalize_obs', False), repetitions=config.repetitions,
-                     mirrored=getattr(config, 'mirrored', False), **kw)
+def build_engine(config, param=None, *, kernels=None, device=None, **kw):
+    """The NESEngine of a config: its fitness source (fitness.from_config) and its optimiser settings.  `kw` goes to
+    NESEngine (process_group, use_graph)."""
+    k, dev = kernels_and_device(kernels, device)
+    src = from_config(config, k, dev, sigma=float(config.sigma), mirrored=config.mirrored)
+    return NESEngine(state_dim=src.d0, hidden=src.H, action_dim=src.A, pop_size=config.pop_size,
+                     theta0=config.initial_weight if param is None else np.asarray(param, dtype=np.float32),
+                     sigma=config.sigma, learning_rate=config.learning_rate, weight_decay=config.weight_decay,
+                     clip=config.clip, beta1=config.opt.beta1, beta2=config.opt.beta2, epsilon=config.opt.epsilon,
+                     mirrored=config.mirrored, source=src, kernels=k, device=dev, **kw)
 
 
 def train(config, engine=None):

@@ -1,7 +1,8 @@
 """The host logic around the kernels, pinned without a GPU: which device ops every NES and CMA-ES mode launches per
 generation, in which order and with which arguments, and which collectives it issues on tensors of which size — one
 process and each rank of a 2-rank gloo run.  The kernels are the oracle-backed CPU stand-ins (cpu_ops.py) behind a
-recording proxy.  Also: CMA-ES on a host-stepped environment sharded over 2 and 3 gloo ranks against the
+recording proxy.  The NES modes a config can describe are pinned a second time through natural_es.build_engine, to the
+same records.  Also: the limits each source checks for CMA-ES, and CMA-ES on a host-stepped environment sharded over 2 and 3 gloo ranks against the
 single-process run."""
 import hashlib
 import inspect
@@ -117,6 +118,24 @@ def _nes(mode, kernels):
                          clip=2.0, **common), Cfg(repetitions=2, test_repetitions=3)
 
 
+def _nes_config(mode):
+    """The config natural_es.build_engine turns into the engine of _nes(mode), for the tape and host-stepped modes (a
+    config cannot set the device modes' 12-step horizon)."""
+    from distributedes_b200.config import HostEnvConfig, SynthTapeConfig
+    if mode.startswith('tape'):         # SynthTapeConfig's tape is orc.synthetic_tape's
+        cfg = SynthTapeConfig(hidden_size=8, state_dim=3, action_dim=2, tape_len=5, clip=1.5)
+        cfg.initial_weight = orc.synthetic_theta(3, 8, 2)
+        cfg.normalize_obs = mode == 'tape_norm'
+        cfg.repetitions, cfg.test_repetitions = (2 if cfg.normalize_obs else 1), 2
+    else:
+        cfg = HostEnvConfig(hs.PendulumProbe, hidden_size=16, clip=2.0,
+                            batch_env_fn=lambda B: hs.PendulumBatch(B, 7, horizon=9))
+        cfg.initial_weight = orc.synthetic_theta(3, 16, 1, seed=3)
+        cfg.repetitions, cfg.test_repetitions = 2, 3
+    cfg.pop_size, cfg.seed, cfg.max_generations, cfg.mirrored = 6, 7, 1, mode.endswith('mirrored')
+    return cfg
+
+
 def _cma_config(mode, seed=7):
     from distributedes_b200.config import ClosedLoopPendulumConfig, HostEnvConfig, SynthTapeConfig
     from distributedes_b200.envs import GymEnvBatch
@@ -138,11 +157,16 @@ def _cma_config(mode, seed=7):
     return cfg
 
 
-def _run_nes(mode):
-    """natural_es.train over one generation (test, evaluate, rank, gradient, apply; then test and evaluate again)."""
+def _run_nes(mode, from_config=False):
+    """natural_es.train over one generation (test, evaluate, rank, gradient, apply; then test and evaluate again), on the
+    engine of _nes(mode) or on the one natural_es.build_engine makes of _nes_config(mode)."""
     from distributedes_b200 import natural_es
     rec = record()
-    eng, cfg = _nes(mode, rec.kernels)
+    if from_config:
+        cfg = _nes_config(mode)
+        eng = natural_es.build_engine(cfg, device='cpu', kernels=rec.kernels)
+    else:
+        eng, cfg = _nes(mode, rec.kernels)
     with rec:
         natural_es.train(cfg, engine=eng)
     return rec.trace()
@@ -170,11 +194,13 @@ def _trace_cma(mode):
 
 
 def _traces():
-    return {('nes', m): _run_nes(m) for m in NES_MODES} | {('cma', m): _trace_cma(m) for m in CMA_MODES}
+    return ({('nes', m): _run_nes(m) for m in NES_MODES} | {('cma', m): _trace_cma(m) for m in CMA_MODES}
+            | {('nes_config', m): _run_nes(m, from_config=True) for m in NES_CONFIG_MODES})
 
 
 NES_MODES = ('tape', 'tape_mirrored', 'tape_norm', 'device', 'device_mirrored', 'host', 'host_mirrored')
 CMA_MODES = ('tape', 'device', 'host')
+NES_CONFIG_MODES = ('tape', 'tape_mirrored', 'tape_norm', 'host', 'host_mirrored')     # built through build_engine
 
 
 # per mode, recorded from the host layer as it was before the fitness sources (fitness.py) took over the evaluation:
@@ -296,16 +322,32 @@ EXPECTED = {('cma', 'device'): (('rollout_eval noise_fill rollout_eval_solutions
                                     'a802077aaf99a0ce'))}
 
 
+def _expected():
+    """EXPECTED, and each NES mode built from a config expects the row of the engine built directly."""
+    return list(EXPECTED.items()) + [(('nes_config', m), EXPECTED[('nes', m)]) for m in NES_CONFIG_MODES]
+
+
 def test_every_mode_issues_the_pinned_ops_and_collectives_in_one_process():
     got = _traces()
-    for key, (one, _, _) in EXPECTED.items():
+    for key, (one, _, _) in _expected():
         assert got[key] == one, key
 
 
 def test_every_mode_issues_the_pinned_ops_and_collectives_on_each_of_two_gloo_ranks():
     r = spawn(2, _traces)
-    for key, (_, r0, r1) in EXPECTED.items():
+    for key, (_, r0, r1) in _expected():
         assert (r[0][key], r[1][key]) == (r0, r1), key
+
+
+@pytest.mark.parametrize('mode,attr,value', [('device', 'repetitions', 11), ('host', 'repetitions', 17),
+                                             ('host', 'test_repetitions', 17), ('host', 'state_dim', 33)])
+def test_a_cma_worker_is_refused_a_config_its_source_cannot_run(mode, attr, value):
+    """Each source checks its own limits when it is built, so CMA-ES meets them when its Worker is made."""
+    from distributedes_b200 import cma_es
+    cfg = _cma_config(mode)
+    setattr(cfg, attr, value)
+    with pytest.raises(ValueError, match=attr):
+        cma_es.Worker(0, None, None, None, None, cfg, device='cpu', kernels=cpu_ops)
 
 
 def _walk_cma():
