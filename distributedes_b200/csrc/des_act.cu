@@ -12,8 +12,8 @@
 //            R = H/16, pk = 0..H-1
 //   a[c]   = pairwise sum over the 16 unit groups g of (fma chain over r < R of W3[c][gR + r] h2[gR + r]), + b3[c]
 //   a[c]  += std * z, z = normal (c % 4) of the quad Philox(t + (c/4)*2^31, member*16 + rep, generation, stream 3)
-//   a[c]   = fminf(fmaxf(a[c], -clip), clip)
-// tanh is tanh_mufu (des_common.cuh).
+//   a[c]   = clip_keep_nan(a[c], clip): np.clip, so a NaN observation or NaN weights give a NaN action
+// tanh is tanh_mufu (des_common.cuh).  Dead slots get 0 whatever their observation holds.
 //
 // One CTA (128 threads) per member: the member's row is staged once per launch into shared memory (coalesced scalar
 // loads: P is odd, rows are not 16-byte aligned), then thread (j, g) computes hidden unit j for the episode block g.
@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(kActThreads) policy_act_kernel(ActArgs a) {
             const float zc = cc == 0 ? z.x : cc == 1 ? z.y : cc == 2 ? z.z : z.w;
             act = __fmaf_rn(zc, a.act_noise, act);
         }
-        act = fminf(fmaxf(act, -a.clip), a.clip);                            // utils.py:134
+        act = clip_keep_nan(act, a.clip);                                    // np.clip, utils.py:134
         a.actions[(i * a.reps + r) * A + c] = alive[r] ? act : 0.f;
     }
 }

@@ -124,6 +124,8 @@ __device__ __forceinline__ float clip_keep_nan(float v, float c) {
     asm("min.NaN.f32 %0, %0, %1;" : "+f"(y) : "f"(c));
     return y;
 }
+// fp64 form (the device Pendulum's dynamics): PTX has no max.NaN.f64, so NaN is tested for explicitly
+__device__ __forceinline__ double clip_keep_nan(double v, double c) { return isnan(v) ? v : fmin(fmax(v, -c), c); }
 __device__ __forceinline__ float sqrt_approx(float x) {
     float y;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

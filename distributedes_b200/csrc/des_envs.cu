@@ -52,14 +52,14 @@ struct Pendulum {
         o[2] = (float)thdot;
     }
     __device__ double step(double u) {                                  // returns the reward; observe() came first
-        u = fmin(fmax(u, -2.0), 2.0);
+        u = clip_keep_nan(u, 2.0);                                       // np.clip: a NaN action makes a NaN state
         const double two_pi = 6.283185307179586, pi = 3.141592653589793;
         const double x = th + pi;
         const double an = (x - two_pi * floor(x * (1.0 / two_pi))) - pi;  // ((th + pi) % 2 pi) - pi, python sign rule
         const double cost = an * an + 0.1 * thdot * thdot + 0.001 * u * u;
         const double nthdot = thdot + (15.0 * sn + 3.0 * u) * 0.05;      // -3g/(2l) sin(th + pi) + 3/(m l^2) u
         th = th + nthdot * 0.05;
-        thdot = fmin(fmax(nthdot, -8.0), 8.0);
+        thdot = clip_keep_nan(nthdot, 8.0);
         return -cost;
     }
 };
@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
             box_muller(xr.x, xr.y, z0, z1);
             act = __fmaf_rn(z0, a.act_noise, act);
         }
-        act = fminf(fmaxf(act, -a.clip), a.clip);                        // config.action_clip, utils.py:134
+        act = clip_keep_nan(act, a.clip);                                // config.action_clip, utils.py:134
         total += env.step((double)act);                                  // utils.py:135-137
     }
     if (writer) {

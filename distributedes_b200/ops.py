@@ -264,7 +264,9 @@ def nes_eval(theta, obs, target, *, hidden, sigma, clip, seed, generation=0, sta
     """Fused sample+forward+fitness for members [member_offset, member_offset+n_local) -> fitness[n_local].
 
     precision 'f16' / 'f16x3' run the hidden layers on tensor cores with fp16 operands: |obs| and |theta'| must stay
-    below 65520, or they overflow to inf.  A NaN action gives a NaN fitness on every path (np.clip keeps NaN)."""
+    below 65520, or they overflow to inf.  A NaN action gives a NaN fitness on every path (np.clip keeps NaN): this
+    tape, the closed-loop rollouts (whose Pendulum clamps the torque and the speed without dropping NaN either) and
+    policy_act, which hands a host environment the NaN."""
     return _nes_eval('des_nes_eval', theta, obs, target, hidden, sigma, clip, seed, generation, state, member_offset,
                      n_local, precision, out, workspace)
 

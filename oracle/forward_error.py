@@ -22,6 +22,16 @@ The bound is a plain triangle-inequality bound: errors are never assumed to canc
 sits far below it (the tests state the measured ratio beside every assert).  A tanh input error E is carried
 through the largest |tanh'| on [|z| - E, |z| + E].
 
+``closed_loop_bound`` is the same bound for the closed-loop policy of rollout_pendulum_kernel (csrc/des_envs.cu) and
+policy_act_kernel (csrc/des_act.cu), precision 'mufu':
+
+  normaliser         x = (o - m) / sqrtf(v + 1e-6f) in fp32: 4 * 2^-24 |x| (subtract, add, sqrtf, divide)
+  layers 1 and 2     FFMA chains that start from the bias: K * 2^-24 * (|b| + sum|terms|)
+  tanh               tanh_mufu, 1 - 2/(1 + ex2(x * 2 log2 e)): 5 * 2^-23 absolute (ex2.approx, the add, rcp.approx,
+                     the final FFMA) plus the 2^-23 relative rounding of its argument
+  layer 3            per unit group an FFMA chain over R = H/16 units, then a 4-level butterfly over the 16 groups:
+                     every term passes through R + 4 roundings; then the add of b3 and the FFMA of the action noise
+
 ``forward_emulated`` rounds the operands exactly as the kernel does (numpy fp16, hi/lo split) and does everything
 else in fp64: its distance from the fp64 forward is the operand-rounding part of the kernel error.
 """
@@ -119,6 +129,70 @@ def forward_error_bound(flat, obs, d0, H, A, precision, dtheta=0.0):
     h2, Eh2 = _tanh(z2, Ez2, b2, precision)
     a, Ea = _dense(h2, Eh2, W3, E3, b3, Eb3, H, 'fp32', False)       # layer 3: fp32 FFMA in every precision
     return Ea
+
+
+TANH_MUFU_ABS = 5 * 2.0 ** -23      # tanh_mufu (des_common.cuh) at an exact fp32 argument; ~2e-7 in practice
+NORM_REL = 4 * U_F32                # the fp32 normaliser (o - m) / sqrtf(v + 1e-6f)
+NORM_EPS = float(np.float32(1e-6))
+
+
+def normalised(obs, stats=None):
+    """fp64 (o - m) / sqrt(v + 1e-6f) of raw observations obs[..., d0] with fp32 stats (m, v, n); o itself when stats
+    is None or n == 0 (StaticNormalizer, utils.py:48-51)."""
+    o = np.asarray(obs, dtype=np.float64)
+    if stats is None or float(stats[2]) == 0.0:
+        return o
+    m = np.asarray(stats[0], np.float32).astype(np.float64)
+    v = np.asarray(stats[1], np.float32).astype(np.float64)
+    return (o - m) / np.sqrt(v + NORM_EPS)
+
+
+def _chain(v, Ev, W, b, K):
+    """z = v W^T + b by an fp32 FFMA chain of K terms starting from b, inputs off by <= Ev: (z, bound)."""
+    mm = lambda x, y: np.einsum('...tk,...nk->...tn', x, y)
+    aW = np.abs(W)
+    z = mm(v, W) + b[..., None, :]
+    err = mm(Ev, aW)
+    return z, err + K * U_F32 * (np.abs(b)[..., None, :] + mm(np.abs(v) + Ev, aW)) * (1 + 2 * K * U_F32)
+
+
+def _tanh_mufu(z, Ez):
+    lo = np.maximum(np.abs(z) - Ez, 0.0)
+    slope = 1.0 - np.tanh(lo) ** 2
+    return np.tanh(z), slope * (Ez + 2.0 ** -23 * (np.abs(z) + Ez)) + TANH_MUFU_ABS
+
+
+def closed_loop_bound(flat, obs, d0, H, A, stats=None, noise=0.0, noise_err=0.0):
+    """Per-action bound B[..., T, A] on |a_kernel - a*| for the closed-loop policy (precision 'mufu', see above), a* the
+    fp64 forward of flat[..., P] at normalised(obs[T, d0], stats), plus `noise` (the std * z the kernel adds, [..., T, A]
+    or scalar).  noise_err bounds |kernel's std * z - noise| (its MUFU Box-Muller and the fp32 std)."""
+    flat = np.asarray(flat, dtype=np.float64)
+    W1, b1, W2, b2, W3, b3 = orc.unflatten(flat, d0, H, A)
+    x = normalised(obs, stats)
+    Ex = NORM_REL * np.abs(x) if (stats is not None and float(stats[2]) != 0.0) else np.zeros_like(x)
+    z1, Ez1 = _chain(x, Ex, W1, b1, d0)
+    h1, Eh1 = _tanh_mufu(z1, Ez1)
+    z2, Ez2 = _chain(h1, Eh1, W2, b2, H)
+    h2, Eh2 = _tanh_mufu(z2, Ez2)
+    mm = lambda u, w: np.einsum('...tk,...nk->...tn', u, w)
+    aW3 = np.abs(W3)
+    terms = mm(np.abs(h2) + Eh2, aW3)
+    a = mm(h2, W3)
+    Ea = mm(Eh2, aW3) + (H // 16 + 4) * U_F32 * terms * (1 + 64 * U_F32)
+    mag = terms + np.abs(b3)[..., None, :]
+    Ea = Ea + U_F32 * mag + U_F32 * (mag + np.abs(noise)) + np.asarray(noise_err, dtype=np.float64)   # + b3, + std*z
+    return Ea * (1 + 4 * U_F32)
+
+
+def closed_loop_actions(flat, obs, d0, H, A, stats=None, noise=0.0, tanh=np.tanh):
+    """a* [..., T, A]: the fp64 forward of flat[..., P] at normalised(obs, stats), plus noise (unclipped).  `tanh`
+    replaces the activation (sensitivity checks with a deliberately wrong one)."""
+    W1, b1, W2, b2, W3, b3 = (w.astype(np.float64) for w in orc.unflatten(np.asarray(flat), d0, H, A))
+    x = normalised(obs, stats)
+    mm = lambda u, w: np.einsum('...tk,...nk->...tn', u, w)
+    h1 = tanh(mm(x, W1) + b1[..., None, :])
+    h2 = tanh(mm(h1, W2) + b2[..., None, :])
+    return mm(h2, W3) + b3[..., None, :] + noise
 
 
 def _f16(x):

@@ -54,11 +54,14 @@ def pendulum_step(th, thdot, u):
     return nth, nthdot, -cost
 
 
-def rollouts(flat, H, seed, gen, members, reps, stats=None, horizon=HORIZON, clip=2.0, act_noise=0.0):
+def rollouts(flat, H, seed, gen, members, reps, stats=None, horizon=HORIZON, clip=2.0, act_noise=0.0, tanh=np.tanh,
+             trace=False):
     """Episodes of the policies flat[n, P] (already perturbed), `reps` each.
 
     stats: None or (m[3], v[3], n) — StaticNormalizer offline stats (identity while n == 0).
-    Returns (returns[n, reps] fp64, obs_sum[3], obs_sumsq[3], count) over the RAW observations seen."""
+    Returns (returns[n, reps] fp64, obs_sum[3], obs_sumsq[3], count) over the RAW observations seen; with trace, also
+    (obs[n, reps, horizon, 3] fp32, u[n, reps, horizon] the torque applied after the environment's clamp).
+    tanh replaces the activation (sensitivity checks with a deliberately wrong one)."""
     flat = np.asarray(flat, dtype=np.float32)
     n = flat.shape[0]
     W1, b1, W2, b2, W3, b3 = [w.astype(np.float64) for w in orc.unflatten(flat, D0, H, A)]
@@ -70,6 +73,7 @@ def rollouts(flat, H, seed, gen, members, reps, stats=None, horizon=HORIZON, cli
         m32 = np.asarray(stats[0], np.float32)
         s32 = np.sqrt(np.asarray(stats[1], np.float32) + np.float32(1e-6)).astype(np.float32)
     members = np.asarray(members, dtype=np.uint64).reshape(-1)
+    obs_tr, u_tr = [], []
     for t in range(horizon):
         o = pendulum_obs(th, thdot).astype(np.float32)                  # FloatTensor cast, utils.py:42-44 / model.py:35
         osum += o.astype(np.float64).sum((0, 1))
@@ -77,8 +81,8 @@ def rollouts(flat, H, seed, gen, members, reps, stats=None, horizon=HORIZON, cli
         cnt += n * reps
         x = ((o - m32) / s32).astype(np.float32) if use else o
         x = x.astype(np.float64)
-        h1 = np.tanh(np.einsum('nhk,nrk->nrh', W1, x) + b1[:, None, :])
-        h2 = np.tanh(np.einsum('nhk,nrk->nrh', W2, h1) + b2[:, None, :])
+        h1 = tanh(np.einsum('nhk,nrk->nrh', W1, x) + b1[:, None, :])
+        h2 = tanh(np.einsum('nhk,nrk->nrh', W2, h1) + b2[:, None, :])
         act = (np.einsum('nak,nrk->nra', W3, h2) + b3[:, None, :])[..., 0]
         if act_noise:
             k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64((seed >> 32) & 0xFFFFFFFF)
@@ -88,8 +92,13 @@ def rollouts(flat, H, seed, gen, members, reps, stats=None, horizon=HORIZON, cli
             z0, _ = orc.box_muller(x0, x1)
             act = act + z0 * act_noise
         act = np.clip(act.astype(np.float32).astype(np.float64), -clip, clip)
+        if trace:
+            obs_tr.append(o)
+            u_tr.append(np.clip(act, -2.0, 2.0))
         th, thdot, r = pendulum_step(th, thdot, act)
         total += r
+    if trace:
+        return total, osum, osq, cnt, (np.stack(obs_tr, axis=2), np.stack(u_tr, axis=2))
     return total, osum, osq, cnt
 
 
