@@ -65,9 +65,5 @@ def nes_generation(theta32, opt, obs, target, *, sigma, clip, seed, gen, N, d0, 
 
 
 def closed_fitness(theta, H, sigma, seed, gen, member_offset, n, reps, stats=None, horizon=po.HORIZON, clip=2.0):
-    """pendulum_oracle.closed_fitness over the mirrored members (what des_rollout_eval_mirrored writes): episodes keyed by
-    the global member index."""
-    flat = orc.perturb(theta, sigma, noise_mirrored(seed, gen, member_offset, n, orc.param_count(po.D0, H, po.A)))
-    ret, osum, osq, cnt = po.rollouts(flat, H, seed, gen, np.arange(member_offset, member_offset + n), reps, stats, horizon,
-                                      clip)
-    return ret.mean(1), (osum, osq, cnt)
+    """pendulum_oracle.closed_fitness over the mirrored rows (what des_rollout_eval_mirrored writes)."""
+    return po.closed_fitness(theta, H, sigma, seed, gen, member_offset, n, reps, stats, horizon, clip, noise_mirrored)

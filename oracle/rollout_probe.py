@@ -20,7 +20,6 @@ rounding of the three observations it reads: (ulp(thdot') + ulp(thdot)) / 2 / 0.
 """
 import numpy as np
 
-from . import nes_oracle as orc
 from . import pendulum_oracle as po
 
 EPISODES = 10                     # episodes the kernel steps per member, whatever the repetitions
@@ -103,13 +102,10 @@ def predict_tolerance(obs, u_err=0.0):
 
 
 def action_normals(seed, gen, member, T):
-    """The action-noise normals of `member`'s episodes, steps 0..T-1: (z0, z1) [EPISODES, T] from
-    Philox(t, member*16 + episode, gen, 3) (utils.py:133; the kernel adds z0)."""
-    ep = (np.uint64(member) * np.uint64(16) + np.arange(EPISODES, dtype=np.uint64)).reshape(-1, 1)
-    t = np.arange(T, dtype=np.uint64).reshape(1, -1)
-    x0, x1, _, _ = orc.philox4x32(t + 0 * ep, ep + 0 * t, np.uint64(gen & 0xFFFFFFFF), np.uint64(po.STREAM_ACT_NOISE),
-                                  seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
-    return orc.box_muller(x0, x1)
+    """The action-noise normals of `member`'s episodes, steps 0..T-1: (z0, z1) [EPISODES, T], the first two of
+    pendulum_oracle.action_noise (utils.py:133; the kernel adds z0)."""
+    z = np.stack([po.action_noise(seed, gen, [member], EPISODES, t, 2)[0] for t in range(T)], axis=1)
+    return z[..., 0], z[..., 1]
 
 
 def normal_error(z0, z1):

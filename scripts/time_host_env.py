@@ -41,24 +41,6 @@ class NoopEnv:
         return np.zeros((self.num_envs, self.d0)), np.zeros(self.num_envs), np.full(self.num_envs, self.t >= self.length)
 
 
-class PendulumBatch:
-    def __init__(self, B, seed):
-        self.num_envs, self.seed = B, seed
-
-    def reset(self, keys):
-        k = np.asarray(keys).astype(np.uint64)
-        x0, x1, _, _ = orc.philox4x32(k[:, 2], k[:, 1], k[:, 0], np.uint64(2), self.seed, 0)
-        u0 = ((x0 & np.uint32(0x7FFFFF)).astype(np.float64) + 0.5) / 8388608.0
-        u1 = ((x1 & np.uint32(0x7FFFFF)).astype(np.float64) + 0.5) / 8388608.0
-        self.th, self.thd, self.t = (2 * u0 - 1) * np.pi, 2 * u1 - 1, 0
-        return po.pendulum_obs(self.th, self.thd)
-
-    def step(self, actions, alive):
-        self.th, self.thd, r = po.pendulum_step(self.th, self.thd, actions[:, 0].astype(np.float64))
-        self.t += 1
-        return po.pendulum_obs(self.th, self.thd), r, np.full(self.num_envs, self.t >= 200)
-
-
 def card():
     name = torch.cuda.get_device_name(0)
     try:
@@ -112,7 +94,7 @@ def time_pendulum(N, H=64, reps=10):
     theta = torch.from_numpy(orc.synthetic_theta(3, H, 1)).cuda()
     stats = torch.cat([torch.zeros(3), torch.ones(3), torch.tensor([100.0])]).cuda()
     rows = torch.empty(N, orc.param_count(3, H, 1), device='cuda')
-    ep = HostEpisodes(ops, 'cuda', PendulumBatch(N * reps, 3), N, reps, 3, H, 1, 2.0, 0.0, 3)
+    ep = HostEpisodes(ops, 'cuda', po.PendulumBatch(N * reps, 3), N, reps, 3, H, 1, 2.0, 0.0, 3)
     part = torch.zeros(N, 7, dtype=torch.float64, device='cuda')
     res = {}
     for name in ('host', 'device'):

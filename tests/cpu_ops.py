@@ -6,7 +6,6 @@ without it the tape evaluation allocates no workspace."""
 import numpy as np
 import torch
 
-from host_env_support import accumulate_stats, policy_actions
 from oracle import cma_oracle as cma
 from oracle import mirrored_oracle as mo
 from oracle import nes_oracle as orc
@@ -202,9 +201,9 @@ def policy_act(rows, obs, alive, *, state_dim, hidden, action_dim, repetitions, 
     o = obs.numpy().reshape(n, reps, d0)
     al = alive.numpy().reshape(n, reps).astype(bool)
     if stat_part is not None:
-        accumulate_stats(stat_part.numpy().reshape(n, 2 * d0 + 1), o, al)
-    act = policy_actions(rows.numpy(), o, al, d0, hidden, action_dim, clip, _stats(obs_stats, d0), action_noise_std,
-                         seed, generation, member_offset, t)
+        po.accumulate_stats(stat_part.numpy().reshape(n, 2 * d0 + 1), o, al)
+    act = po.policy_actions(rows.numpy(), o, al, d0, hidden, action_dim, clip, _stats(obs_stats, d0), action_noise_std,
+                            seed, generation, member_offset, t)
     return _out(_f32(act).reshape(n, reps, action_dim), out)
 
 

@@ -16,6 +16,7 @@ import torch.distributed as dist
 import cpu_ops
 import host_env_support as hs
 from oracle import nes_oracle as orc
+from oracle import pendulum_oracle as po
 from oracle import synth_walk as sw
 from ranks import spawn
 
@@ -113,7 +114,7 @@ def _nes(mode, kernels):
     if mode.startswith('device'):
         return RolloutEngine(hidden=16, theta0=orc.synthetic_theta(3, 16, 1, seed=2), repetitions=2, horizon=12,
                              action_noise_std=0.1, **common), Cfg(repetitions=2)
-    return HostEnvEngine(env_fn=None, state_dim=3, action_dim=1, batch_env_fn=lambda B: hs.PendulumBatch(B, 7, horizon=9),
+    return HostEnvEngine(env_fn=None, state_dim=3, action_dim=1, batch_env_fn=lambda B: po.PendulumBatch(B, 7, horizon=9),
                          hidden=16, theta0=orc.synthetic_theta(3, 16, 1, seed=3), repetitions=2, test_repetitions=3,
                          clip=2.0, **common), Cfg(repetitions=2, test_repetitions=3)
 
@@ -129,7 +130,7 @@ def _nes_config(mode):
         cfg.repetitions, cfg.test_repetitions = (2 if cfg.normalize_obs else 1), 2
     else:
         cfg = HostEnvConfig(hs.PendulumProbe, hidden_size=16, clip=2.0,
-                            batch_env_fn=lambda B: hs.PendulumBatch(B, 7, horizon=9))
+                            batch_env_fn=lambda B: po.PendulumBatch(B, 7, horizon=9))
         cfg.initial_weight = orc.synthetic_theta(3, 16, 1, seed=3)
         cfg.repetitions, cfg.test_repetitions = 2, 3
     cfg.pop_size, cfg.seed, cfg.max_generations, cfg.mirrored = 6, 7, 1, mode.endswith('mirrored')
@@ -147,7 +148,7 @@ def _cma_config(mode, seed=7):
         cfg.repetitions = cfg.test_repetitions = 2
     elif mode == 'host':
         cfg = HostEnvConfig(hs.PendulumProbe, hidden_size=16, clip=2.0, task='Pendulum-v0',
-                            batch_env_fn=lambda B: hs.PendulumBatch(B, seed, horizon=9))
+                            batch_env_fn=lambda B: po.PendulumBatch(B, seed, horizon=9))
         cfg.repetitions, cfg.test_repetitions = 2, 3
     else:       # episodes of varying length
         cfg = HostEnvConfig(sw.SynthWalkEnv, hidden_size=16, task='SynthWalk-v0',

@@ -241,7 +241,7 @@ def host_pendulum(g):
     from distributedes_b200.config import HostEnvConfig
     seed = int(g['seed'])
     return _pendulum_run(HostEnvConfig(hs.PendulumProbe, hidden_size=int(g['H']), clip=2.0, task='Pendulum-v0',
-                                       batch_env_fn=lambda B: hs.PendulumBatch(B, seed)), g)
+                                       batch_env_fn=lambda B: po.PendulumBatch(B, seed)), g)
 
 
 def synth_walk(g):

@@ -51,13 +51,13 @@ def test_policy_act_matches_fp64_forward(H, d0, A, reps):
             act = ops.policy_act(dev(rows), dev(obs), dev(alive, torch.uint8), state_dim=d0, hidden=H, action_dim=A,
                                  repetitions=reps, clip=1.5, action_noise_std=noise, seed=seed, generation=gen,
                                  member_offset=off, t=4, obs_stats=st, stat_part=part).cpu().numpy()
-            ref = hs.policy_actions(rows, obs, alive, d0, H, A, 1.5, stats if use_stats else None, noise, seed, gen, off,
+            ref = po.policy_actions(rows, obs, alive, d0, H, A, 1.5, stats if use_stats else None, noise, seed, gen, off,
                                     4)
             assert act.shape == (n, reps, A)
             assert np.all(act[~alive] == 0.0)
             assert np.max(np.abs(act - ref) / (1 + np.abs(ref))) < 3e-5, (use_stats, noise)
             want = np.zeros((n, 2 * d0 + 1))
-            hs.accumulate_stats(want, obs, alive)
+            po.accumulate_stats(want, obs, alive)
             assert np.array_equal(part.cpu().numpy(), want)
 
 
@@ -77,10 +77,10 @@ def test_action_noise_is_the_counter_stream_and_statistics_accumulate_in_step_or
         act = ops.policy_act(rows, dev(obs), dev(alive, torch.uint8), state_dim=d0, hidden=H, action_dim=A,
                              repetitions=reps, clip=10.0, action_noise_std=1.0, seed=99, generation=6, member_offset=11,
                              t=t, stat_part=part).cpu().numpy()
-        z = hs.action_noise(99, 6, np.arange(11, 11 + n), reps, t, A)
+        z = po.action_noise(99, 6, np.arange(11, 11 + n), reps, t, A)
         assert np.all(np.abs(act - z)[alive] <= 4e-6 * (1 + np.abs(z[alive])))
         assert np.all(act[~alive] == 0)
-        hs.accumulate_stats(want, obs, alive)
+        po.accumulate_stats(want, obs, alive)
         assert np.array_equal(part.cpu().numpy(), want)
     tot = ops.obs_parts_reduce(part, d0).cpu().numpy()
     assert np.array_equal(tot, want[0] + want[1] + want[2])
@@ -119,7 +119,7 @@ def test_policy_act_rejects_bad_arguments():
 # ---- host-stepped Pendulum-v0 against the device rollout's oracle ----------------------------------------------------
 def _pendulum_engine(H, N, reps, seed, theta0, **kw):
     from distributedes_b200.engine import HostEnvEngine
-    return HostEnvEngine(env_fn=hs.PendulumProbe, batch_env_fn=lambda B: hs.PendulumBatch(B, seed), hidden=H, pop_size=N,
+    return HostEnvEngine(env_fn=hs.PendulumProbe, batch_env_fn=lambda B: po.PendulumBatch(B, seed), hidden=H, pop_size=N,
                          theta0=theta0, sigma=0.1, learning_rate=0.1, repetitions=reps, clip=2.0, seed=seed, **kw)
 
 
@@ -150,7 +150,7 @@ def test_two_shards_on_one_gpu_equal_one_shard():
     out = []
     for lo, hi in ((0, N), (0, 5), (5, N)):
         part = torch.zeros((hi - lo, 7), dtype=torch.float64, device='cuda')
-        ep = HostEpisodes(ops, 'cuda', hs.PendulumBatch((hi - lo) * reps, seed, horizon=60), hi - lo, reps, 3, H, 1, 2.0,
+        ep = HostEpisodes(ops, 'cuda', po.PendulumBatch((hi - lo) * reps, seed, horizon=60), hi - lo, reps, 3, H, 1, 2.0,
                           0.2, seed)
         ret, steps = ep.run(rows[lo:hi].contiguous(), generation=gen, member_offset=lo, stat_part=part)
         out.append((ret.mean(1).astype(np.float32), part.cpu().numpy(), steps))

@@ -119,13 +119,12 @@ def test_closed_loop_equals_explicit_rows(H):
 def test_host_stepped_pendulum_equals_closed_loop():
     """HostEnvEngine(mirrored=True) stepping Pendulum-v0 on the host evaluates the members RolloutEngine(mirrored=True)
     evaluates on the device, and both match the oracle's mirrored closed-loop fitness."""
-    import host_env_support as hs
     from distributedes_b200.engine import HostEnvEngine, RolloutEngine
     H, N, reps, seed = 32, 12, 3, 5
     theta0 = orc.synthetic_theta(3, H, 1, seed=4)
     kw = dict(hidden=H, pop_size=N, theta0=theta0, sigma=0.1, learning_rate=0.1, repetitions=reps, seed=seed,
               mirrored=True)
-    host = HostEnvEngine(env_fn=None, state_dim=3, action_dim=1, batch_env_fn=lambda B: hs.PendulumBatch(B, seed),
+    host = HostEnvEngine(env_fn=None, state_dim=3, action_dim=1, batch_env_fn=lambda B: po.PendulumBatch(B, seed),
                          clip=2.0, **kw)
     roll = RolloutEngine(**kw)
     fh, fr = host.evaluate().cpu().numpy(), roll.evaluate().cpu().numpy()
