@@ -51,6 +51,14 @@ SIGNATURES = {
     'des_rollout_eval_solutions': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _P,
                                              C.c_size_t, _P]),
     'des_obs_stats_merge_totals': (C.c_int, [_P, _P, _I32, _P]),
+    'des_rollout_eval_runs': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _D, _U64, _U64, _P, _I64, _I64,
+                                        C.c_int, _P, C.c_size_t, _P]),
+    'des_rank_runs_workspace_bytes': (_SZ, [_I64, _I64]),
+    'des_centered_rank_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _P, _SZ, _P]),
+    'des_grad_runs_workspace_bytes': (_SZ, [_I64, _I64, _I64]),
+    'des_nes_grad_partial_runs': (C.c_int, [_P, _P, _I64, _I64, _I64, _U64, _U64, _P, _P, _SZ, _P]),
+    'des_nes_apply_runs': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, Opt, _P, _P]),
+    'des_obs_stats_merge_totals_runs': (C.c_int, [_P, _P, _I32, _I64, _P]),
     'des_policy_act': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _I64, _P]),
     'des_obs_parts_reduce': (C.c_int, [_P, _P, _I64, _I32, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),

@@ -27,6 +27,19 @@ int not_whole_pairs(const char *who, const char *count, int64_t member_offset, i
     return DES_ERR_INVALID_ARGUMENT;
 }
 
+int check_runs(const char *who, int64_t n_runs, int64_t run_size, int64_t min_size) {
+    DES_REQUIRE(n_runs >= 0 && run_size >= min_size, "%s: need n_runs >= 0 and run_size >= %lld (got %lld and %lld)", who,
+                (long long)min_size, (long long)n_runs, (long long)run_size);
+    if (run_size > kRunMaxSize) {
+        set_error("%s: run_size %lld > %lld: batches hold runs of up to %lld members (a larger population fills the GPU "
+                  "alone)", who, (long long)run_size, (long long)kRunMaxSize, (long long)kRunMaxSize);
+        return DES_ERR_UNSUPPORTED;
+    }
+    DES_REQUIRE(n_runs <= ((int64_t)1 << 28) / run_size, "%s: n_runs x run_size = %lld x %lld members, past 2^28", who,
+                (long long)n_runs, (long long)run_size);
+    return DES_OK;
+}
+
 int eval_ffma_launch(float *fitness, const float *theta, const float *obs, const float *target, des_dims dims,
                      double sigma, double clip, uint64_t seed, uint64_t generation, const des_state *state,
                      int64_t member_offset, int64_t n_local, const float *solutions, bool mirrored, cudaStream_t st);

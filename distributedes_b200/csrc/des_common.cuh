@@ -243,6 +243,13 @@ inline bool member_range_ok(int64_t member_offset, int64_t n, int bits) {
 inline bool whole_pairs(int64_t member_offset, int64_t n) { return member_offset % 2 == 0 && n % 2 == 0; }
 // Reports a shard that whole_pairs rejects (`count` names n's argument): DES_ERR_INVALID_ARGUMENT.
 int not_whole_pairs(const char *who, const char *count, int64_t member_offset, int64_t n);
+// A batch of independent runs (the *_runs entry points): n_runs populations of run_size members each, run r's member i
+// the global member r * run_size + i.  Runs stop at the counting rank's population (kRunMaxSize): a larger population
+// fills the GPU without batching.  check_runs returns DES_OK or reports a bad batch: n_runs >= 0 and
+// min_size <= run_size (DES_ERR_INVALID_ARGUMENT), run_size <= kRunMaxSize (DES_ERR_UNSUPPORTED), and every member
+// index below 2^28 (DES_ERR_INVALID_ARGUMENT).
+constexpr int64_t kRunMaxSize = 2048;
+int check_runs(const char *who, int64_t n_runs, int64_t run_size, int64_t min_size);
 // Hidden widths of the closed-loop policy kernels (rollout_pendulum_kernel, policy_act_kernel): H/16 units per lane.
 inline bool policy_width_ok(int H) { return H == 16 || H == 32 || H == 64 || H == 96 || H == 128; }
 
@@ -258,6 +265,8 @@ int launch_smem(const char *name, void (*kernel)(Params...), dim3 grid, dim3 blo
 
 // totals[c] = sum over the n_local rows of parts[n_local][width] (des_obs.cu), in member order
 int obs_parts_reduce(double *totals, const double *parts, int64_t n_local, int width, cudaStream_t st);
+// totals[r][c] = sum over run r's run_size rows of parts[n_runs * run_size][width], each run exactly as obs_parts_reduce
+int obs_parts_reduce_runs(double *totals, const double *parts, int64_t n_runs, int64_t run_size, int width, cudaStream_t st);
 
 // ---- CMA rank-mu (des_cma.cu: fp32 FFMA kernel and the entry point; des_cma_tc.cu: split-fp16 wgmma SYRK) ----------
 constexpr int64_t kCmaTcMinN = 2048;     // n >= this runs on the tensor cores, smaller n on the FFMA kernel

@@ -9,6 +9,7 @@
 // returns, cma_es.py:22-29).  Everything after the weights are staged is the same code in both modes.
 // Policy arithmetic fp32 (FFMA, MUFU-based tanh), dynamics fp64 (gym keeps its state in float64).
 // Algorithmic work per environment step: 2*(3H + H*H + H) flop; no HBM traffic beyond theta (L2 resident).
+#include <type_traits>
 #include "des_common.cuh"
 
 namespace des {
@@ -32,6 +33,12 @@ struct RollArgs {
     uint32_t reset_member_base;        // counter word for the reset stream: member index (or the test-episode index)
     int noiseless;                     // 1: evaluate theta itself (test(), natural_es.py:101-110)
     int mirrored;                      // NES mode: member m perturbs with (-1)^(m & 1) * eps of counter word m >> 1
+};
+
+// The arguments of a batch of runs (des_rollout_eval_runs).  A struct of its own, so that the single-population kernels
+// keep RollArgs, their parameter block, exactly as it is.
+struct RunArgs : RollArgs {
+    int run_size;                      // members per run
 };
 
 __device__ __forceinline__ double unit_open(uint32_t x) { return ((double)(x & 0x7FFFFFu) + 0.5) * (1.0 / 8388608.0); }
@@ -73,9 +80,16 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // transposed weights and one 5-float broadcast of h1.  The fp64 dynamics of episode 5*eg + rg%5 run in every lane
 // (the copies in rg >= 5 are redundant), i.e. once per step for the whole member.
 // kRows: the weights are row blockIdx.x of a.rows (no noise is generated); otherwise theta + sigma*eps of the member.
-template <int R, bool kRows>   // H = 16*R
-__global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
+// Args = RunArgs: a batch of independent runs (des_rollout_eval_runs, member_offset 0): CTA b is member b % run_size of
+// run b / run_size, global member b, with its run's row of theta and of the statistics.  Everything else is the same code.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs or RunArgs
+__global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
+    if constexpr (std::is_same<Args, RunArgs>::value) {
+        const unsigned run = blockIdx.x / (unsigned)a.run_size;
+        a.theta += (size_t)run * a.L.P;
+        if (a.obs_stats) a.obs_stats += (size_t)run * 7;
+    }
     extern __shared__ __align__(16) float sm[];
     float *W2T = sm;                     // [k][j] = W2[j][k]
     // h1 panels, one per episode half, rows in the permuted order p(k) = (k % R)*16 + k/R so that the 16 unit groups
@@ -256,14 +270,16 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(RollArgs a) {
     }
 }
 
-// Shared by both entry points: argument checks (before any CUDA work), workspace, launch.  rows_mode selects the
-// explicit-solution kernels: `weights` is then rows[n_local][P] instead of the theta that sigma*eps perturbs.
+// Shared by the entry points: argument checks (before any CUDA work), workspace, launch.  rows_mode selects the
+// explicit-solution kernels: `weights` is then rows[n_local][P] instead of the theta that sigma*eps perturbs.  run_size > 0
+// makes the n_local members a batch of runs of run_size (des_rollout_eval_runs, member_offset 0): `weights` and
+// `obs_stats_dev` hold one row per run, and the observation totals are reduced per run.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                           double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
-                          void *workspace_dev, size_t workspace_bytes, bool mirrored, cudaStream_t st) {
+                          void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size, cudaStream_t st) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -299,13 +315,29 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     const int H = dims.hidden;
     const size_t smem = sizeof(float) * ((size_t)H * H + 2 * (size_t)H * kHS + 8 + 40 + (size_t)H * 4 + 3 * (size_t)H + 4) +
                         sizeof(double) * 80;
+    if (run_size > 0) {
+        RunArgs ra;
+        static_cast<RollArgs &>(ra) = a;
+        ra.run_size = (int)run_size;
+        void (*runs_kernel)(RunArgs);
+        switch (H / 16) {
+            case 1: runs_kernel = rollout_pendulum_kernel<1, false, RunArgs>; break;
+            case 2: runs_kernel = rollout_pendulum_kernel<2, false, RunArgs>; break;
+            case 4: runs_kernel = rollout_pendulum_kernel<4, false, RunArgs>; break;
+            case 6: runs_kernel = rollout_pendulum_kernel<6, false, RunArgs>; break;
+            default: runs_kernel = rollout_pendulum_kernel<8, false, RunArgs>; break;
+        }
+        const int rc = launch_smem("rollout_pendulum_kernel", runs_kernel, (unsigned)n_local, 32, smem, st, ra);
+        if (rc != DES_OK || !obs_totals_out_dev) return rc;
+        return obs_parts_reduce_runs(obs_totals_out_dev, a.stat_part, n_local / run_size, run_size, 7, st);
+    }
     void (*kernel)(RollArgs);
     switch (H / 16) {                    // R = H/16 hidden units per lane
-        case 1: kernel = rows_mode ? rollout_pendulum_kernel<1, true> : rollout_pendulum_kernel<1, false>; break;
-        case 2: kernel = rows_mode ? rollout_pendulum_kernel<2, true> : rollout_pendulum_kernel<2, false>; break;
-        case 4: kernel = rows_mode ? rollout_pendulum_kernel<4, true> : rollout_pendulum_kernel<4, false>; break;
-        case 6: kernel = rows_mode ? rollout_pendulum_kernel<6, true> : rollout_pendulum_kernel<6, false>; break;
-        default: kernel = rows_mode ? rollout_pendulum_kernel<8, true> : rollout_pendulum_kernel<8, false>; break;
+        case 1: kernel = rows_mode ? rollout_pendulum_kernel<1, true, RollArgs> : rollout_pendulum_kernel<1, false, RollArgs>; break;
+        case 2: kernel = rows_mode ? rollout_pendulum_kernel<2, true, RollArgs> : rollout_pendulum_kernel<2, false, RollArgs>; break;
+        case 4: kernel = rows_mode ? rollout_pendulum_kernel<4, true, RollArgs> : rollout_pendulum_kernel<4, false, RollArgs>; break;
+        case 6: kernel = rows_mode ? rollout_pendulum_kernel<6, true, RollArgs> : rollout_pendulum_kernel<6, false, RollArgs>; break;
+        default: kernel = rows_mode ? rollout_pendulum_kernel<8, true, RollArgs> : rollout_pendulum_kernel<8, false, RollArgs>; break;
     }
     const int rc = launch_smem("rollout_pendulum_kernel", kernel, (unsigned)n_local, 32, smem, st, a);
     if (rc != DES_OK || !obs_totals_out_dev) return rc;
@@ -324,7 +356,7 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     return des::rollout_launch("des_rollout_eval", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               false, (cudaStream_t)stream);
+                               false, 0, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -337,7 +369,7 @@ extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *
     return des::rollout_launch("des_rollout_eval_mirrored", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                theta_dev, false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               true, (cudaStream_t)stream);
+                               true, 0, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -349,5 +381,22 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
     return des::rollout_launch("des_rollout_eval_solutions", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
-                               false, (cudaStream_t)stream);
+                               false, 0, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *episode_returns_out_dev,
+                                             double *obs_totals_out_dev, const float *theta_dev, const float *obs_stats_dev,
+                                             int env, des_dims dims, int32_t repetitions, double sigma, double clip,
+                                             double action_noise_std, uint64_t seed, uint64_t generation,
+                                             const des_state *state_dev, int64_t n_runs, int64_t run_size, int noiseless,
+                                             void *workspace_dev, size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_runs";
+    const int rc = des::check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(!noiseless || run_size == 1, "%s: test episodes (noiseless) evaluate one theta per run: run_size must be 1 "
+                "(got %lld)", who, (long long)run_size);
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
+                               obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
+                               state_dev, 0, n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size,
+                               (cudaStream_t)stream);
 }

@@ -3,6 +3,7 @@
 //   des_obs_normalize            (o - m)/sqrt(v + 1e-6) of the tape
 //   des_obs_parts_reduce         per-member partial sums -> totals               (des_rollout_eval, des_policy_act rows)
 //   des_obs_stats_merge_totals   totals (all-reduced over ranks) -> shared statistics
+//   des_obs_stats_merge_totals_runs  the same for a batch of runs: one row of totals into one row of statistics per run
 // In the reference every worker feeds each observation into online Welford statistics (utils.py:68-73) and, after
 // the generation, the master Chan-merges them into the shared statistics (utils.py:85-96); observations are
 // normalised with the statistics of the PREVIOUS generations, (o - m)/sqrt(v + 1e-6), raw while n == 0
@@ -77,6 +78,38 @@ __global__ void stat_part_reduce_kernel(double *__restrict__ totals, const doubl
     totals[c] = s;
 }
 
+// one CTA per run: run blockIdx.x's rows in member order, as stat_part_reduce_kernel sums a single population's
+__global__ void stat_part_reduce_runs_kernel(double *__restrict__ totals, const double *__restrict__ part, int64_t run_size,
+                                             int width) {
+    const int c = threadIdx.x;
+    if (c >= width) return;
+    const double *p = part + (int64_t)blockIdx.x * run_size * width;
+    double s = 0.0;
+    for (int64_t i = 0; i < run_size; ++i) s += p[i * width + c];
+    totals[(int64_t)blockIdx.x * width + c] = s;
+}
+
+// one CTA per run, the columns of obs_stats_merge_totals_kernel
+__global__ void obs_stats_merge_totals_runs_kernel(float *__restrict__ stats, const double *__restrict__ totals, int d0) {
+    const int k = threadIdx.x;
+    if (k >= d0) return;
+    const int w = 2 * d0 + 1;
+    stats += (int64_t)blockIdx.x * w;
+    totals += (int64_t)blockIdx.x * w;
+    const double nB = totals[2 * d0];
+    if (nB <= 0) return;
+    const double mb = totals[k] / nB, vb = fmax(totals[d0 + k] / nB - mb * mb, 0.0);
+    chan_merge(stats, d0, k, mb, vb, nB);
+}
+
+int obs_parts_reduce_runs(double *totals, const double *parts, int64_t n_runs, int64_t run_size, int width, cudaStream_t st) {
+    if (n_runs == 0) return DES_OK;
+    stat_part_reduce_runs_kernel<<<(unsigned)n_runs, (unsigned)((width + 31) / 32 * 32), 0, st>>>(totals, parts, run_size,
+                                                                                                 width);
+    DES_LAUNCH_CHECK("stat_part_reduce_runs_kernel");
+    return DES_OK;
+}
+
 int obs_parts_reduce(double *totals, const double *parts, int64_t n_local, int width, cudaStream_t st) {
     stat_part_reduce_kernel<<<1, (unsigned)((width + 31) / 32 * 32), 0, st>>>(totals, parts, n_local, width);
     DES_LAUNCH_CHECK("stat_part_reduce_kernel");
@@ -117,5 +150,19 @@ extern "C" DES_API int des_obs_stats_merge_totals(float *stats_dev, const double
     DES_REQUIRE(stats_dev && obs_totals_dev && state_dim > 0 && state_dim <= 1024, "des_obs_stats_merge_totals: bad arguments");
     des::obs_stats_merge_totals_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(stats_dev, obs_totals_dev, state_dim);
     DES_LAUNCH_CHECK("obs_stats_merge_totals_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API int des_obs_stats_merge_totals_runs(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,
+                                                       int64_t n_runs, void *stream) {
+    const char *who = "des_obs_stats_merge_totals_runs";
+    DES_REQUIRE(state_dim > 0 && state_dim <= 1024, "%s: state_dim must be in [1, 1024] (got %d)", who, (int)state_dim);
+    DES_REQUIRE(n_runs >= 0 && n_runs <= ((int64_t)1 << 28), "%s: need 0 <= n_runs <= 2^28 (got %lld)", who,
+                (long long)n_runs);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(stats_dev && obs_totals_dev, "%s: NULL pointer", who);
+    des::obs_stats_merge_totals_runs_kernel<<<(unsigned)n_runs, (unsigned)((state_dim + 31) / 32 * 32), 0,
+                                              (cudaStream_t)stream>>>(stats_dev, obs_totals_dev, state_dim);
+    DES_LAUNCH_CHECK("obs_stats_merge_totals_runs_kernel");
     return DES_OK;
 }

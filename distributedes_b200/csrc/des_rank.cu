@@ -23,12 +23,11 @@ __device__ __forceinline__ uint32_t order_key(float f) {
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
-__global__ void __launch_bounds__(kRankThreads) rank_count_kernel(int32_t *__restrict__ counts,
-                                                                   const float *__restrict__ fitness, int64_t N,
-                                                                   int64_t member_offset, int64_t n_local,
-                                                                   int64_t j_per_block) {
+// counts[il] += #{j in the CTA's j-slice : (key_j, j) < (key_i, i)} for member i = member_offset + il, il in member block bx
+__device__ __forceinline__ void rank_count(int32_t *__restrict__ counts, const float *__restrict__ fitness, int64_t N,
+                                           int64_t member_offset, int64_t n_local, int64_t j_per_block, unsigned bx) {
     __shared__ uint32_t keys[kRankTile];
-    const int64_t il = (int64_t)blockIdx.x * kRankThreads + threadIdx.x;
+    const int64_t il = (int64_t)bx * kRankThreads + threadIdx.x;
     const bool live = il < n_local;
     const int64_t ig = member_offset + il;
     const uint64_t mine = live ? (((uint64_t)order_key(__ldg(fitness + ig)) << 32) | (uint64_t)(uint32_t)ig) : 0;
@@ -50,6 +49,43 @@ __global__ void __launch_bounds__(kRankThreads) rank_count_kernel(int32_t *__res
         }
     }
     if (live && cnt) atomicAdd(counts + il, cnt);
+}
+
+__global__ void __launch_bounds__(kRankThreads) rank_count_kernel(int32_t *__restrict__ counts,
+                                                                   const float *__restrict__ fitness, int64_t N,
+                                                                   int64_t member_offset, int64_t n_local,
+                                                                   int64_t j_per_block) {
+    rank_count(counts, fitness, N, member_offset, n_local, j_per_block, blockIdx.x);
+}
+
+// A batch of runs of N members (des_centered_rank_runs): member blocks of all runs along x, blocks_per_run per run, each
+// run ranked within itself exactly as des_centered_rank ranks a population of N.
+__global__ void __launch_bounds__(kRankThreads) rank_count_runs_kernel(int32_t *__restrict__ counts,
+                                                                        const float *__restrict__ fitness, int64_t N,
+                                                                        int64_t j_per_block, unsigned blocks_per_run) {
+    const int64_t run = blockIdx.x / blocks_per_run;
+    rank_count(counts + run * N, fitness + run * N, N, 0, N, j_per_block, blockIdx.x % blocks_per_run);
+}
+
+// The counting path's grid: bx member blocks of n_local, by j-slices of j_per_block keys (a multiple of the smem tile).
+struct CountPlan {
+    unsigned bx, by;
+    int64_t j_per_block;
+};
+static CountPlan count_plan(int64_t N, int64_t n_local) {
+    CountPlan p;
+    p.bx = (unsigned)((n_local + kRankThreads - 1) / kRankThreads);
+    // enough j-slices to fill the machine a few times over, each a multiple of the smem tile
+    int64_t want_blocks = 132 * 8;                 // 132 SMs (H100 SXM)
+    int64_t by = (want_blocks + p.bx - 1) / p.bx;
+    int64_t max_by = (N + kRankTile - 1) / kRankTile;
+    if (by > max_by) by = max_by;
+    if (by < 1) by = 1;
+    if (by > 65535) by = 65535;
+    int64_t j_per_block = (N + by - 1) / by;
+    p.j_per_block = ((j_per_block + kRankTile - 1) / kRankTile) * kRankTile;
+    p.by = (unsigned)((N + p.j_per_block - 1) / p.j_per_block);
+    return p;
 }
 
 __global__ void rank_finish_kernel(float *__restrict__ shaped, int32_t *__restrict__ rank_out,
@@ -340,22 +376,45 @@ extern "C" DES_API int des_centered_rank(float *shaped_out_dev, int32_t *rank_ou
     }
     int32_t *counts = (int32_t *)workspace_dev;
     DES_CUDA(cudaMemsetAsync(counts, 0, (size_t)n_local * sizeof(int32_t), st));
-    const unsigned bx = (unsigned)((n_local + kRankThreads - 1) / kRankThreads);
-    // enough j-slices to fill the machine a few times over, each a multiple of the smem tile
-    int64_t want_blocks = 132 * 8;                 // 132 SMs (H100 SXM)
-    int64_t by = (want_blocks + bx - 1) / bx;
-    int64_t max_by = (N + kRankTile - 1) / kRankTile;
-    if (by > max_by) by = max_by;
-    if (by < 1) by = 1;
-    if (by > 65535) by = 65535;
-    int64_t j_per_block = (N + by - 1) / by;
-    j_per_block = ((j_per_block + kRankTile - 1) / kRankTile) * kRankTile;
-    by = (N + j_per_block - 1) / j_per_block;
-    rank_count_kernel<<<dim3(bx, (unsigned)by), kRankThreads, 0, st>>>(counts, fitness_all_dev, N, member_offset,
-                                                                       n_local, j_per_block);
+    const CountPlan p = count_plan(N, n_local);
+    rank_count_kernel<<<dim3(p.bx, p.by), kRankThreads, 0, st>>>(counts, fitness_all_dev, N, member_offset, n_local,
+                                                                 p.j_per_block);
     DES_LAUNCH_CHECK("rank_count_kernel");
     rank_finish_kernel<<<(unsigned)((n_local + 255) / 256), 256, 0, st>>>(shaped_out_dev, rank_out_dev, counts, N,
                                                                           n_local);
+    DES_LAUNCH_CHECK("rank_finish_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API size_t des_rank_runs_workspace_bytes(int64_t n_runs, int64_t run_size) {
+    if (n_runs <= 0 || run_size <= 0 || run_size > des::kRunMaxSize || n_runs > ((int64_t)1 << 28) / run_size) return 0;
+    return (size_t)(n_runs * run_size) * sizeof(int32_t);
+}
+
+extern "C" DES_API int des_centered_rank_runs(float *shaped_out_dev, int32_t *rank_out_dev, const float *fitness_dev,
+                                              int64_t n_runs, int64_t run_size, void *workspace_dev, size_t workspace_bytes,
+                                              void *stream) {
+    using namespace des;
+    const char *who = "des_centered_rank_runs";
+    const int rc = check_runs(who, n_runs, run_size, 2);      // utils.py:146 divides by N-1
+    if (rc != DES_OK) return rc;
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(shaped_out_dev && fitness_dev, "%s: NULL pointer", who);
+    const size_t need = des_rank_runs_workspace_bytes(n_runs, run_size);
+    if (!workspace_dev || workspace_bytes < need) {
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t n = n_runs * run_size;
+    int32_t *counts = (int32_t *)workspace_dev;
+    DES_CUDA(cudaMemsetAsync(counts, 0, (size_t)n * sizeof(int32_t), st));
+    const CountPlan p = count_plan(run_size, run_size);       // one run's plan: a single j-slice up to 2048 members
+    rank_count_runs_kernel<<<dim3((unsigned)(p.bx * n_runs), p.by), kRankThreads, 0, st>>>(counts, fitness_dev, run_size,
+                                                                                          p.j_per_block, p.bx);
+    DES_LAUNCH_CHECK("rank_count_runs_kernel");
+    // the finishing step is elementwise in the rank: the batch is one vector of n ranks within runs of run_size
+    rank_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(shaped_out_dev, rank_out_dev, counts, run_size, n);
     DES_LAUNCH_CHECK("rank_finish_kernel");
     return DES_OK;
 }

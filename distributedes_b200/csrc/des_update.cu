@@ -53,7 +53,9 @@ __host__ inline GradPlan grad_plan(int64_t n_local, int64_t P) {
 
 // kMirror: i runs over the n_local pairs of a mirrored shard, member_offset is the pair index of its first pair, and
 // pair i contributes (s_2i - s_2i+1) * eps_i: sum_m s_m eps_m with eps_2i+1 = -eps_2i, half the normals to regenerate
-template <bool kMirror>
+// kRuns: CTA row z takes run z of a batch (des_nes_grad_partial_runs), a shard of n_local members at member_offset +
+// z * n_local whose gridDim.y slices have their own rows of ws.
+template <bool kMirror, bool kRuns>
 __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restrict__ ws, const float *__restrict__ shaped,
                                                                    int64_t n_local, int64_t nq, int64_t Ppad,
                                                                    int64_t per_chunk, PhiloxKey key,
@@ -61,6 +63,11 @@ __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restr
                                                                    uint64_t member_offset) {
     const int64_t q = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
     if (q >= nq) return;
+    if constexpr (kRuns) {
+        ws += (int64_t)blockIdx.z * gridDim.y * Ppad;
+        shaped += (int64_t)blockIdx.z * n_local;
+        member_offset += (uint64_t)blockIdx.z * n_local;
+    }
     const uint32_t gen = generation_word(state, gen_arg);
     const int64_t i0 = (int64_t)blockIdx.y * per_chunk;
     const int64_t i1 = min(n_local, i0 + per_chunk);
@@ -85,8 +92,8 @@ __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restr
 // threads takes 32 columns; row y adds chunks y, y+8, ... in order, then row 0 adds the eight row sums in order.
 // (One thread per column walking all chunks serially took 13 us at P = 6020 / 128 chunks: 24 CTAs of dependent loads.)
 constexpr int kReduceRows = 8;
-__global__ void __launch_bounds__(32 * kReduceRows) grad_reduce_kernel(float *__restrict__ partial, const float *__restrict__ ws,
-                                                                       int64_t P, int64_t Ppad, int chunks) {
+__device__ __forceinline__ void grad_reduce(float *__restrict__ partial, const float *__restrict__ ws, int64_t P,
+                                            int64_t Ppad, int chunks) {
     __shared__ double rows[kReduceRows][33];
     const int x = threadIdx.x, y = threadIdx.y;
     const int64_t j = (int64_t)blockIdx.x * 32 + x;
@@ -103,12 +110,26 @@ __global__ void __launch_bounds__(32 * kReduceRows) grad_reduce_kernel(float *__
     }
 }
 
-__global__ void apply_kernel(float *__restrict__ theta, double *__restrict__ am, double *__restrict__ av,
-                             float *__restrict__ update_out, double *__restrict__ grad_out,
-                             const float *__restrict__ partial, int64_t P, double inv_n_unused, int64_t N, des_opt o,
-                             const des_state *__restrict__ state) {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= P) return;
+__global__ void __launch_bounds__(32 * kReduceRows) grad_reduce_kernel(float *__restrict__ partial, const float *__restrict__ ws,
+                                                                       int64_t P, int64_t Ppad, int chunks) {
+    grad_reduce(partial, ws, P, Ppad, chunks);
+}
+
+// run r: partial[r][P] from its `chunks` rows of ws; runs along y, strided past 65535
+__global__ void __launch_bounds__(32 * kReduceRows) grad_reduce_runs_kernel(float *__restrict__ partial,
+                                                                            const float *__restrict__ ws, int64_t n_runs,
+                                                                            int64_t P, int64_t Ppad, int chunks) {
+    for (int64_t r = blockIdx.y; r < n_runs; r += gridDim.y) {
+        grad_reduce(partial + r * P, ws + r * chunks * Ppad, P, Ppad, chunks);
+        __syncthreads();                 // the shared row sums are reused by the next run
+    }
+}
+
+// parameter j of one population
+__device__ __forceinline__ void apply_at(int64_t j, float *__restrict__ theta, double *__restrict__ am,
+                                         double *__restrict__ av, float *__restrict__ update_out,
+                                         double *__restrict__ grad_out, const float *__restrict__ partial, int64_t N,
+                                         const des_opt &o, const des_state *__restrict__ state) {
     // utils.py:160-161: beta_t *= beta happens before use, so this step uses beta^(t+1)
     const double b1t = state->beta1_t * o.beta1;
     const double b2t = state->beta2_t * o.beta2;
@@ -127,6 +148,29 @@ __global__ void apply_kernel(float *__restrict__ theta, double *__restrict__ am,
     const float upd = __fmul_rn((float)o.learning_rate, step32);   // :96 lr * gradient (fp32 tensor op)
     if (update_out) update_out[j] = upd;
     theta[j] = __fadd_rn(theta[j], upd);                        // :96 param.add_
+}
+
+__global__ void apply_kernel(float *__restrict__ theta, double *__restrict__ am, double *__restrict__ av,
+                             float *__restrict__ update_out, double *__restrict__ grad_out,
+                             const float *__restrict__ partial, int64_t P, double inv_n_unused, int64_t N, des_opt o,
+                             const des_state *__restrict__ state) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= P) return;
+    apply_at(j, theta, am, av, update_out, grad_out, partial, N, o, state);
+}
+
+// run r's rows of every [n_runs][P] argument; runs along y, strided past 65535
+__global__ void apply_runs_kernel(float *__restrict__ theta, double *__restrict__ am, double *__restrict__ av,
+                                  float *__restrict__ update_out, double *__restrict__ grad_out,
+                                  const float *__restrict__ partial, int64_t P, int64_t n_runs, int64_t N, des_opt o,
+                                  const des_state *__restrict__ state) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= P) return;
+    for (int64_t r = blockIdx.y; r < n_runs; r += gridDim.y) {
+        const int64_t o_r = r * P;
+        apply_at(j, theta + o_r, am + o_r, av + o_r, update_out ? update_out + o_r : nullptr,
+                 grad_out ? grad_out + o_r : nullptr, partial + o_r, N, o, state);
+    }
 }
 
 __global__ void state_init_kernel(des_state *st, uint64_t generation) {
@@ -181,11 +225,11 @@ static int grad_partial(const char *who, float *partial_out_dev, const float *sh
     if (mirrored) {
         const int64_t pairs = n_local / 2, per_chunk = (p.per_chunk + 1) / 2;
         chunks = (int)((pairs + per_chunk - 1) / per_chunk);     // <= p.chunks
-        grad_chunk_kernel<true><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
+        grad_chunk_kernel<true, false><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
             ws, shaped_local_dev, pairs, p.nq, p.Ppad, per_chunk, key, (uint32_t)generation, state_dev,
             (uint64_t)member_offset / 2);
     } else {
-        grad_chunk_kernel<false><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
+        grad_chunk_kernel<false, false><<<dim3(bx, (unsigned)chunks), kGradThreads, 0, st>>>(
             ws, shaped_local_dev, n_local, p.nq, p.Ppad, p.per_chunk, key, (uint32_t)generation, state_dev,
             (uint64_t)member_offset);
     }
@@ -237,5 +281,66 @@ extern "C" DES_API int des_state_advance(des_state *state_dev, double beta1, dou
     DES_REQUIRE(state_dev, "des_state_advance: state_dev is NULL");
     des::state_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state_dev, beta1, beta2);
     DES_LAUNCH_CHECK("state_advance_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API size_t des_grad_runs_workspace_bytes(int64_t n_runs, int64_t run_size, int64_t P) {
+    if (n_runs <= 0 || run_size <= 0 || P <= 0 || run_size > des::kRunMaxSize || n_runs > ((int64_t)1 << 28) / run_size)
+        return 0;
+    return (size_t)n_runs * des_grad_workspace_bytes(run_size, P);
+}
+
+extern "C" DES_API int des_nes_grad_partial_runs(float *partial_out_dev, const float *shaped_dev, int64_t n_runs,
+                                                 int64_t run_size, int64_t P, uint64_t seed, uint64_t generation,
+                                                 const des_state *state_dev, void *workspace_dev, size_t workspace_bytes,
+                                                 void *stream) {
+    using namespace des;
+    const char *who = "des_nes_grad_partial_runs";
+    const int rc = check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(P > 0, "%s: bad size P=%lld", who, (long long)P);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(partial_out_dev && shaped_dev, "%s: NULL pointer", who);
+    const GradPlan p = grad_plan(run_size, P);           // each run sliced as a shard of run_size members
+    const size_t need = des_grad_runs_workspace_bytes(n_runs, run_size, P);
+    if (!workspace_dev || workspace_bytes < need) {
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
+    DES_REQUIRE(((uintptr_t)workspace_dev & 15) == 0, "%s: workspace must be 16-byte aligned", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    float *ws = (float *)workspace_dev;
+    const unsigned bx = (unsigned)((p.nq + kGradThreads - 1) / kGradThreads);
+    const PhiloxKey key = make_philox_key(seed);
+    for (int64_t r0 = 0; r0 < n_runs; r0 += 65535) {            // grid z: up to 65535 runs per launch
+        const int64_t nr = n_runs - r0 < 65535 ? n_runs - r0 : 65535;
+        grad_chunk_kernel<false, true><<<dim3(bx, (unsigned)p.chunks, (unsigned)nr), kGradThreads, 0, st>>>(
+            ws + r0 * p.chunks * p.Ppad, shaped_dev + r0 * run_size, run_size, p.nq, p.Ppad, p.per_chunk, key,
+            (uint32_t)generation, state_dev, (uint64_t)(r0 * run_size));
+        DES_LAUNCH_CHECK("grad_chunk_kernel");
+    }
+    const unsigned bz = (unsigned)(n_runs < 65535 ? n_runs : 65535);
+    grad_reduce_runs_kernel<<<dim3((unsigned)((P + 31) / 32), bz), dim3(32, kReduceRows), 0, st>>>(partial_out_dev, ws,
+                                                                                                 n_runs, P, p.Ppad, p.chunks);
+    DES_LAUNCH_CHECK("grad_reduce_runs_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API int des_nes_apply_runs(float *theta_dev, double *adam_m_dev, double *adam_v_dev, float *update_out_dev,
+                                          double *grad_out_dev, const float *partial_sum_dev, int64_t P, int64_t n_runs,
+                                          int64_t run_size, des_opt opt, const des_state *state_dev, void *stream) {
+    using namespace des;
+    const char *who = "des_nes_apply_runs";
+    const int rc = check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(P > 0, "%s: bad size P=%lld", who, (long long)P);
+    DES_REQUIRE(opt.sigma > 0.0, "%s: sigma must be > 0 (natural_es.py:92 divides by it)", who);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(theta_dev && adam_m_dev && adam_v_dev && partial_sum_dev && state_dev, "%s: NULL pointer", who);
+    const unsigned by = (unsigned)(n_runs < 65535 ? n_runs : 65535);
+    apply_runs_kernel<<<dim3((unsigned)((P + 255) / 256), by), 256, 0, (cudaStream_t)stream>>>(
+        theta_dev, adam_m_dev, adam_v_dev, update_out_dev, grad_out_dev, partial_sum_dev, P, n_runs, run_size, opt,
+        state_dev);
+    DES_LAUNCH_CHECK("apply_runs_kernel");
     return DES_OK;
 }

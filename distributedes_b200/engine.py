@@ -76,6 +76,23 @@ class RankGroup:
         return out
 
 
+def capture_generation(device, live, generation):
+    """`generation` captured as one CUDA graph, after a warm-up run on a side stream whose effect on the `live` tensors
+    (the state a generation advances) is rolled back: capture does not execute, the warm-up did."""
+    saved = [t.clone() for t in live]
+    s = torch.cuda.Stream(device=device)
+    s.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(s):
+        generation()                             # warm-up on the side stream (lazy module loading etc.)
+    torch.cuda.current_stream(device).wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        generation()
+    for t, v in zip(live, saved):
+        t.copy_(v)
+    return g
+
+
 def kernels_and_device(kernels=None, device=None):
     """The device ops and the device of a trainer: `kernels` None is distributedes_b200.ops (libdes_b200.so), `device`
     None the current CUDA device.  The library has no CPU path, so it is refused a CPU device here, at construction."""
@@ -232,18 +249,7 @@ class NESEngine:
         """Capture eval -> rank -> grad -> apply -> advance as one CUDA graph.  Generation / Adam counters
         live in device memory (des_state), so the same graph is replayed every generation."""
         live = [self.theta, self.adam_m, self.adam_v, self.state] + ([self.obs_stats] if self.normalize_obs else [])
-        saved = [t.clone() for t in live]
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(s):
-            self._generation_eager()                 # warm-up on the side stream (lazy module loading etc.)
-        torch.cuda.current_stream(self.device).wait_stream(s)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._generation_eager()
-        for t, v in zip(live, saved):
-            t.copy_(v)                                # capture does not execute, the warm-up did: roll it back
-        self._graph = g
+        self._graph = capture_generation(self.device, live, self._generation_eager)
 
     # -- host-buffer entry (the reference-facing call: inputs and results live on the host) ---------------------
     def set_tape(self, obs, target):
@@ -320,3 +326,123 @@ class HostEnvEngine(NESEngine):
         super().__init__(state_dim=src.d0, hidden=hidden, action_dim=src.A, pop_size=pop_size, theta0=theta0, sigma=sigma,
                          learning_rate=learning_rate, clip=clip, mirrored=mirrored, source=src, kernels=k, device=dev,
                          **kw)
+
+
+class RolloutRunsEngine:
+    """R independent NES runs of `pop_size` members on the device's closed-loop Pendulum, trained together: every
+    generation evaluates all runs' members in one rollout launch and ranks, reduces, applies and merges the statistics of
+    all runs in one launch each, so the launches per generation do not depend on R.
+
+    Run r's member i is the global member r*pop_size + i of the one seed (ops_runs), so run 0 is RolloutEngine's run, bit
+    for bit, and runs 1..R-1 are further independent streams of the same seed, not the runs of seeds 1..R-1.  Each run has
+    its own theta [R, P], fp64 Adam moments, fitness [R, N] and normaliser statistics [R, 2*d0+1]; all runs share the
+    des_state (generation word, Adam's t and beta^t), the hyper-parameters and, unless theta0 is [R, P], the start point.
+    `kernels` is the module of device ops (default: distributedes_b200.ops_runs); a stand-in runs the host logic on CPU.
+    One GPU; the runs are not sharded."""
+
+    MAX_RUN_SIZE = 2048           # des_*_runs: a larger population fills the GPU without batching
+
+    def __init__(self, *, task='Pendulum-v0', hidden, pop_size, runs, theta0, sigma, learning_rate, weight_decay=0.005,
+                 repetitions=10, horizon=None, action_noise_std=0.0, normalize_obs=True, clip=None, seed=0, beta1=0.9,
+                 beta2=0.999, epsilon=1e-8, use_graph=True, kernels=None, device=None):
+        from . import ops_runs
+        self.k, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
+        if self.k is ops_runs and self.device.type != 'cuda':
+            raise RuntimeError('distributedes_b200 needs a CUDA device, got %s: there is no CPU fallback' % self.device)
+        self.R, self.N = int(runs), int(pop_size)
+        if self.R < 1:
+            raise ValueError('runs must be >= 1; got %r' % (runs,))
+        if not 2 <= self.N <= self.MAX_RUN_SIZE:
+            raise ValueError('RolloutRunsEngine: pop_size must be in [2, %d] (runs are batched up to the counting rank\'s '
+                             'population; a larger one fills the GPU alone); got %d' % (self.MAX_RUN_SIZE, self.N))
+        if self.R * self.N > 1 << 28:
+            raise ValueError('RolloutRunsEngine: runs x pop_size = %d members, past 2^28' % (self.R * self.N))
+        # the source describes the environment and its limits; its kernels are never called
+        src = DeviceRollouts(self.k, self.device, task=task, hidden=hidden, repetitions=repetitions, horizon=horizon,
+                             clip=clip, action_noise_std=action_noise_std, seed=seed, normalize_obs=normalize_obs,
+                             sigma=float(sigma), mirrored=False)
+        self.d0, self.H, self.A, self.clip = src.d0, src.H, src.A, src.clip
+        self.repetitions, self.test_repetitions, self.horizon = src.repetitions, src.test_repetitions, src.horizon
+        self.env_id, self.action_noise_std, self.seed = src.env_id, src.action_noise_std, src.seed
+        self.normalize_obs = src.normalize_obs
+        self.sigma, self.lr, self.wd = float(sigma), float(learning_rate), float(weight_decay)
+        self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
+        self.P = self.k.param_count(self.d0, self.H, self.A)
+        theta0 = np.ascontiguousarray(theta0, dtype=np.float32)
+        if theta0.size == self.P:
+            theta0 = np.tile(theta0.reshape(1, -1), (self.R, 1))
+        elif theta0.size != self.R * self.P:
+            raise ValueError('theta0 has %d entries; the (%d,%d,%d) MLP needs %d, or %d x %d for one start point per run'
+                             % (theta0.size, self.d0, self.H, self.A, self.P, self.R, self.P))
+        dev, R, N, P, w = self.device, self.R, self.N, self.P, 2 * self.d0 + 1
+        self.theta = torch.from_numpy(theta0.reshape(R, P).copy()).to(dev)
+        self.adam_m = torch.zeros((R, P), dtype=torch.float64, device=dev)
+        self.adam_v = torch.zeros((R, P), dtype=torch.float64, device=dev)
+        self.fitness_all = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.shaped = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.partial = torch.zeros((R, P), dtype=torch.float32, device=dev)
+        self.update = torch.zeros((R, P), dtype=torch.float32, device=dev)
+        self.obs_stats = torch.zeros((R, w), dtype=torch.float32, device=dev) if self.normalize_obs else None
+        self.obs_totals = torch.zeros((R, w), dtype=torch.float64, device=dev)
+        self.roll_ws = torch.empty(R * N * w, dtype=torch.float64, device=dev)
+        self.test_fitness = torch.empty((R, 1), dtype=torch.float32, device=dev)
+        self.state = self.k.new_state(dev, 0)
+        self.rank_ws = self.k.rank_runs_workspace(R, N, dev)
+        self.grad_ws = self.k.grad_runs_workspace(R, N, P, dev)
+        self.generation_index = 0
+        self.steps_taken = N * self.repetitions * self.horizon      # per run (natural_es.py:75)
+        self._graph = None
+        self._use_graph = bool(use_graph) and dev.type == 'cuda'
+
+    def _env(self):
+        return dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip,
+                    action_noise_std=self.action_noise_std, seed=self.seed)
+
+    def evaluate(self):
+        self.k.rollout_eval_runs(self.theta, repetitions=self.repetitions, sigma=self.sigma, state=self.state,
+                                 run_size=self.N, obs_stats=self.obs_stats,
+                                 totals_out=self.obs_totals if self.normalize_obs else None, workspace=self.roll_ws,
+                                 out=self.fitness_all, **self._env())
+        return self.fitness_all
+
+    def rank_and_reduce(self):
+        self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
+        self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
+                                     out=self.partial)
+        return self.partial
+
+    def apply(self):
+        self.k.nes_apply_runs(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state, sigma=self.sigma,
+                              learning_rate=self.lr, weight_decay=self.wd, beta1=self.beta1, beta2=self.beta2,
+                              epsilon=self.epsilon, update_out=self.update)
+        self.k.state_advance(self.state, self.beta1, self.beta2)
+        if self.normalize_obs:    # natural_es.py:85-89, each run's observations into its own statistics
+            self.k.obs_stats_merge_totals_runs(self.obs_stats, self.obs_totals, self.d0)
+
+    def _generation_eager(self):
+        self.evaluate()
+        self.rank_and_reduce()
+        self.apply()
+
+    def generation(self):
+        """One generation of every run, device-resident (a replayed CUDA graph on the GPU); read .fitness_all / .theta."""
+        if self._use_graph:
+            if self._graph is None:
+                live = [self.theta, self.adam_m, self.adam_v, self.state] + ([self.obs_stats] if self.normalize_obs else [])
+                self._graph = capture_generation(self.device, live, self._generation_eager)
+            self._graph.replay()
+        else:
+            self._generation_eager()
+        self.generation_index += 1
+
+    def test_returns(self, repetitions=None):
+        """[R, repetitions] fp64 returns of noiseless test episodes of every run's theta with its own statistics, from
+        one launch: run r's are RolloutEngine.test_returns of theta[r] (the same resets and generation word)."""
+        reps = int(repetitions or self.test_repetitions)
+        episodes = torch.empty((self.R, 1, reps), dtype=torch.float32, device=self.device)
+        self.k.rollout_eval_runs(self.theta, repetitions=reps, sigma=0.0, state=self.state, run_size=1, noiseless=True,
+                                 obs_stats=self.obs_stats, out=self.test_fitness, episodes_out=episodes, **self._env())
+        return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
+
+    def theta_numpy(self):
+        return self.theta.detach().cpu().numpy()

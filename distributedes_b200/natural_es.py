@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .engine import NESEngine, kernels_and_device
+from .engine import NESEngine, RolloutRunsEngine, kernels_and_device
 from .fitness import from_config
 from .utils import Evaluator, SharedStats, StaticNormalizer, logger
 
@@ -90,6 +90,73 @@ def train(config, engine=None):
     return [training_rewards, training_steps, training_timestamps]
 
 
+def check_runs_config(config):
+    """Raises ValueError unless train_runs can batch runs of `config`: a closed-loop device environment
+    (ClosedLoopPendulumConfig), plain sampling, at most 2048 members, one process."""
+    if getattr(config, 'host_env', False):
+        raise ValueError('train_runs: host-stepped environments are not batched over runs (the device batches its own '
+                         'closed-loop environments only: ClosedLoopPendulumConfig); use train()')
+    if not getattr(config, 'closed_loop', False):
+        raise ValueError('train_runs: tape configs are not batched over runs (the device batches its own closed-loop '
+                         'environments only: ClosedLoopPendulumConfig); use train()')
+    if config.mirrored:
+        raise ValueError('train_runs: mirrored sampling is not batched over runs; use train()')
+    if int(config.pop_size) > RolloutRunsEngine.MAX_RUN_SIZE:
+        raise ValueError('train_runs: pop_size %d > %d: runs are batched up to %d members (a larger population fills the '
+                         'GPU alone); use train()' % (config.pop_size, RolloutRunsEngine.MAX_RUN_SIZE,
+                                                      RolloutRunsEngine.MAX_RUN_SIZE))
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError('train_runs: a batch of runs trains on one GPU; the process group has world size %d'
+                         % dist.get_world_size())
+
+
+def build_runs_engine(config, runs, *, kernels=None, device=None, **kw):
+    """The RolloutRunsEngine of `runs` runs of a config that check_runs_config accepts, every run starting from
+    config.initial_weight (as the reference's multi_runs does).  `kw` goes to RolloutRunsEngine (use_graph)."""
+    check_runs_config(config)
+    return RolloutRunsEngine(task=config.task, hidden=config.hidden_size, pop_size=config.pop_size, runs=runs,
+                             theta0=config.initial_weight, sigma=config.sigma, learning_rate=config.learning_rate,
+                             weight_decay=config.weight_decay, repetitions=config.repetitions, clip=config.clip,
+                             action_noise_std=config.action_noise_std, normalize_obs=config.normalize_obs,
+                             seed=config.seed, beta1=config.opt.beta1, beta2=config.opt.beta2,
+                             epsilon=config.opt.epsilon, kernels=kernels, device=device, **kw)
+
+
+def train_runs(config, runs, engine=None):
+    """`runs` independent train(config) runs trained together on one GPU (engine.RolloutRunsEngine): a list of `runs`
+    [training_rewards, training_steps, training_timestamps] triples.  Run 0 is train(config), bit for bit; runs 1.. draw
+    further independent streams of config.seed (not the runs of other seeds).  The runs share one clock, so they share
+    steps and timestamps.  ClosedLoopPendulumConfig only (see check_runs_config)."""
+    check_runs_config(config)
+    engine = engine if engine is not None else build_runs_engine(config, runs)
+    R = engine.R
+    rewards, steps, timestamps = [[] for _ in range(R)], [], []
+    initial_time = time.time()
+    total_steps = 0
+    iteration = 0
+    while True:
+        returns = engine.test_returns(config.test_repetitions)                 # [R, repetitions], one launch
+        elapsed_time = time.time() - initial_time
+        for r in range(R):
+            rewards[r].append(np.mean(returns[r]))                             # test(), natural_es.py:101-110
+        steps.append(total_steps)
+        timestamps.append(elapsed_time)
+        logger.info('Test: total steps %d, mean over %d runs %f, elapsed time %d'
+                    % (total_steps, R, float(np.mean([rw[-1] for rw in rewards])), elapsed_time))
+        fitness = engine.evaluate()
+        total_steps += engine.steps_taken
+        logger.info('Train: iteration %d, mean fitness over %d runs %f' % (iteration, R, float(fitness.mean())))
+        iteration += 1
+        if config.max_steps and total_steps > config.max_steps:
+            break
+        if getattr(config, 'max_generations', 0) and iteration > config.max_generations:
+            break
+        engine.rank_and_reduce()
+        engine.apply()
+        engine.generation_index += 1
+    return [[rewards[r], list(steps), list(timestamps)] for r in range(R)]
+
+
 def test(config, solution, stats, engine=None):
     """natural_es.py:101-110: mean and 'ste' of test_repetitions noiseless episodes of `solution`
     (None = the engine's current parameters)."""
@@ -143,22 +210,32 @@ def launch(config_fn, world_size, port=None):
 
 
 # ---- run bookkeeping (natural_es.py:113-124; SURVEY 8f row 4) ----------------------------------------------------------
-def multi_runs(config, runs=10, log_dir='log', data_dir='data'):
+def multi_runs(config, runs=10, log_dir='log', data_dir='data', batched=False):
     """natural_es.py:113-124: `runs` sequential train() runs, a per-task log file and the pickle of
     [[rewards, steps, timestamps], ...] rewritten after every run — same file names and on-disk format as the reference
     (its plotting scripts read data/<tag>-stats-<task>.bin).  Unlike the reference the directories are created, and the
-    optimiser state does not leak from one run to the next (natural_es.py:120-122 reuses config.opt)."""
+    optimiser state does not leak from one run to the next (natural_es.py:120-122 reuses config.opt).
+    batched=True trains the runs together through train_runs (ClosedLoopPendulumConfig only) and writes the same files
+    once: run 0 is the first sequential run, the others are independent streams of the same seed."""
     os.makedirs(log_dir, exist_ok=True)
     os.makedirs(data_dir, exist_ok=True)
+    if batched:
+        check_runs_config(config)
     fh = logging.FileHandler(os.path.join(log_dir, '%s-%s.txt' % (config.tag, config.task)))
     fh.setLevel(logging.DEBUG)
     logger.addHandler(fh)
     stats = []
+    path = os.path.join(data_dir, '%s-stats-%s.bin' % (config.tag, config.task))
     try:
-        for run in range(runs):
+        if batched:
+            logger.info('Runs 0-%d, batched' % (runs - 1))
+            stats = train_runs(config, runs)
+            with open(path, 'wb') as f:
+                pickle.dump(stats, f)
+        for run in range(0 if batched else runs):
             logger.info('Run %d' % (run))
             stats.append(train(config))
-            with open(os.path.join(data_dir, '%s-stats-%s.bin' % (config.tag, config.task)), 'wb') as f:
+            with open(path, 'wb') as f:
                 pickle.dump(stats, f)
     finally:
         logger.removeHandler(fh)

@@ -177,6 +177,48 @@ DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_re
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
 DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim, void *stream);
 
+/* ---- batches of independent runs: many small populations trained together on one device ------------------------
+ *
+ * A batch holds n_runs runs of run_size members that share the seed, the generation word (state_dev or `generation`) and
+ * the hyper-parameters.  Run r's member i is the global member r * run_size + i: its eps (stream 0), resets (stream 2)
+ * and action noise (stream 3) are those of member_offset = r * run_size in the single-population entry points, so run 0
+ * is the population those entry points evaluate alone, and runs 1.. are further independent streams of the same seed.
+ * Per-run arrays are row-major with one row per run: theta, Adam's m and v, partial sums [n_runs][P], fitness and shaped
+ * fitness [n_runs][run_size], statistics and observation totals [n_runs][2*state_dim+1].  Each entry point equals, for
+ * every run r, the single-population call named beside it, bit for bit.  1 <= run_size <= 2048 (2 for the rank) and
+ * n_runs * run_size <= 2^28; run_size above 2048 is DES_ERR_UNSUPPORTED (such a population fills the GPU alone).
+ * n_runs == 0 does nothing and accepts NULL pointers.
+ *
+ * des_rollout_eval_runs        des_rollout_eval(theta_r, obs_stats_r, member_offset = r * run_size, n_local = run_size)
+ *                              with outputs fitness [n_runs][run_size], episode returns [n_runs][run_size][repetitions]
+ *                              and observation totals [n_runs][2*state_dim+1] (workspace: n_runs * run_size *
+ *                              (2*state_dim+1) * 8 bytes).  noiseless != 0 needs run_size == 1: run r's test episodes are
+ *                              des_rollout_eval(noiseless) of theta_r at member_offset r (the reset member 0x40000000 of
+ *                              every test episode; with action noise on, run r draws member r's).
+ * des_centered_rank_runs       des_centered_rank(fitness_r, run_size, 0, run_size): ranks within each run.
+ * des_nes_grad_partial_runs    des_nes_grad_partial(shaped_r, run_size, P, member_offset = r * run_size), sliced as that call
+ *                              slices one run.
+ * des_nes_apply_runs           des_nes_apply(theta_r, m_r, v_r, update_r, grad_r, partial_r, P, N = run_size); Adam's t and
+ *                              beta^t of state_dev are shared (advance them once per generation).
+ * des_obs_stats_merge_totals_runs   des_obs_stats_merge_totals(stats_r, totals_r). */
+DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                  const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                  int32_t repetitions, double sigma, double clip, double action_noise_std, uint64_t seed,
+                                  uint64_t generation, const des_state *state_dev, int64_t n_runs, int64_t run_size,
+                                  int noiseless, void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API size_t des_rank_runs_workspace_bytes(int64_t n_runs, int64_t run_size);
+DES_API int des_centered_rank_runs(float *shaped_out_dev, int32_t *rank_out_dev, const float *fitness_dev, int64_t n_runs,
+                                   int64_t run_size, void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API size_t des_grad_runs_workspace_bytes(int64_t n_runs, int64_t run_size, int64_t P);
+DES_API int des_nes_grad_partial_runs(float *partial_out_dev, const float *shaped_dev, int64_t n_runs, int64_t run_size,
+                                      int64_t P, uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                      void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API int des_nes_apply_runs(float *theta_dev, double *adam_m_dev, double *adam_v_dev, float *update_out_dev,
+                               double *grad_out_dev, const float *partial_sum_dev, int64_t P, int64_t n_runs,
+                               int64_t run_size, des_opt opt, const des_state *state_dev, void *stream);
+DES_API int des_obs_stats_merge_totals_runs(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,
+                                            int64_t n_runs, void *stream);
+
 /* ---- environments stepped on the host: the population's policy step on the device ------------------------------ */
 
 /* One environment step of n_local members x `repetitions` episodes whose environments the caller steps on the host:
