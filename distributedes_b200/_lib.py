@@ -31,6 +31,12 @@ class State(C.Structure):
     _fields_ = [('generation', C.c_uint64), ('adam_t', C.c_uint64), ('beta1_t', C.c_double), ('beta2_t', C.c_double)]
 
 
+class RunHp(C.Structure):
+    """des_run_hp: one run's row of a sweep's table (40 bytes, kept in device memory)."""
+    _fields_ = [('seed', C.c_uint64), ('sigma', C.c_double), ('learning_rate', C.c_double),
+                ('weight_decay', C.c_double), ('action_noise_std', C.c_double)]
+
+
 _P, _I64, _U64, _U32, _I32, _D, _SZ = C.c_void_p, C.c_int64, C.c_uint64, C.c_uint32, C.c_int32, C.c_double, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol include/des_b200.h declares (tests check this)
@@ -59,6 +65,10 @@ SIGNATURES = {
     'des_nes_grad_partial_runs': (C.c_int, [_P, _P, _I64, _I64, _I64, _U64, _U64, _P, _P, _SZ, _P]),
     'des_nes_apply_runs': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, Opt, _P, _P]),
     'des_obs_stats_merge_totals_runs': (C.c_int, [_P, _P, _I32, _I64, _P]),
+    'des_rollout_eval_sweep': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _P, _U64, _P, _I64, _I64, C.c_int, _P,
+                                         C.c_size_t, _P]),
+    'des_nes_grad_partial_sweep': (C.c_int, [_P, _P, _I64, _I64, _I64, _P, _U64, _P, _P, _SZ, _P]),
+    'des_nes_apply_sweep': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _P, _D, _D, _D, _P, _P]),
     'des_policy_act': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _I64, _P]),
     'des_obs_parts_reduce': (C.c_int, [_P, _P, _I64, _I32, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),

@@ -250,6 +250,18 @@ int not_whole_pairs(const char *who, const char *count, int64_t member_offset, i
 // index below 2^28 (DES_ERR_INVALID_ARGUMENT).
 constexpr int64_t kRunMaxSize = 2048;
 int check_runs(const char *who, int64_t n_runs, int64_t run_size, int64_t min_size);
+// A sweep's per-run table (the *_sweep entry points) as the header lays it out; ctypes mirrors it (_lib.RunHp).
+static_assert(sizeof(des_run_hp) == 40 && offsetof(des_run_hp, sigma) == 8 && offsetof(des_run_hp, learning_rate) == 16 &&
+              offsetof(des_run_hp, weight_decay) == 24 && offsetof(des_run_hp, action_noise_std) == 32,
+              "des_run_hp: 40 bytes, the header's field offsets");
+// The round keys of make_philox_key(seed), computed where the seed is: a sweep's kernels read it from their run's table.
+__device__ __forceinline__ void philox_round_keys(uint64_t seed, PhiloxKey &k) {
+#pragma unroll
+    for (int r = 0; r < kPhiloxRounds; ++r) {
+        k.k0[r] = (uint32_t)seed + (uint32_t)r * kPhiloxW0;
+        k.k1[r] = (uint32_t)(seed >> 32) + (uint32_t)r * kPhiloxW1;
+    }
+}
 // Hidden widths of the closed-loop policy kernels (rollout_pendulum_kernel, policy_act_kernel): H/16 units per lane.
 inline bool policy_width_ok(int H) { return H == 16 || H == 32 || H == 64 || H == 96 || H == 128; }
 

@@ -41,6 +41,20 @@ struct RunArgs : RollArgs {
     int run_size;                      // members per run
 };
 
+// The arguments of a sweep (des_rollout_eval_sweep): a batch of runs whose seed, sigma and action noise are run r's row
+// of the device table hp.  The key, sigma and act_noise of the RollArgs part are unused: each CTA sets them from its row.
+struct SweepArgs : RunArgs {
+    const des_run_hp *hp;              // [n_runs]
+};
+
+// The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
+// except in a sweep, where every run is a population of its own.
+template <typename Args>
+__device__ __forceinline__ unsigned member_slot(const Args &a) {
+    if constexpr (std::is_same<Args, SweepArgs>::value) return blockIdx.x % (unsigned)a.run_size;
+    else return blockIdx.x;
+}
+
 __device__ __forceinline__ double unit_open(uint32_t x) { return ((double)(x & 0x7FFFFFu) + 0.5) * (1.0 / 8388608.0); }
 
 // gym Pendulum-v0 (gym/envs/classic_control/pendulum.py): g = 10, m = l = 1, dt = 0.05, max_speed 8, max_torque 2
@@ -82,13 +96,21 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // kRows: the weights are row blockIdx.x of a.rows (no noise is generated); otherwise theta + sigma*eps of the member.
 // Args = RunArgs: a batch of independent runs (des_rollout_eval_runs, member_offset 0): CTA b is member b % run_size of
 // run b / run_size, global member b, with its run's row of theta and of the statistics.  Everything else is the same code.
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs or RunArgs
+// Args = SweepArgs: a sweep (des_rollout_eval_sweep): as RunArgs, but CTA b is member b % run_size of a standalone
+// population under its run's seed, with the run's sigma and action noise; the round keys are set up from that seed.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs or SweepArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
-    if constexpr (std::is_same<Args, RunArgs>::value) {
+    if constexpr (std::is_base_of<RunArgs, Args>::value) {
         const unsigned run = blockIdx.x / (unsigned)a.run_size;
         a.theta += (size_t)run * a.L.P;
         if (a.obs_stats) a.obs_stats += (size_t)run * 7;
+        if constexpr (std::is_same<Args, SweepArgs>::value) {
+            const des_run_hp hp = a.hp[run];
+            philox_round_keys(hp.seed, a.key);                  // make_philox_key's words, as the host makes them
+            a.sigma = a.noiseless ? 0.f : (float)hp.sigma;      // the host's conversions of the single call
+            a.act_noise = (float)hp.action_noise_std;
+        }
     }
     extern __shared__ __align__(16) float sm[];
     float *W2T = sm;                     // [k][j] = W2[j][k]
@@ -105,7 +127,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     const Layout L = a.L;
     const int lane = threadIdx.x, rg = lane >> 1, eg = lane & 1;
     const uint32_t gen = generation_word(a.state, a.gen);
-    const uint32_t member = (uint32_t)(a.member_offset + blockIdx.x);
+    const uint32_t member = (uint32_t)(a.member_offset + member_slot(a));
 
     // flat parameter j of the member -> its place in shared memory
     auto stage = [&](int j, float w) {
@@ -156,7 +178,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     const int csel = rg % C, ep = C * eg + csel;         // the episode whose dynamics this lane carries
     const bool writer = rg < C;                           // one lane per episode publishes
     Pendulum env;
-    env.reset((uint32_t)ep, a.reset_member_base + (a.noiseless ? 0u : (uint32_t)blockIdx.x), gen, a.key);
+    env.reset((uint32_t)ep, a.reset_member_base + (a.noiseless ? 0u : (uint32_t)member_slot(a)), gen, a.key);
     double total = 0.0, osum[3] = {0, 0, 0}, osq[3] = {0, 0, 0};
     for (int t = 0; t < a.horizon; ++t) {
         {
@@ -273,13 +295,15 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
 // Shared by the entry points: argument checks (before any CUDA work), workspace, launch.  rows_mode selects the
 // explicit-solution kernels: `weights` is then rows[n_local][P] instead of the theta that sigma*eps perturbs.  run_size > 0
 // makes the n_local members a batch of runs of run_size (des_rollout_eval_runs, member_offset 0): `weights` and
-// `obs_stats_dev` hold one row per run, and the observation totals are reduced per run.
+// `obs_stats_dev` hold one row per run, and the observation totals are reduced per run.  A table hp_dev makes that batch a
+// sweep (des_rollout_eval_sweep): seed, sigma and action_noise_std are then each run's row of the table.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                           double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
-                          void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size, cudaStream_t st) {
+                          void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
+                          const des_run_hp *hp_dev, cudaStream_t st) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -319,6 +343,22 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
         RunArgs ra;
         static_cast<RollArgs &>(ra) = a;
         ra.run_size = (int)run_size;
+        if (hp_dev) {
+            SweepArgs sa;
+            static_cast<RunArgs &>(sa) = ra;
+            sa.hp = hp_dev;
+            void (*sweep_kernel)(SweepArgs);
+            switch (H / 16) {
+                case 1: sweep_kernel = rollout_pendulum_kernel<1, false, SweepArgs>; break;
+                case 2: sweep_kernel = rollout_pendulum_kernel<2, false, SweepArgs>; break;
+                case 4: sweep_kernel = rollout_pendulum_kernel<4, false, SweepArgs>; break;
+                case 6: sweep_kernel = rollout_pendulum_kernel<6, false, SweepArgs>; break;
+                default: sweep_kernel = rollout_pendulum_kernel<8, false, SweepArgs>; break;
+            }
+            const int rc = launch_smem("rollout_pendulum_kernel", sweep_kernel, (unsigned)n_local, 32, smem, st, sa);
+            if (rc != DES_OK || !obs_totals_out_dev) return rc;
+            return obs_parts_reduce_runs(obs_totals_out_dev, a.stat_part, n_local / run_size, run_size, 7, st);
+        }
         void (*runs_kernel)(RunArgs);
         switch (H / 16) {
             case 1: runs_kernel = rollout_pendulum_kernel<1, false, RunArgs>; break;
@@ -356,7 +396,7 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     return des::rollout_launch("des_rollout_eval", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               false, 0, (cudaStream_t)stream);
+                               false, 0, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -369,7 +409,7 @@ extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *
     return des::rollout_launch("des_rollout_eval_mirrored", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                theta_dev, false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               true, 0, (cudaStream_t)stream);
+                               true, 0, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -381,7 +421,7 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
     return des::rollout_launch("des_rollout_eval_solutions", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
-                               false, 0, (cudaStream_t)stream);
+                               false, 0, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -398,5 +438,23 @@ extern "C" DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *epis
     return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
                                obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
                                state_dev, 0, n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size,
+                               nullptr, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
+                                              double *obs_totals_out_dev, const float *theta_dev, const float *obs_stats_dev,
+                                              int env, des_dims dims, int32_t repetitions, double clip,
+                                              const des_run_hp *hp_dev, uint64_t generation, const des_state *state_dev,
+                                              int64_t n_runs, int64_t run_size, int noiseless, void *workspace_dev,
+                                              size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_sweep";
+    const int rc = des::check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(!noiseless || run_size == 1, "%s: test episodes (noiseless) evaluate one theta per run: run_size must be 1 "
+                "(got %lld)", who, (long long)run_size);
+    DES_REQUIRE(n_runs == 0 || hp_dev, "%s: NULL pointer", who);
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
+                               obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, state_dev, 0,
+                               n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size, hp_dev,
                                (cudaStream_t)stream);
 }

@@ -51,24 +51,15 @@ __host__ inline GradPlan grad_plan(int64_t n_local, int64_t P) {
     return p;
 }
 
+// Quad q of slice blockIdx.y of a shard: ws[blockIdx.y][4q..4q+3] = sum over the slice's members i of s_i * eps_i.
 // kMirror: i runs over the n_local pairs of a mirrored shard, member_offset is the pair index of its first pair, and
-// pair i contributes (s_2i - s_2i+1) * eps_i: sum_m s_m eps_m with eps_2i+1 = -eps_2i, half the normals to regenerate
-// kRuns: CTA row z takes run z of a batch (des_nes_grad_partial_runs), a shard of n_local members at member_offset +
-// z * n_local whose gridDim.y slices have their own rows of ws.
-template <bool kMirror, bool kRuns>
-__global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restrict__ ws, const float *__restrict__ shaped,
-                                                                   int64_t n_local, int64_t nq, int64_t Ppad,
-                                                                   int64_t per_chunk, PhiloxKey key,
-                                                                   uint32_t gen_arg, const des_state *state,
-                                                                   uint64_t member_offset) {
-    const int64_t q = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
-    if (q >= nq) return;
-    if constexpr (kRuns) {
-        ws += (int64_t)blockIdx.z * gridDim.y * Ppad;
-        shaped += (int64_t)blockIdx.z * n_local;
-        member_offset += (uint64_t)blockIdx.z * n_local;
-    }
-    const uint32_t gen = generation_word(state, gen_arg);
+// pair i contributes (s_2i - s_2i+1) * eps_i: sum_m s_m eps_m with eps_2i+1 = -eps_2i, half the normals to regenerate.
+// member_offset is taken by reference: passed by value, ptxas scheduled grad_chunk_kernel<false, true>'s loop differently
+// from the kernel it was before this body moved here.
+template <bool kMirror>
+__device__ __forceinline__ void grad_chunk(float *__restrict__ ws, const float *__restrict__ shaped, int64_t n_local,
+                                           int64_t q, int64_t Ppad, int64_t per_chunk, const PhiloxKey &key, uint32_t gen,
+                                           const uint64_t &member_offset) {   // a reference: see below
     const int64_t i0 = (int64_t)blockIdx.y * per_chunk;
     const int64_t i1 = min(n_local, i0 + per_chunk);
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -86,6 +77,43 @@ __global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restr
         acc.w = __fmaf_rn(bs, b.s, acc.w);
     }
     *reinterpret_cast<float4 *>(ws + (int64_t)blockIdx.y * Ppad + 4 * q) = acc;
+}
+
+// kRuns: CTA row z takes run z of a batch (des_nes_grad_partial_runs), a shard of n_local members at member_offset +
+// z * n_local whose gridDim.y slices have their own rows of ws.
+template <bool kMirror, bool kRuns>
+__global__ void __launch_bounds__(kGradThreads) grad_chunk_kernel(float *__restrict__ ws, const float *__restrict__ shaped,
+                                                                   int64_t n_local, int64_t nq, int64_t Ppad,
+                                                                   int64_t per_chunk, PhiloxKey key,
+                                                                   uint32_t gen_arg, const des_state *state,
+                                                                   uint64_t member_offset) {
+    const int64_t q = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
+    if (q >= nq) return;
+    if constexpr (kRuns) {
+        ws += (int64_t)blockIdx.z * gridDim.y * Ppad;
+        shaped += (int64_t)blockIdx.z * n_local;
+        member_offset += (uint64_t)blockIdx.z * n_local;
+    }
+    const uint32_t gen = generation_word(state, gen_arg);
+    grad_chunk<kMirror>(ws, shaped, n_local, q, Ppad, per_chunk, key, gen, member_offset);
+}
+
+// A sweep (des_nes_grad_partial_sweep): CTA row z takes run z, a standalone shard of n_local members (member_offset 0)
+// under its own seed hp[z].seed, with grad_chunk_kernel<false, true>'s ws rows.  The round keys live in registers, set
+// up from the seed; `one` is PhiloxKey::one_bits, a parameter so that it stays a register operand.
+__global__ void __launch_bounds__(kGradThreads) grad_chunk_sweep_kernel(float *__restrict__ ws,
+                                                                         const float *__restrict__ shaped, int64_t n_local,
+                                                                         int64_t nq, int64_t Ppad, int64_t per_chunk,
+                                                                         const des_run_hp *__restrict__ hp, uint32_t one,
+                                                                         uint32_t gen_arg, const des_state *state) {
+    const int64_t q = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
+    if (q >= nq) return;
+    ws += (int64_t)blockIdx.z * gridDim.y * Ppad;
+    shaped += (int64_t)blockIdx.z * n_local;
+    PhiloxKey key;
+    philox_round_keys(hp[blockIdx.z].seed, key);
+    key.one_bits = one;
+    grad_chunk<false>(ws, shaped, n_local, q, Ppad, per_chunk, key, generation_word(state, gen_arg), 0);
 }
 
 // partial[j] = fp32( sum_c ws[c][j] ) with the cross-chunk sum in fp64, fixed order (deterministic): a CTA of 32 x 8
@@ -168,6 +196,22 @@ __global__ void apply_runs_kernel(float *__restrict__ theta, double *__restrict_
     if (j >= P) return;
     for (int64_t r = blockIdx.y; r < n_runs; r += gridDim.y) {
         const int64_t o_r = r * P;
+        apply_at(j, theta + o_r, am + o_r, av + o_r, update_out ? update_out + o_r : nullptr,
+                 grad_out ? grad_out + o_r : nullptr, partial + o_r, N, o, state);
+    }
+}
+
+// run r's rows of every [n_runs][P] argument, with the optimiser of run r's row of the table and the shared beta / epsilon
+__global__ void apply_sweep_kernel(float *__restrict__ theta, double *__restrict__ am, double *__restrict__ av,
+                                   float *__restrict__ update_out, double *__restrict__ grad_out,
+                                   const float *__restrict__ partial, int64_t P, int64_t n_runs, int64_t N,
+                                   const des_run_hp *__restrict__ hp, double beta1, double beta2, double epsilon,
+                                   const des_state *__restrict__ state) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= P) return;
+    for (int64_t r = blockIdx.y; r < n_runs; r += gridDim.y) {
+        const int64_t o_r = r * P;
+        const des_opt o = {hp[r].sigma, hp[r].learning_rate, hp[r].weight_decay, beta1, beta2, epsilon};
         apply_at(j, theta + o_r, am + o_r, av + o_r, update_out ? update_out + o_r : nullptr,
                  grad_out ? grad_out + o_r : nullptr, partial + o_r, N, o, state);
     }
@@ -342,5 +386,60 @@ extern "C" DES_API int des_nes_apply_runs(float *theta_dev, double *adam_m_dev, 
         theta_dev, adam_m_dev, adam_v_dev, update_out_dev, grad_out_dev, partial_sum_dev, P, n_runs, run_size, opt,
         state_dev);
     DES_LAUNCH_CHECK("apply_runs_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API int des_nes_grad_partial_sweep(float *partial_out_dev, const float *shaped_dev, int64_t n_runs,
+                                                  int64_t run_size, int64_t P, const des_run_hp *hp_dev, uint64_t generation,
+                                                  const des_state *state_dev, void *workspace_dev, size_t workspace_bytes,
+                                                  void *stream) {
+    using namespace des;
+    const char *who = "des_nes_grad_partial_sweep";
+    const int rc = check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(P > 0, "%s: bad size P=%lld", who, (long long)P);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(partial_out_dev && shaped_dev && hp_dev, "%s: NULL pointer", who);
+    const GradPlan p = grad_plan(run_size, P);           // each run sliced as a shard of run_size members
+    const size_t need = des_grad_runs_workspace_bytes(n_runs, run_size, P);
+    if (!workspace_dev || workspace_bytes < need) {
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
+    DES_REQUIRE(((uintptr_t)workspace_dev & 15) == 0, "%s: workspace must be 16-byte aligned", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    float *ws = (float *)workspace_dev;
+    const unsigned bx = (unsigned)((p.nq + kGradThreads - 1) / kGradThreads);
+    const uint32_t one = make_philox_key(0).one_bits;
+    for (int64_t r0 = 0; r0 < n_runs; r0 += 65535) {            // grid z: up to 65535 runs per launch
+        const int64_t nr = n_runs - r0 < 65535 ? n_runs - r0 : 65535;
+        grad_chunk_sweep_kernel<<<dim3(bx, (unsigned)p.chunks, (unsigned)nr), kGradThreads, 0, st>>>(
+            ws + r0 * p.chunks * p.Ppad, shaped_dev + r0 * run_size, run_size, p.nq, p.Ppad, p.per_chunk, hp_dev + r0, one,
+            (uint32_t)generation, state_dev);
+        DES_LAUNCH_CHECK("grad_chunk_sweep_kernel");
+    }
+    const unsigned bz = (unsigned)(n_runs < 65535 ? n_runs : 65535);
+    grad_reduce_runs_kernel<<<dim3((unsigned)((P + 31) / 32), bz), dim3(32, kReduceRows), 0, st>>>(partial_out_dev, ws,
+                                                                                                 n_runs, P, p.Ppad, p.chunks);
+    DES_LAUNCH_CHECK("grad_reduce_runs_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API int des_nes_apply_sweep(float *theta_dev, double *adam_m_dev, double *adam_v_dev, float *update_out_dev,
+                                           double *grad_out_dev, const float *partial_sum_dev, int64_t P, int64_t n_runs,
+                                           int64_t run_size, const des_run_hp *hp_dev, double beta1, double beta2,
+                                           double epsilon, const des_state *state_dev, void *stream) {
+    using namespace des;
+    const char *who = "des_nes_apply_sweep";
+    const int rc = check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(P > 0, "%s: bad size P=%lld", who, (long long)P);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(theta_dev && adam_m_dev && adam_v_dev && partial_sum_dev && hp_dev && state_dev, "%s: NULL pointer", who);
+    const unsigned by = (unsigned)(n_runs < 65535 ? n_runs : 65535);
+    apply_sweep_kernel<<<dim3((unsigned)((P + 255) / 256), by), 256, 0, (cudaStream_t)stream>>>(
+        theta_dev, adam_m_dev, adam_v_dev, update_out_dev, grad_out_dev, partial_sum_dev, P, n_runs, run_size, hp_dev,
+        beta1, beta2, epsilon, state_dev);
+    DES_LAUNCH_CHECK("apply_sweep_kernel");
     return DES_OK;
 }

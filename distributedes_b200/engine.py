@@ -338,13 +338,18 @@ class RolloutRunsEngine:
     its own theta [R, P], fp64 Adam moments, fitness [R, N] and normaliser statistics [R, 2*d0+1]; all runs share the
     des_state (generation word, Adam's t and beta^t), the hyper-parameters and, unless theta0 is [R, P], the start point.
     `kernels` is the module of device ops (default: distributedes_b200.ops_runs); a stand-in runs the host logic on CPU.
-    One GPU; the runs are not sharded."""
+    One GPU; the runs are not sharded.
+
+    `seeds`, a sequence of R seeds, makes the batch a sweep (ops_sweep): run r is then RolloutEngine(seed=seeds[r],
+    sigma=sigma[r], ...), bit for bit, and `sigma`, `learning_rate`, `weight_decay` and `action_noise_std` may each be
+    a scalar or a sequence of R values.  Runs with equal seeds and hyper-parameters are identical.  Without `seeds` the
+    hyper-parameters are scalars: the two contracts do not mix."""
 
     MAX_RUN_SIZE = 2048           # des_*_runs: a larger population fills the GPU without batching
 
     def __init__(self, *, task='Pendulum-v0', hidden, pop_size, runs, theta0, sigma, learning_rate, weight_decay=0.005,
                  repetitions=10, horizon=None, action_noise_std=0.0, normalize_obs=True, clip=None, seed=0, beta1=0.9,
-                 beta2=0.999, epsilon=1e-8, use_graph=True, kernels=None, device=None):
+                 beta2=0.999, epsilon=1e-8, use_graph=True, kernels=None, device=None, seeds=None):
         from . import ops_runs
         self.k, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
         if self.k is ops_runs and self.device.type != 'cuda':
@@ -357,15 +362,42 @@ class RolloutRunsEngine:
                              'population; a larger one fills the GPU alone); got %d' % (self.MAX_RUN_SIZE, self.N))
         if self.R * self.N > 1 << 28:
             raise ValueError('RolloutRunsEngine: runs x pop_size = %d members, past 2^28' % (self.R * self.N))
-        # the source describes the environment and its limits; its kernels are never called
-        src = DeviceRollouts(self.k, self.device, task=task, hidden=hidden, repetitions=repetitions, horizon=horizon,
-                             clip=clip, action_noise_std=action_noise_std, seed=seed, normalize_obs=normalize_obs,
-                             sigma=float(sigma), mirrored=False)
+        hyper = dict(sigma=sigma, learning_rate=learning_rate, weight_decay=weight_decay,
+                     action_noise_std=action_noise_std)
+        if seeds is None:
+            for name, v in hyper.items():
+                if np.ndim(v) > 0:
+                    raise ValueError('RolloutRunsEngine: %s per run needs seeds= (a sweep); a batch of runs without '
+                                     'seeds shares one seed and its hyper-parameters' % name)
+            runs_hyper = [dict(hyper, seed=seed)]
+        else:
+            from .ops_sweep import per_run
+            if np.ndim(seeds) == 0:
+                raise ValueError('RolloutRunsEngine: seeds must be a sequence of one seed per run; got %r' % (seeds,))
+            cols = dict({n: per_run(v, self.R, n) for n, v in hyper.items()}, seed=per_run(seeds, self.R, 'seeds'))
+            runs_hyper = [{n: cols[n][r] for n in cols} for r in range(self.R)]
+            for r, h in enumerate(runs_hyper):
+                if not float(h['sigma']) > 0.0:
+                    raise ValueError('RolloutRunsEngine: sigma must be > 0 (natural_es.py:92 divides by it); run %d has %r'
+                                     % (r, h['sigma']))
+        # the source describes the environment and its limits (one per run of a sweep); its kernels are never called
+        srcs = [DeviceRollouts(self.k, self.device, task=task, hidden=hidden, repetitions=repetitions, horizon=horizon,
+                               clip=clip, action_noise_std=h['action_noise_std'], seed=h['seed'],
+                               normalize_obs=normalize_obs, sigma=float(h['sigma']), mirrored=False) for h in runs_hyper]
+        src = srcs[0]
         self.d0, self.H, self.A, self.clip = src.d0, src.H, src.A, src.clip
         self.repetitions, self.test_repetitions, self.horizon = src.repetitions, src.test_repetitions, src.horizon
-        self.env_id, self.action_noise_std, self.seed = src.env_id, src.action_noise_std, src.seed
-        self.normalize_obs = src.normalize_obs
-        self.sigma, self.lr, self.wd = float(sigma), float(learning_rate), float(weight_decay)
+        self.env_id, self.normalize_obs = src.env_id, src.normalize_obs
+        if seeds is None:
+            self.action_noise_std, self.seed = src.action_noise_std, src.seed
+            self.sigma, self.lr, self.wd = float(sigma), float(learning_rate), float(weight_decay)
+            self.hp = None
+        else:           # lists of R values, and the device table of the sweep ops
+            self.seed, self.action_noise_std = [x.seed for x in srcs], [x.action_noise_std for x in srcs]
+            self.sigma, self.lr, self.wd = ([float(h[n]) for h in runs_hyper]
+                                            for n in ('sigma', 'learning_rate', 'weight_decay'))
+            self.hp = self.k.run_table(self.seed, self.sigma, self.lr, self.wd, self.action_noise_std, self.device,
+                                       runs=self.R)
         self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
         self.P = self.k.param_count(self.d0, self.H, self.A)
         theta0 = np.ascontiguousarray(theta0, dtype=np.float32)
@@ -395,26 +427,40 @@ class RolloutRunsEngine:
         self._use_graph = bool(use_graph) and dev.type == 'cuda'
 
     def _env(self):
-        return dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip,
-                    action_noise_std=self.action_noise_std, seed=self.seed)
+        env = dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip)
+        return env if self.hp is not None else dict(env, action_noise_std=self.action_noise_std, seed=self.seed)
+
+    def _rollout(self, **kw):
+        """rollout_eval_sweep with the table, or rollout_eval_runs with the shared seed and sigma."""
+        if self.hp is not None:
+            kw.pop('sigma')
+            return self.k.rollout_eval_sweep(self.theta, self.hp, **kw, **self._env())
+        return self.k.rollout_eval_runs(self.theta, **kw, **self._env())
 
     def evaluate(self):
-        self.k.rollout_eval_runs(self.theta, repetitions=self.repetitions, sigma=self.sigma, state=self.state,
-                                 run_size=self.N, obs_stats=self.obs_stats,
-                                 totals_out=self.obs_totals if self.normalize_obs else None, workspace=self.roll_ws,
-                                 out=self.fitness_all, **self._env())
+        self._rollout(repetitions=self.repetitions, sigma=self.sigma, state=self.state, run_size=self.N,
+                      obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                      workspace=self.roll_ws, out=self.fitness_all)
         return self.fitness_all
 
     def rank_and_reduce(self):
         self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
-        self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
-                                     out=self.partial)
+        if self.hp is not None:
+            self.k.nes_grad_partial_sweep(self.shaped, self.P, self.hp, state=self.state, workspace=self.grad_ws,
+                                          out=self.partial)
+        else:
+            self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
+                                         out=self.partial)
         return self.partial
 
     def apply(self):
-        self.k.nes_apply_runs(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state, sigma=self.sigma,
-                              learning_rate=self.lr, weight_decay=self.wd, beta1=self.beta1, beta2=self.beta2,
-                              epsilon=self.epsilon, update_out=self.update)
+        if self.hp is not None:
+            self.k.nes_apply_sweep(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state, self.hp,
+                                   beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
+        else:
+            self.k.nes_apply_runs(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state,
+                                  sigma=self.sigma, learning_rate=self.lr, weight_decay=self.wd, beta1=self.beta1,
+                                  beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
         self.k.state_advance(self.state, self.beta1, self.beta2)
         if self.normalize_obs:    # natural_es.py:85-89, each run's observations into its own statistics
             self.k.obs_stats_merge_totals_runs(self.obs_stats, self.obs_totals, self.d0)
@@ -437,11 +483,12 @@ class RolloutRunsEngine:
 
     def test_returns(self, repetitions=None):
         """[R, repetitions] fp64 returns of noiseless test episodes of every run's theta with its own statistics, from
-        one launch: run r's are RolloutEngine.test_returns of theta[r] (the same resets and generation word)."""
+        one launch: run r's are RolloutEngine.test_returns of theta[r] (the same resets and generation word; in a sweep,
+        under run r's seed)."""
         reps = int(repetitions or self.test_repetitions)
         episodes = torch.empty((self.R, 1, reps), dtype=torch.float32, device=self.device)
-        self.k.rollout_eval_runs(self.theta, repetitions=reps, sigma=0.0, state=self.state, run_size=1, noiseless=True,
-                                 obs_stats=self.obs_stats, out=self.test_fitness, episodes_out=episodes, **self._env())
+        self._rollout(repetitions=reps, sigma=0.0, state=self.state, run_size=1, noiseless=True, obs_stats=self.obs_stats,
+                      out=self.test_fitness, episodes_out=episodes)
         return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
 
     def theta_numpy(self):

@@ -157,6 +157,61 @@ def train_runs(config, runs, engine=None):
     return [[rewards[r], list(steps), list(timestamps)] for r in range(R)]
 
 
+# The fields every config of a sweep shares: the runs of one RolloutRunsEngine share its shapes, its stopping rule and
+# Adam's beta and epsilon (beta^t is in the one des_state).  Only seed, sigma, learning_rate, weight_decay,
+# action_noise_std and initial_weight may differ; fields the trainer does not read (tag, ...) are not compared.
+SWEEP_SHARED = ('task', 'hidden_size', 'pop_size', 'repetitions', 'test_repetitions', 'clip', 'normalize_obs',
+                'opt.beta1', 'opt.beta2', 'opt.epsilon', 'max_steps', 'max_generations')
+
+
+def _field(config, name):
+    value = config
+    for part in name.split('.'):
+        value = getattr(value, part, None)
+    return value
+
+
+def check_sweep_configs(configs):
+    """Raises ValueError unless train_sweep can train `configs` as one sweep: each passes check_runs_config, and they
+    agree on every field of SWEEP_SHARED (the first that differs is named)."""
+    if not len(configs):
+        raise ValueError('train_sweep: no configs')
+    for c in configs:
+        check_runs_config(c)
+    for i, c in enumerate(configs[1:], 1):
+        for name in SWEEP_SHARED:
+            a, b = _field(configs[0], name), _field(c, name)
+            if a != b:
+                raise ValueError('train_sweep: configs differ in %s (%r in configs[0], %r in configs[%d]); the runs of a '
+                                 'sweep may differ only in seed, sigma, learning_rate, weight_decay, action_noise_std '
+                                 'and initial_weight' % (name, a, b, i))
+
+
+def build_sweep_engine(configs, *, kernels=None, device=None, **kw):
+    """The RolloutRunsEngine of a sweep: run r is train(configs[r])'s run, with its seed, hyper-parameters and
+    initial_weight.  `kw` goes to RolloutRunsEngine (use_graph)."""
+    check_sweep_configs(configs)
+    c = configs[0]
+    return RolloutRunsEngine(task=c.task, hidden=c.hidden_size, pop_size=c.pop_size, runs=len(configs),
+                             theta0=np.stack([np.asarray(x.initial_weight, dtype=np.float32).reshape(-1) for x in configs]),
+                             seeds=[x.seed for x in configs], sigma=[x.sigma for x in configs],
+                             learning_rate=[x.learning_rate for x in configs],
+                             weight_decay=[x.weight_decay for x in configs],
+                             action_noise_std=[x.action_noise_std for x in configs], repetitions=c.repetitions,
+                             clip=c.clip, normalize_obs=c.normalize_obs, beta1=c.opt.beta1, beta2=c.opt.beta2,
+                             epsilon=c.opt.epsilon, kernels=kernels, device=device, **kw)
+
+
+def train_sweep(configs, engine=None):
+    """train(configs[r]) for every r, trained together on one GPU as one sweep (engine.RolloutRunsEngine with seeds):
+    one [training_rewards, training_steps, training_timestamps] triple per config, whose rewards and steps are those of
+    train(configs[r]).  The runs share one clock, as in train_runs.  The configs may differ only in seed, sigma,
+    learning_rate, weight_decay, action_noise_std and initial_weight (check_sweep_configs)."""
+    check_sweep_configs(configs)
+    engine = engine if engine is not None else build_sweep_engine(configs)
+    return train_runs(configs[0], len(configs), engine=engine)       # its loop reads only the fields the configs share
+
+
 def test(config, solution, stats, engine=None):
     """natural_es.py:101-110: mean and 'ste' of test_repetitions noiseless episodes of `solution`
     (None = the engine's current parameters)."""

@@ -99,3 +99,7 @@ def nes_apply_runs(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learn
             _ptr(grad_out, 'grad_out', F64, R * P, dev, True), _ptr(partial_sum, 'partial_sum', F32, R * P, dev), P, R,
             int(N), Opt(sigma, learning_rate, weight_decay, beta1, beta2, epsilon),
             _ptr(state, 'state', U8, STATE_BYTES, dev))
+
+# The sweep ops (seeds and NES hyper-parameters per run): defined in ops_sweep, listed here so that this module stays the
+# whole set of device ops engine.RolloutRunsEngine calls.
+from .ops_sweep import nes_apply_sweep, nes_grad_partial_sweep, rollout_eval_sweep, run_table  # noqa: E402,F401

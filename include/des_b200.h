@@ -219,6 +219,45 @@ DES_API int des_nes_apply_runs(float *theta_dev, double *adam_m_dev, double *ada
 DES_API int des_obs_stats_merge_totals_runs(float *stats_dev, const double *obs_totals_dev, int32_t state_dim,
                                             int64_t n_runs, void *stream);
 
+/* ---- sweeps: a batch of runs whose seeds and NES hyper-parameters differ per run ------------------------------------
+ *
+ * A sweep is a batch of runs (above: the same shapes, limits, per-run rows and n_runs == 0 rule) in which run r has its
+ * own seed, sigma, learning rate, weight decay and action-noise std, read from hp_dev[r], a table in DEVICE memory.
+ * Run r's member i is member i of a standalone population under hp_dev[r].seed (member_offset 0), not the global
+ * member r * run_size + i: its eps (stream 0), resets (stream 2) and action noise (stream 3) are keyed by run r's seed,
+ * so run r of a sweep is the standalone run of its own seed and hyper-parameters, bit for bit.  Runs with equal entries
+ * are identical.  Shared: the generation word and Adam's t and beta^t (state_dev), the dims, repetitions, horizon, clip
+ * and Adam's beta1, beta2 and epsilon.  The library cannot read the table's values (they are on the device): a sigma
+ * <= 0 is the caller's to refuse.  Ranking and the statistics merge need no table: use des_centered_rank_runs and
+ * des_obs_stats_merge_totals_runs.
+ *
+ * des_rollout_eval_sweep       des_rollout_eval(theta_r, obs_stats_r, seed = s_r, sigma = sigma_r, action_noise_std =
+ *                              a_r, member_offset = 0, n_local = run_size), outputs as des_rollout_eval_runs.
+ *                              noiseless != 0 needs run_size == 1: run r's test episodes under s_r.
+ * des_nes_grad_partial_sweep   des_nes_grad_partial(shaped_r, run_size, P, seed = s_r, member_offset = 0); workspace of
+ *                              des_grad_runs_workspace_bytes.
+ * des_nes_apply_sweep          des_nes_apply(theta_r, m_r, v_r, update_r, grad_r, partial_r, P, N = run_size, opt =
+ *                              {sigma_r, lr_r, wd_r, beta1, beta2, epsilon}); Adam's t and beta^t of state_dev are shared. */
+typedef struct des_run_hp {
+    uint64_t seed;              /* config.seed               offset 0  */
+    double sigma;               /* config.sigma              offset 8  */
+    double learning_rate;       /* config.learning_rate      offset 16 */
+    double weight_decay;        /* config.weight_decay       offset 24 */
+    double action_noise_std;    /* config.action_noise_std   offset 32 */
+} des_run_hp;                   /* 40 bytes */
+DES_API int des_rollout_eval_sweep(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                   const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                   int32_t repetitions, double clip, const des_run_hp *hp_dev, uint64_t generation,
+                                   const des_state *state_dev, int64_t n_runs, int64_t run_size, int noiseless,
+                                   void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API int des_nes_grad_partial_sweep(float *partial_out_dev, const float *shaped_dev, int64_t n_runs, int64_t run_size,
+                                       int64_t P, const des_run_hp *hp_dev, uint64_t generation, const des_state *state_dev,
+                                       void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API int des_nes_apply_sweep(float *theta_dev, double *adam_m_dev, double *adam_v_dev, float *update_out_dev,
+                                double *grad_out_dev, const float *partial_sum_dev, int64_t P, int64_t n_runs,
+                                int64_t run_size, const des_run_hp *hp_dev, double beta1, double beta2, double epsilon,
+                                const des_state *state_dev, void *stream);
+
 /* ---- environments stepped on the host: the population's policy step on the device ------------------------------ */
 
 /* One environment step of n_local members x `repetitions` episodes whose environments the caller steps on the host:
