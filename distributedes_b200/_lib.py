@@ -71,6 +71,9 @@ SIGNATURES = {
     'des_nes_apply_sweep': (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _P, _D, _D, _D, _P, _P]),
     'des_policy_act': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _D, _U64, _U64, _I64, _I64, _I64, _P]),
     'des_obs_parts_reduce': (C.c_int, [_P, _P, _I64, _I32, _P]),
+    'des_nes_perturb_sweep': (C.c_int, [_P, _P, _I64, _I64, _I64, _P, _U64, _P]),
+    'des_policy_act_sweep': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _P, _U64, _I64, _I64, _I64, _P]),
+    'des_obs_parts_reduce_runs': (C.c_int, [_P, _P, _I64, _I64, _I32, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_nes_eval_mirrored': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),

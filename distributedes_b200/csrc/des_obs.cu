@@ -166,3 +166,15 @@ extern "C" DES_API int des_obs_stats_merge_totals_runs(float *stats_dev, const d
     DES_LAUNCH_CHECK("obs_stats_merge_totals_runs_kernel");
     return DES_OK;
 }
+
+extern "C" DES_API int des_obs_parts_reduce_runs(double *obs_totals_out_dev, const double *parts_dev, int64_t n_runs,
+                                                 int64_t run_size, int32_t state_dim, void *stream) {
+    const char *who = "des_obs_parts_reduce_runs";
+    const int rc = des::check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(state_dim > 0 && state_dim <= 511, "%s: state_dim must be in [1, 511] (got %d)", who, (int)state_dim);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(obs_totals_out_dev && parts_dev, "%s: NULL pointer", who);
+    return des::obs_parts_reduce_runs(obs_totals_out_dev, parts_dev, n_runs, run_size, 2 * state_dim + 1,
+                                      (cudaStream_t)stream);
+}

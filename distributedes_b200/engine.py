@@ -25,6 +25,7 @@ import torch.distributed as dist
 
 from . import ops
 from .fitness import DeviceRollouts, HostEpisodes, HostRollouts, Tape  # noqa: F401  (engine.HostEpisodes stays public)
+from .fitness import HostSweep
 
 
 def shard_bounds(N, world_size, rank):
@@ -328,7 +329,38 @@ class HostEnvEngine(NESEngine):
                          **kw)
 
 
-class RolloutRunsEngine:
+class _RunsUpdate:
+    """The update of a batch of runs after its evaluation, one launch per step for all runs: ranking, the partial sums,
+    Adam and the statistics merge.  With a sweep table `hp` each run has its own seed and hyper-parameters (ops_sweep);
+    without one the runs share `seed`, `sigma`, `lr` and `wd`."""
+
+    def rank_and_reduce(self):
+        self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
+        if self.hp is not None:
+            self.k.nes_grad_partial_sweep(self.shaped, self.P, self.hp, state=self.state, workspace=self.grad_ws,
+                                          out=self.partial)
+        else:
+            self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
+                                         out=self.partial)
+        return self.partial
+
+    def apply(self):
+        if self.hp is not None:
+            self.k.nes_apply_sweep(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state, self.hp,
+                                   beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
+        else:
+            self.k.nes_apply_runs(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state,
+                                  sigma=self.sigma, learning_rate=self.lr, weight_decay=self.wd, beta1=self.beta1,
+                                  beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
+        self.k.state_advance(self.state, self.beta1, self.beta2)
+        if self.normalize_obs:    # natural_es.py:85-89, each run's observations into its own statistics
+            self.k.obs_stats_merge_totals_runs(self.obs_stats, self.obs_totals, self.d0)
+
+    def theta_numpy(self):
+        return self.theta.detach().cpu().numpy()
+
+
+class RolloutRunsEngine(_RunsUpdate):
     """R independent NES runs of `pop_size` members on the device's closed-loop Pendulum, trained together: every
     generation evaluates all runs' members in one rollout launch and ranks, reduces, applies and merges the statistics of
     all runs in one launch each, so the launches per generation do not depend on R.
@@ -443,28 +475,6 @@ class RolloutRunsEngine:
                       workspace=self.roll_ws, out=self.fitness_all)
         return self.fitness_all
 
-    def rank_and_reduce(self):
-        self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
-        if self.hp is not None:
-            self.k.nes_grad_partial_sweep(self.shaped, self.P, self.hp, state=self.state, workspace=self.grad_ws,
-                                          out=self.partial)
-        else:
-            self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
-                                         out=self.partial)
-        return self.partial
-
-    def apply(self):
-        if self.hp is not None:
-            self.k.nes_apply_sweep(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state, self.hp,
-                                   beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
-        else:
-            self.k.nes_apply_runs(self.theta, self.adam_m, self.adam_v, self.partial, self.N, self.state,
-                                  sigma=self.sigma, learning_rate=self.lr, weight_decay=self.wd, beta1=self.beta1,
-                                  beta2=self.beta2, epsilon=self.epsilon, update_out=self.update)
-        self.k.state_advance(self.state, self.beta1, self.beta2)
-        if self.normalize_obs:    # natural_es.py:85-89, each run's observations into its own statistics
-            self.k.obs_stats_merge_totals_runs(self.obs_stats, self.obs_totals, self.d0)
-
     def _generation_eager(self):
         self.evaluate()
         self.rank_and_reduce()
@@ -491,5 +501,101 @@ class RolloutRunsEngine:
                       out=self.test_fitness, episodes_out=episodes)
         return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
 
-    def theta_numpy(self):
-        return self.theta.detach().cpu().numpy()
+
+class HostEnvSweepEngine(_RunsUpdate):
+    """A sweep of R NES runs on environments stepped on the HOST (fitness.HostSweep): run r is HostEnvEngine(env_fn=
+    env_fn[r], batch_env_fn=batch_env_fn[r], seed=seeds[r], sigma=sigma[r], ...), bit for bit, on one GPU.  Every
+    environment step of every run is one des_policy_act_sweep, and every run's rows, ranking, partial sums, Adam and
+    statistics merge are one launch each, so the launches per step and per generation do not depend on R.  The runs share
+    the shapes, repetitions, clip, normaliser setting and Adam's beta and epsilon; `env_fn`, `batch_env_fn`, `sigma`,
+    `learning_rate`, `weight_decay` and `action_noise_std` may each be one value or a sequence of R.  theta0 is [P] or
+    [R, P].
+
+    The surface is RolloutRunsEngine's, eager: evaluate() -> fitness_all [R, N], steps_taken [R], test_returns() ->
+    [R, repetitions], rank_and_reduce(), apply(), generation(), theta [R, P].  `running` [R] (all True at first) says which
+    runs the host loop serves: clear run r's entry once its training has ended, and its environments are never reset or
+    stepped again; its slots enter every later launch dead, and what the engine computes for it is to be ignored."""
+
+    MAX_RUN_SIZE = RolloutRunsEngine.MAX_RUN_SIZE
+
+    def __init__(self, *, env_fn, hidden, pop_size, runs, theta0, seeds, sigma, learning_rate, weight_decay=0.005,
+                 state_dim=None, action_dim=None, repetitions=10, test_repetitions=None, action_noise_std=0.0,
+                 normalize_obs=True, batch_env_fn=None, clip=1.0, beta1=0.9, beta2=0.999, epsilon=1e-8, kernels=None,
+                 device=None):
+        from . import ops_runs
+        from .ops_sweep import per_run
+        self.k, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
+        if self.k is ops_runs and self.device.type != 'cuda':
+            raise RuntimeError('distributedes_b200 needs a CUDA device, got %s: there is no CPU fallback' % self.device)
+        self.R, self.N = int(runs), int(pop_size)
+        if self.R < 1:
+            raise ValueError('runs must be >= 1; got %r' % (runs,))
+        if not 2 <= self.N <= self.MAX_RUN_SIZE:
+            raise ValueError('HostEnvSweepEngine: pop_size must be in [2, %d] (runs are batched up to the counting rank\'s '
+                             'population; a larger one fills the GPU alone); got %d' % (self.MAX_RUN_SIZE, self.N))
+        if np.ndim(seeds) == 0:
+            raise ValueError('HostEnvSweepEngine: seeds must be a sequence of one seed per run; got %r' % (seeds,))
+        cols = dict(env_fn=env_fn, batch_env_fn=batch_env_fn, seed=seeds, sigma=sigma, learning_rate=learning_rate,
+                    weight_decay=weight_decay, action_noise_std=action_noise_std)
+        cols = {n: per_run(v, self.R, 'seeds' if n == 'seed' else n) for n, v in cols.items()}
+        for r, s in enumerate(cols['sigma']):
+            if not float(s) > 0.0:
+                raise ValueError('HostEnvSweepEngine: sigma must be > 0 (natural_es.py:92 divides by it); run %d has %r'
+                                 % (r, s))
+        self.source = HostSweep(self.k, self.device, hidden=hidden, repetitions=repetitions, clip=clip,
+                                normalize_obs=normalize_obs, state_dim=state_dim, action_dim=action_dim,
+                                test_repetitions=test_repetitions,
+                                runs=[dict(env_fn=cols['env_fn'][r], batch_env_fn=cols['batch_env_fn'][r],
+                                           seed=cols['seed'][r], sigma=float(cols['sigma'][r]),
+                                           action_noise_std=cols['action_noise_std'][r]) for r in range(self.R)])
+        src = self.source
+        self.d0, self.H, self.A, self.clip = src.d0, src.H, src.A, src.clip
+        self.repetitions, self.test_repetitions, self.normalize_obs = src.repetitions, src.test_repetitions, src.normalize_obs
+        self.seed = [x.seed for x in src.runs]
+        self.action_noise_std = [x.action_noise_std for x in src.runs]
+        self.sigma, self.lr, self.wd = ([float(v) for v in cols[n]] for n in ('sigma', 'learning_rate', 'weight_decay'))
+        self.hp = self.k.run_table(self.seed, self.sigma, self.lr, self.wd, self.action_noise_std, self.device,
+                                   runs=self.R)
+        self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
+        self.P = self.k.param_count(self.d0, self.H, self.A)
+        theta0 = np.ascontiguousarray(theta0, dtype=np.float32)
+        if theta0.size == self.P:
+            theta0 = np.tile(theta0.reshape(1, -1), (self.R, 1))
+        elif theta0.size != self.R * self.P:
+            raise ValueError('theta0 has %d entries; the (%d,%d,%d) MLP needs %d, or %d x %d for one start point per run'
+                             % (theta0.size, self.d0, self.H, self.A, self.P, self.R, self.P))
+        dev, R, N, P = self.device, self.R, self.N, self.P
+        self.theta = torch.from_numpy(theta0.reshape(R, P).copy()).to(dev)
+        self.adam_m = torch.zeros((R, P), dtype=torch.float64, device=dev)
+        self.adam_v = torch.zeros((R, P), dtype=torch.float64, device=dev)
+        self.fitness_all = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.shaped = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.partial = torch.zeros((R, P), dtype=torch.float32, device=dev)
+        self.update = torch.zeros((R, P), dtype=torch.float32, device=dev)
+        self.obs_stats, self.obs_totals = src.obs_stats, src.obs_totals
+        self.state = self.k.new_state(dev, 0)
+        self.rank_ws = self.k.rank_runs_workspace(R, N, dev)
+        self.grad_ws = self.k.grad_runs_workspace(R, N, P, dev)
+        self.generation_index = 0
+        self.steps_taken = np.zeros(R, dtype=np.int64)      # per run, the episodes' real lengths (natural_es.py:75)
+        self.running = np.ones(R, dtype=bool)
+
+    def evaluate(self):
+        self.source.members(self.theta, self.hp, generation=self.generation_index, run_size=self.N,
+                            running=self.running, out=self.fitness_all)
+        self.steps_taken = self.source.last_steps
+        return self.fitness_all
+
+    def generation(self):
+        """One generation of every run, eager (the host loop is inside it); read .fitness_all / .theta."""
+        self.evaluate()
+        self.rank_and_reduce()
+        self.apply()
+        self.generation_index += 1
+
+    def test_returns(self, repetitions=None):
+        """[R, repetitions] fp64 returns of noiseless test episodes of every running run's theta with its own statistics,
+        keyed (generation_index, TEST_MEMBER, repetition): run r's are HostEnvEngine.test_returns of theta[r].  The
+        runs `running` leaves out return zeros."""
+        reps = int(repetitions or self.test_repetitions)
+        return self.source.test_returns(self.theta, self.hp, reps, self.generation_index, self.running)

@@ -1,6 +1,6 @@
 """Fitness sources, one per kind of environment: the tape (Tape), episodes stepped on the device (DeviceRollouts) and
 episodes stepped on the host (HostRollouts).  engine.NESEngine and cma_es.Worker evaluate through one and never ask
-which.  A source evaluates NES members theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
+which.  HostSweep is HostRollouts for every run of a sweep at once (engine.HostEnvSweepEngine).  A source evaluates NES members theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
 holds the normaliser statistics `obs_stats` [m | v | n] (or None) and the fp64 observation totals `obs_totals` of its
 last evaluation, shares and merges them over an engine.RankGroup, counts its environment steps and says whether a CUDA
 graph may capture it.  from_config builds the source a config describes, for both trainers."""
@@ -332,6 +332,131 @@ class HostRollouts(_Episodes):
 
     def capturable(self, world):
         return False
+
+
+class HostSweepEpisodes:
+    """HostEpisodes for every run of a sweep in lockstep.  envs[r] is run r's batch environment of n * repetitions slots
+    and rows r*n .. r*n + n - 1 of the weights are its members (ops_sweep: member_offset 0 under run r's seed).  Per step:
+    every slot's observations and alive flags to the device in one copy each, one des_policy_act_sweep, the actions back in
+    one copy and one synchronise, then step(actions_r, alive_r) of every run that still has an alive slot.  So each run's
+    environment receives exactly the reset and step calls its standalone HostEpisodes makes.  The runs `running` leaves
+    out are neither reset nor stepped: their slots enter every launch dead."""
+
+    def __init__(self, kernels, device, envs, n, repetitions, state_dim, hidden, action_dim, clip):
+        self.k, self.device, self.envs = kernels, torch.device(device), list(envs)
+        self.R, self.n, self.reps = len(self.envs), int(n), int(repetitions)
+        self.d0, self.H, self.A, self.clip = int(state_dim), int(hidden), int(action_dim), float(clip)
+        B = self.n * self.reps
+        for r, env in enumerate(self.envs):
+            if int(env.num_envs) != B:
+                raise ValueError('run %d: the batch environment has %d slots; %d members x %d repetitions need %d'
+                                 % (r, env.num_envs, self.n, self.reps, B))
+        pin, RB = self.device.type == 'cuda', self.R * B
+        self.obs_h = torch.zeros((RB, self.d0), dtype=torch.float32, pin_memory=pin)
+        self.alive_h = torch.zeros(RB, dtype=torch.uint8, pin_memory=pin)
+        self.act_h = torch.zeros((RB, self.A), dtype=torch.float32, pin_memory=pin)
+        self.obs_d = torch.zeros((RB, self.d0), dtype=torch.float32, device=self.device)
+        self.alive_d = torch.zeros(RB, dtype=torch.uint8, device=self.device)
+        self.act_d = torch.zeros((RB, self.A), dtype=torch.float32, device=self.device)
+
+    def run(self, rows, hp, *, generation, running, key_member=None, obs_stats=None, stat_part=None):
+        """Returns (returns[R, n, repetitions] fp64, environment steps[R]); the runs not `running` return zeros.  The
+        episodes' keys are HostEpisodes.run's at member_offset 0, the same for every run (each env seeds with its run's
+        seed)."""
+        R, n, reps, B, d0 = self.R, self.n, self.reps, self.n * self.reps, self.d0
+        members = (np.full(n, int(key_member), dtype=np.int64) if key_member is not None else np.arange(n, dtype=np.int64))
+        keys = np.stack([np.full(B, int(generation) & 0xFFFFFFFF, dtype=np.int64), np.repeat(members, reps),
+                         np.tile(np.arange(reps, dtype=np.int64), n)], axis=1)
+        returns, reward, done = (np.zeros((R, B), dtype=np.float64), np.zeros((R, B)), np.zeros((R, B), dtype=bool))
+        steps = np.zeros(R, dtype=np.int64)
+        alive = np.zeros((R, B), dtype=bool)
+        obs_h = self.obs_h.numpy().reshape(R, B, d0)
+        alive_h, act_h = self.alive_h.numpy().reshape(R, B), self.act_h.numpy().reshape(R, B, self.A)
+        for r in np.flatnonzero(running):
+            obs_h[r] = self.envs[r].reset(keys.copy())                # fp32 cast: FloatTensor(o), utils.py:42-45
+            alive[r] = True
+        cuda, t = self.device.type == 'cuda', 0
+        while alive.any():
+            alive_h[:] = alive
+            self.obs_d.copy_(self.obs_h, non_blocking=True)
+            self.alive_d.copy_(self.alive_h, non_blocking=True)
+            self.k.policy_act_sweep(rows, self.obs_d, self.alive_d, hp, state_dim=d0, hidden=self.H, action_dim=self.A,
+                                    repetitions=reps, clip=self.clip, generation=generation, run_size=n, t=t,
+                                    obs_stats=obs_stats, stat_part=stat_part, out=self.act_d)
+            self.act_h.copy_(self.act_d, non_blocking=True)
+            if cuda:
+                torch.cuda.current_stream(self.device).synchronize()
+            for r in np.flatnonzero(alive.any(axis=1)):
+                obs_h[r], reward[r], done[r] = self.envs[r].step(act_h[r], alive[r])
+            np.add(returns, reward, out=returns, where=alive)                   # utils.py:137, alive slots only
+            steps += alive.sum(axis=1)
+            alive &= ~done
+            t += 1
+        return returns.reshape(R, n, reps), steps
+
+
+class HostSweep:
+    """Episodes stepped on the host for every run of a sweep (engine.HostEnvSweepEngine): run r is the HostRollouts of its
+    own environment factories, seed, sigma and action noise, at member_offset 0, and all runs step in lockstep through
+    HostSweepEpisodes.  `runs` holds one dict per run with env_fn, batch_env_fn (None: envs.GymEnvBatch of env_fn under
+    the run's seed), seed, sigma and action_noise_std; the rest is shared.  Owns each run's batch environments (built as
+    HostRollouts builds them: batch_env_fn(N * repetitions) for the members, batch_env_fn(test_repetitions) for the test
+    episodes), the pinned and device buffers of the bridges, the weight rows [R * N, P], stat_part [R * N, 2*d0+1], the
+    statistics obs_stats and the observation totals obs_totals [R, 2*d0+1]."""
+
+    def __init__(self, kernels, device, *, runs, hidden, repetitions, clip, normalize_obs, state_dim=None,
+                 action_dim=None, test_repetitions=None):
+        self.k, self.device = kernels, torch.device(device)
+        self.runs = [HostRollouts(kernels, device, hidden=hidden, repetitions=repetitions, state_dim=state_dim,
+                                  action_dim=action_dim, test_repetitions=test_repetitions, clip=clip,
+                                  normalize_obs=normalize_obs, mirrored=False, **run) for run in runs]
+        src = self.runs[0]
+        for r, x in enumerate(self.runs):
+            if (x.d0, x.A) != (src.d0, src.A):
+                raise ValueError('HostSweep: run %d\'s environment has state_dim %d and action_dim %d; run 0\'s has %d '
+                                 'and %d' % (r, x.d0, x.A, src.d0, src.A))
+        self.R, self.d0, self.H, self.A, self.clip = len(self.runs), src.d0, src.H, src.A, src.clip
+        self.repetitions, self.test_repetitions, self.normalize_obs = src.repetitions, src.test_repetitions, src.normalize_obs
+        w = 2 * self.d0 + 1
+        self.obs_stats = torch.zeros((self.R, w), dtype=torch.float32, device=self.device) if self.normalize_obs else None
+        self.obs_totals = torch.zeros((self.R, w), dtype=torch.float64, device=self.device)
+        self._bridges = {}            # (rows per run, repetitions) -> HostSweepEpisodes
+        self.rows = self.stat_part = None
+        self.last_steps = np.zeros(self.R, dtype=np.int64)
+
+    def _bridge(self, n, reps):
+        ep = self._bridges.get((n, reps))
+        if ep is None:
+            ep = HostSweepEpisodes(self.k, self.device, [x.batch_env_fn(n * reps) for x in self.runs], n, reps, self.d0,
+                                   self.H, self.A, self.clip)
+            self._bridges[(n, reps)] = ep
+        return ep
+
+    def members(self, theta, hp, *, generation, run_size, running, out):
+        """fitness out[R, N] of every run's members theta_r + sigma_r eps (one des_nes_perturb_sweep), its steps in
+        last_steps and, normalising, its observation totals in obs_totals."""
+        N, w = int(run_size), 2 * self.d0 + 1
+        self.obs_totals.zero_()
+        if self.rows is None:
+            self.rows = torch.empty((self.R * N, theta.shape[1]), dtype=torch.float32, device=self.device)
+            self.stat_part = torch.zeros((self.R * N, w), dtype=torch.float64, device=self.device)
+        else:
+            self.stat_part.zero_()
+        self.k.nes_perturb_sweep(theta, hp, N, generation, out=self.rows)
+        part = self.stat_part if self.normalize_obs else None
+        ret, self.last_steps = self._bridge(N, self.repetitions).run(self.rows, hp, generation=generation,
+                                                                     running=running, obs_stats=self.obs_stats,
+                                                                     stat_part=part)
+        out.copy_(torch.from_numpy(np.stack([ret[r].mean(axis=1).astype(np.float32) for r in range(self.R)])))
+        if part is not None:
+            self.k.obs_parts_reduce_runs(part, self.d0, N, out=self.obs_totals)
+
+    def test_returns(self, theta, hp, repetitions, generation, running):
+        """[R, repetitions] fp64: every running run's episodes keyed (generation, TEST_MEMBER, repetition) of theta[r]
+        with its statistics, as HostRollouts.test_returns; they do not feed the statistics."""
+        ret, _ = self._bridge(1, int(repetitions)).run(theta, hp, generation=generation, running=running,
+                                                       key_member=TEST_MEMBER, obs_stats=self.obs_stats)
+        return ret[:, 0]
 
 
 def from_config(config, kernels, device, *, sigma=None, mirrored=False):

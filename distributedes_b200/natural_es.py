@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .engine import NESEngine, RolloutRunsEngine, kernels_and_device
+from .engine import HostEnvSweepEngine, NESEngine, RolloutRunsEngine, kernels_and_device
 from .fitness import from_config
 from .utils import Evaluator, SharedStats, StaticNormalizer, logger
 
@@ -171,45 +171,116 @@ def _field(config, name):
     return value
 
 
+# The fields every host-stepped config of a sweep shares (HostEnvSweepEngine): each run may also have its own env_fn and
+# batch_env_fn, and its task names nothing the trainer reads.
+SWEEP_HOST_SHARED = ('hidden_size', 'pop_size', 'state_dim', 'action_dim', 'repetitions', 'test_repetitions', 'clip',
+                     'normalize_obs', 'opt.beta1', 'opt.beta2', 'opt.epsilon', 'max_steps', 'max_generations')
+
+
+def _host_sweep(configs):
+    """Whether `configs` is a host-stepped sweep; a list that mixes host-stepped and other configs is refused."""
+    host = [bool(getattr(c, 'host_env', False)) for c in configs]
+    if any(host) and not all(host):
+        raise ValueError('train_sweep: configs[%d] is host-stepped and configs[%d] is not; the runs of a sweep are all '
+                         'host-stepped (HostEnvConfig) or all closed-loop (ClosedLoopPendulumConfig)'
+                         % (host.index(True), host.index(False)))
+    return all(host)
+
+
+def check_host_sweep_config(config):
+    """Raises ValueError unless a host-stepped sweep can hold a run of `config`: plain sampling, at most 2048 members,
+    one process."""
+    if config.mirrored:
+        raise ValueError('train_sweep: mirrored sampling is not batched over runs; use train()')
+    if int(config.pop_size) > HostEnvSweepEngine.MAX_RUN_SIZE:
+        raise ValueError('train_sweep: pop_size %d > %d: runs are batched up to %d members (a larger population fills '
+                         'the GPU alone); use train()' % (config.pop_size, HostEnvSweepEngine.MAX_RUN_SIZE,
+                                                          HostEnvSweepEngine.MAX_RUN_SIZE))
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError('train_sweep: a sweep trains on one GPU; the process group has world size %d'
+                         % dist.get_world_size())
+
+
 def check_sweep_configs(configs):
-    """Raises ValueError unless train_sweep can train `configs` as one sweep: each passes check_runs_config, and they
-    agree on every field of SWEEP_SHARED (the first that differs is named)."""
+    """Raises ValueError unless train_sweep can train `configs` as one sweep: all closed-loop configs that each pass
+    check_runs_config and agree on every field of SWEEP_SHARED, or all host-stepped configs that each pass
+    check_host_sweep_config and agree on every field of SWEEP_HOST_SHARED.  The first field that differs is named."""
     if not len(configs):
         raise ValueError('train_sweep: no configs')
+    host = _host_sweep(configs)
     for c in configs:
-        check_runs_config(c)
+        (check_host_sweep_config if host else check_runs_config)(c)
     for i, c in enumerate(configs[1:], 1):
-        for name in SWEEP_SHARED:
+        for name in SWEEP_HOST_SHARED if host else SWEEP_SHARED:
             a, b = _field(configs[0], name), _field(c, name)
             if a != b:
                 raise ValueError('train_sweep: configs differ in %s (%r in configs[0], %r in configs[%d]); the runs of a '
                                  'sweep may differ only in seed, sigma, learning_rate, weight_decay, action_noise_std '
-                                 'and initial_weight' % (name, a, b, i))
+                                 'and initial_weight%s' % (name, a, b, i, ' (and, host-stepped, their own env_fn and '
+                                                           'batch_env_fn)' if host else ''))
 
 
 def build_sweep_engine(configs, *, kernels=None, device=None, **kw):
-    """The RolloutRunsEngine of a sweep: run r is train(configs[r])'s run, with its seed, hyper-parameters and
-    initial_weight.  `kw` goes to RolloutRunsEngine (use_graph)."""
+    """The engine of a sweep: run r is train(configs[r])'s run, with its seed, hyper-parameters and initial_weight (and,
+    host-stepped, its own environments).  Closed-loop configs give a RolloutRunsEngine (`kw`: use_graph), host-stepped
+    ones a HostEnvSweepEngine."""
     check_sweep_configs(configs)
     c = configs[0]
-    return RolloutRunsEngine(task=c.task, hidden=c.hidden_size, pop_size=c.pop_size, runs=len(configs),
-                             theta0=np.stack([np.asarray(x.initial_weight, dtype=np.float32).reshape(-1) for x in configs]),
-                             seeds=[x.seed for x in configs], sigma=[x.sigma for x in configs],
-                             learning_rate=[x.learning_rate for x in configs],
-                             weight_decay=[x.weight_decay for x in configs],
-                             action_noise_std=[x.action_noise_std for x in configs], repetitions=c.repetitions,
-                             clip=c.clip, normalize_obs=c.normalize_obs, beta1=c.opt.beta1, beta2=c.opt.beta2,
-                             epsilon=c.opt.epsilon, kernels=kernels, device=device, **kw)
+    per_run = dict(theta0=np.stack([np.asarray(x.initial_weight, dtype=np.float32).reshape(-1) for x in configs]),
+                   seeds=[x.seed for x in configs], sigma=[x.sigma for x in configs],
+                   learning_rate=[x.learning_rate for x in configs], weight_decay=[x.weight_decay for x in configs],
+                   action_noise_std=[x.action_noise_std for x in configs])
+    shared = dict(hidden=c.hidden_size, pop_size=c.pop_size, runs=len(configs), repetitions=c.repetitions, clip=c.clip,
+                  normalize_obs=c.normalize_obs, beta1=c.opt.beta1, beta2=c.opt.beta2, epsilon=c.opt.epsilon,
+                  kernels=kernels, device=device)
+    if _host_sweep(configs):
+        return HostEnvSweepEngine(env_fn=[x.env_fn for x in configs],
+                                  batch_env_fn=[getattr(x, 'batch_env_fn', None) for x in configs],
+                                  state_dim=c.state_dim, action_dim=c.action_dim, test_repetitions=c.test_repetitions,
+                                  **per_run, **shared, **kw)
+    return RolloutRunsEngine(task=c.task, **per_run, **shared, **kw)
 
 
 def train_sweep(configs, engine=None):
-    """train(configs[r]) for every r, trained together on one GPU as one sweep (engine.RolloutRunsEngine with seeds):
-    one [training_rewards, training_steps, training_timestamps] triple per config, whose rewards and steps are those of
-    train(configs[r]).  The runs share one clock, as in train_runs.  The configs may differ only in seed, sigma,
-    learning_rate, weight_decay, action_noise_std and initial_weight (check_sweep_configs)."""
+    """train(configs[r]) for every r, trained together on one GPU as one sweep: one [training_rewards, training_steps,
+    training_timestamps] triple per config, whose rewards and steps are those of train(configs[r]).  The runs share one
+    clock.  The configs may differ only in seed, sigma, learning_rate, weight_decay, action_noise_std and initial_weight
+    (check_sweep_configs); host-stepped ones also in their env_fn and batch_env_fn.  Closed-loop configs train through
+    engine.RolloutRunsEngine with seeds, all runs for the same generations; host-stepped ones through
+    engine.HostEnvSweepEngine, where each run counts its own steps and stops where train() would."""
     check_sweep_configs(configs)
     engine = engine if engine is not None else build_sweep_engine(configs)
-    return train_runs(configs[0], len(configs), engine=engine)       # its loop reads only the fields the configs share
+    if not _host_sweep(configs):
+        return train_runs(configs[0], len(configs), engine=engine)   # its loop reads only the fields the configs share
+    c, R = configs[0], len(configs)
+    out = [[[], [], []] for _ in range(R)]
+    total_steps = np.zeros(R, dtype=np.int64)
+    initial_time = time.time()
+    iteration = 0
+    while True:
+        live = np.flatnonzero(engine.running)
+        returns = engine.test_returns(c.test_repetitions)                   # natural_es.py:54, every running run
+        elapsed_time = time.time() - initial_time
+        for r in live:
+            for log, value in zip(out[r], (np.mean(returns[r]), int(total_steps[r]), elapsed_time)):
+                log.append(value)
+        logger.info('Test: %d runs running, mean %f, elapsed time %d'
+                    % (len(live), float(np.mean([out[r][0][-1] for r in live])), elapsed_time))
+        fitness = engine.evaluate()
+        total_steps[live] += engine.steps_taken[live]                       # :75, each run's episodes' real lengths
+        logger.info('Train: iteration %d, mean fitness over %d runs %f'
+                    % (iteration, len(live), float(fitness[torch.as_tensor(live)].mean())))
+        iteration += 1
+        for r in live:                                                      # :82-84, where train(configs[r]) breaks
+            if (c.max_steps and total_steps[r] > c.max_steps) or \
+                    (getattr(c, 'max_generations', 0) and iteration > c.max_generations):
+                engine.running[r] = False
+        if not engine.running.any():
+            break
+        engine.rank_and_reduce()
+        engine.apply()
+        engine.generation_index += 1
+    return out
 
 
 def test(config, solution, stats, engine=None):

@@ -101,5 +101,6 @@ def nes_apply_runs(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learn
             _ptr(state, 'state', U8, STATE_BYTES, dev))
 
 # The sweep ops (seeds and NES hyper-parameters per run): defined in ops_sweep, listed here so that this module stays the
-# whole set of device ops engine.RolloutRunsEngine calls.
-from .ops_sweep import nes_apply_sweep, nes_grad_partial_sweep, rollout_eval_sweep, run_table  # noqa: E402,F401
+# whole set of device ops engine.RolloutRunsEngine and engine.HostEnvSweepEngine call.
+from .ops_sweep import (nes_apply_sweep, nes_grad_partial_sweep, nes_perturb_sweep, obs_parts_reduce_runs,  # noqa: E402,F401
+                        policy_act_sweep, rollout_eval_sweep, run_table)

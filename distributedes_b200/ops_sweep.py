@@ -4,8 +4,11 @@ device table, `hp` (run_table), one 40-byte des_run_hp row per run.  Run r's mem
 population under run r's seed, so each op equals, run by run, the op of ops.py it is named after with run r's seed and
 hyper-parameters at member_offset 0.  The checks are those of ops._ptr; the table is checked like every other tensor.
 
-ops_runs re-exports these ops, so that it stays the one module of device ops engine.RolloutRunsEngine calls.  Ranking
-and the statistics merge need no table: ops_runs.centered_rank_runs and ops_runs.obs_stats_merge_totals_runs.
+ops_runs re-exports these ops, so that it stays the one module of device ops engine.RolloutRunsEngine and
+engine.HostEnvSweepEngine call.  Ranking and the statistics merge need no table: ops_runs.centered_rank_runs and
+ops_runs.obs_stats_merge_totals_runs.  On host-stepped environments the rows of every run come from nes_perturb_sweep, each
+environment step of every run is one policy_act_sweep, and obs_parts_reduce_runs sums each run's observation rows
+(defined in ops_host_sweep, listed here).
 """
 from __future__ import annotations
 
@@ -103,3 +106,7 @@ def nes_apply_sweep(theta, adam_m, adam_v, partial_sum, N, state, hp, *, beta1=0
             _ptr(grad_out, 'grad_out', F64, R * P, dev, True), _ptr(partial_sum, 'partial_sum', F32, R * P, dev), P, R,
             int(N), _hp(hp, R, dev), float(beta1), float(beta2), float(epsilon),
             _ptr(state, 'state', U8, STATE_BYTES, dev))
+
+
+# The sweep ops of host-stepped environments (engine.HostEnvSweepEngine) live in ops_host_sweep, on the same table.
+from .ops_host_sweep import nes_perturb_sweep, obs_parts_reduce_runs, policy_act_sweep  # noqa: E402,F401

@@ -297,6 +297,31 @@ DES_API int des_policy_act(float *actions_out_dev, double *stat_part_dev, const 
 DES_API int des_obs_parts_reduce(double *obs_totals_out_dev, const double *parts_dev, int64_t n_local, int32_t state_dim,
                                  void *stream);
 
+/* ---- sweeps on host-stepped environments: the policy step of every run in one launch ----------------------------------
+ *
+ * A sweep (above: the des_run_hp table, the shapes and the n_runs == 0 rule of a batch of runs) whose environments the
+ * caller steps on the host.  Run r's member i is row r * run_size + i of every per-member array and member i of a
+ * standalone population under hp_dev[r].seed (member_offset 0).  Each entry point equals, for every run r, the call named
+ * beside it, bit for bit.
+ *
+ * des_nes_perturb_sweep        rows_out [n_runs * run_size][P]: run r's rows are des_nes_perturb(theta_r, run_size, P,
+ *                              sigma_r, s_r, generation, member_offset = 0).
+ * des_policy_act_sweep         des_policy_act(rows_r, obs_r, alive_r, obs_stats_r, stat_part_r, action_noise_std = a_r,
+ *                              seed = s_r, member_offset = 0, n_local = run_size) for rows, obs, alive, actions and
+ *                              stat_part of n_runs * run_size rows and obs_stats_dev [n_runs][2*state_dim+1] (optional).
+ *                              The limits of des_policy_act apply.  run_size == 1 with the test repetitions gives every
+ *                              run's test episodes (member 0's action noise), as des_policy_act does for one row.
+ * des_obs_parts_reduce_runs    obs_totals_out [n_runs][2*state_dim+1]: run r's row is des_obs_parts_reduce of its
+ *                              run_size rows of parts_dev, in member order. */
+DES_API int des_nes_perturb_sweep(float *rows_out_dev, const float *theta_dev, int64_t n_runs, int64_t run_size, int64_t P,
+                                  const des_run_hp *hp_dev, uint64_t generation, void *stream);
+DES_API int des_policy_act_sweep(float *actions_out_dev, double *stat_part_dev, const float *rows_dev, int64_t P,
+                                 const float *obs_dev, const uint8_t *alive_dev, const float *obs_stats_dev, des_dims dims,
+                                 int32_t repetitions, double clip, const des_run_hp *hp_dev, uint64_t generation,
+                                 int64_t n_runs, int64_t run_size, int64_t t, void *stream);
+DES_API int des_obs_parts_reduce_runs(double *obs_totals_out_dev, const double *parts_dev, int64_t n_runs,
+                                      int64_t run_size, int32_t state_dim, void *stream);
+
 /* ---- fused sample + forward + fitness ------------------------------------------------------ */
 
 /* fitness_out_dev[i] (i < n_local) = sum_t -|| clip(pi_{theta+sigma*eps_m}(obs_t), -clip, clip) - target_t ||^2
