@@ -74,6 +74,12 @@ SIGNATURES = {
     'des_nes_perturb_sweep': (C.c_int, [_P, _P, _I64, _I64, _I64, _P, _U64, _P]),
     'des_policy_act_sweep': (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, Dims, _I32, _D, _P, _U64, _I64, _I64, _I64, _P]),
     'des_obs_parts_reduce_runs': (C.c_int, [_P, _P, _I64, _I64, _I32, _P]),
+    'des_noise_fill_sweep': (C.c_int, [_P, _I64, _I64, _I64, _P, _U64, _U32, _P]),
+    'des_rollout_eval_solutions_sweep': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _P, _U64, _I64, _I64, _P,
+                                                   _SZ, _P]),
+    'des_cma_rank_mu_runs_workspace_bytes': (_SZ, [_I64, _I64, _I64]),
+    'des_cma_rank_mu_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
+    'des_cma_cov_apply_runs': (C.c_int, [_P, _P, _P, _P, _D, _D, _I64, _I64, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_nes_eval_mirrored': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),

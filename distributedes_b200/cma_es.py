@@ -15,6 +15,7 @@ import time
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import fitness
 from .engine import RankGroup, kernels_and_device
@@ -95,8 +96,39 @@ class CMAEvolutionStrategy:
 
     def tell(self, solutions, cost):
         """cma_es.py:90.  solutions: the rank's [n_local, n] (as returned by ask; all lambda on a single GPU),
-        cost [lambda] GLOBAL (lower is better; rank-shaped or raw — only the order matters)."""
-        k, n = self.k, self.n
+        cost [lambda] GLOBAL (lower is better; rank-shaped or raw — only the order matters).  The three phases around the
+        two kernels are the ones CMASweep runs around its run-batched kernels."""
+        order, Y32, w32, yw = self._tell_rank_mu_inputs(solutions, cost)
+        # ---- the hot part: rank-mu partial of the shard on our kernel (fp32), summed over ranks.  Sharded runs keep the
+        # partial as packed upper-triangular tiles: the all-reduce moves half the bytes of the [n, n] matrix and the
+        # covariance update mirrors the tiles while applying them.
+        packed = self.world > 1
+        if packed:
+            if getattr(self, 'dC_tiles', None) is None:
+                self.dC_tiles = torch.zeros(self.kn.cma_packed_elems(self.n), dtype=torch.float32, device=self.device)
+            if self.n_local:
+                self.kn.cma_rank_mu_packed(Y32, w32, out=self.dC_tiles)
+            else:
+                self.dC_tiles.zero_()
+            self.group.sum_(self.dC_tiles)                                    # the CMA collective of north_star
+        else:
+            if self.n_local:
+                self.kn.cma_rank_mu(Y32, w32, out=self.dC)
+            else:
+                self.dC.zero_()
+        pc32, decay, norm_ps = self._tell_paths(yw)
+        c1, cmu = self.k['c1'], self.k['cmu']
+        if packed:
+            self.kn.cma_cov_apply_packed(self.C, self.dC_tiles, pc32, decay=decay, c1=c1, cmu=cmu)
+        else:
+            self.kn.cma_cov_apply(self.C, self.dC, pc32, decay=decay, c1=c1, cmu=cmu)
+        self._tell_step(norm_ps)
+        return order
+
+    def _tell_rank_mu_inputs(self, solutions, cost):
+        """tell() before the rank-mu partial: the order of the costs, the weights of the local members, Y and
+        yw = sum_i w_i y_i.  Returns (order, Y fp32, w fp32, yw)."""
+        n = self.n
         cost = torch.as_tensor(cost, device=self.device, dtype=torch.float64).reshape(-1)
         if cost.numel() != self.lam:
             raise ValueError('tell() needs the cost of all %d members (got %d)' % (self.lam, cost.numel()))
@@ -113,24 +145,12 @@ class CMAEvolutionStrategy:
         else:
             Y = (X.to(torch.float64) - self.m) / self.sigma                   # foreign solutions: y_i from x_i
         yw = w_loc64 @ Y if self.n_local else torch.zeros(n, dtype=torch.float64, device=self.device)
-        # ---- the hot part: rank-mu partial of the shard on our kernel (fp32), summed over ranks.  Sharded runs keep the
-        # partial as packed upper-triangular tiles: the all-reduce moves half the bytes of the [n, n] matrix and the
-        # covariance update mirrors the tiles while applying them.
-        packed = self.world > 1
-        Y32, w32 = Y.to(torch.float32).contiguous(), w_loc64.to(torch.float32).contiguous()
-        if packed:
-            if getattr(self, 'dC_tiles', None) is None:
-                self.dC_tiles = torch.zeros(self.kn.cma_packed_elems(n), dtype=torch.float32, device=self.device)
-            if self.n_local:
-                self.kn.cma_rank_mu_packed(Y32, w32, out=self.dC_tiles)
-            else:
-                self.dC_tiles.zero_()
-            self.group.sum_(self.dC_tiles)                                    # the CMA collective of north_star
-        else:
-            if self.n_local:
-                self.kn.cma_rank_mu(Y32, w32, out=self.dC)
-            else:
-                self.dC.zero_()
+        return order, Y.to(torch.float32).contiguous(), w_loc64.to(torch.float32).contiguous(), yw
+
+    def _tell_paths(self, yw):
+        """tell() between the rank-mu partial and the covariance update: yw summed over ranks, the mean, p_sigma, hsig,
+        p_c and the decay of C.  Returns (p_c fp32, decay, |p_sigma|)."""
+        k, n = self.k, self.n
         self.group.sum_(yw)
         self.m = self.m + self.sigma * yw
         cs, ds, cc, c1, cmu, mu_eff = k['cs'], k['ds'], k['cc'], k['c1'], k['cmu'], k['mu_eff']
@@ -140,17 +160,92 @@ class CMAEvolutionStrategy:
         hsig = float(norm_ps / np.sqrt(1 - (1 - cs) ** (2 * (self.gen + 1))) / self.chiN < 1.4 + 2.0 / (n + 1))
         self.pc = (1 - cc) * self.pc + hsig * np.sqrt(cc * (2 - cc) * mu_eff) * yw
         decay = 1 + c1 * (1 - hsig) * cc * (2 - cc) - c1 - cmu * float(k['w'].sum())
-        pc32 = self.pc.to(torch.float32).contiguous()
-        if packed:
-            self.kn.cma_cov_apply_packed(self.C, self.dC_tiles, pc32, decay=decay, c1=c1, cmu=cmu)
-        else:
-            self.kn.cma_cov_apply(self.C, self.dC, pc32, decay=decay, c1=c1, cmu=cmu)
-        self.sigma = self.sigma * float(np.exp((cs / ds) * (norm_ps / self.chiN - 1)))
+        return self.pc.to(torch.float32).contiguous(), decay, norm_ps
+
+    def _tell_step(self, norm_ps):
+        """tell() after the covariance update: the step size, the generation and the lazy eigendecomposition."""
+        k = self.k
+        self.sigma = self.sigma * float(np.exp((k['cs'] / k['ds']) * (norm_ps / self.chiN - 1)))
         self.gen += 1
         if self.gen % self.eigen_gap == 0:
             d2, self.B = torch.linalg.eigh(self.C.to(torch.float64))        # library eigendecomposition (cuSOLVER)
             self.D = torch.sqrt(torch.clamp(d2, min=1e-300))
-        return order
+
+
+class CMASweep:
+    """R CMA-ES strategies trained as one batch on one GPU (train_sweep): strategy r is the CMAEvolutionStrategy of
+    train(configs[r]) (x0, sigma0, lambda, its seed), and its state stays bit-equal to that run's.  The runs share lambda
+    and n.  Each strategy's C and dC are views into stacked [R, n, n] tensors, so that one des_cma_rank_mu_runs and one
+    des_cma_cov_apply_runs serve every run, and ask()'s normals of every run are one des_noise_fill_sweep (stream 1,
+    member_offset 0, under each run's seed: the hp table).  The library calls each run's train() makes stay per run: the
+    sampling GEMM of ask, the fp64 vector bookkeeping of tell and the eigendecomposition.
+
+    `running` [R] says which runs still train (train_sweep clears a run's entry where its train() would stop): stopped
+    runs are neither asked nor told, and stop(r) detaches their C and dC from the stacked tensors, which the batched
+    kernels keep writing, so that a stopped run's reported state is its state at its stop."""
+
+    def __init__(self, x0s, sigma0s, popsize, hp, device=None, kernels=None):
+        from . import ops_runs
+        self.kn, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
+        self.hp, self.R, self.lam = hp, len(x0s), int(popsize)
+        self.es = [CMAEvolutionStrategy(x0, s0, self.lam, seed=0, device=self.device, kernels=self.kn)
+                   for x0, s0 in zip(x0s, sigma0s)]
+        es0, R, lam = self.es[0], self.R, self.lam
+        self.n, self.k = es0.n, es0.k
+        dev, n = self.device, self.n
+        self.C = torch.eye(n, dtype=torch.float32, device=dev).repeat(R, 1, 1)
+        self.dC = torch.empty_like(self.C)
+        for r, es in enumerate(self.es):
+            es.C, es.dC = self.C[r], self.dC[r]
+        self.X = torch.empty((R, lam, n), dtype=torch.float32, device=dev)
+        self.Y = torch.zeros((R, lam, n), dtype=torch.float32, device=dev)
+        self.w = torch.zeros((R, lam), dtype=torch.float32, device=dev)
+        self.pc = torch.zeros((R, n), dtype=torch.float32, device=dev)
+        self.decay = np.ones(R)
+        self.running = np.ones(R, dtype=bool)
+        self.gen = 0
+
+    def ask(self):
+        """[R * lambda, n] fp32: run r's rows r*lambda .. are es[r].ask() (a running run's; a stopped run's rows are
+        stale), from one des_noise_fill_sweep."""
+        R, lam, n = self.R, self.lam, self.n
+        z = self.kn.noise_fill_sweep(self.hp, lam, n, self.gen, stream_tag=1).reshape(R, lam, n)
+        for r in np.flatnonzero(self.running):
+            # a tensor of its own, as a run's own z is: the sampling GEMM then sees the allocator's alignment whatever
+            # lambda * n is, so cuBLAS picks the algorithm train() gets
+            self.X[r] = self.es[r].ask(z=z[r].clone())
+        return self.X.reshape(R * lam, n)
+
+    def tell(self, shaped, mark=None):
+        """tell() of every running run with its row of shaped [R, lambda], around one des_cma_rank_mu_runs and one
+        des_cma_cov_apply_runs.  `mark`, if given, is called with the name of each phase as it ends: 'update' after the
+        covariance update, 'eigh' after each run's step size and lazy eigendecomposition (scripts/time_cma_sweep.py)."""
+        live = np.flatnonzero(self.running)
+        state = {}
+        for r in live:
+            es = self.es[r]
+            order, Y32, w32, yw = es._tell_rank_mu_inputs(es.X, shaped[r])
+            self.Y[r], self.w[r] = Y32, w32
+            state[r] = yw
+        self.kn.cma_rank_mu_runs(self.Y, self.w, out=self.dC)
+        for r in live:
+            pc32, self.decay[r], state[r] = self.es[r]._tell_paths(state[r])
+            self.pc[r] = pc32
+        decay = torch.as_tensor(self.decay, dtype=torch.float64).to(self.device)
+        self.kn.cma_cov_apply_runs(self.C, self.dC, self.pc, decay, c1=self.k['c1'], cmu=self.k['cmu'])
+        if mark is not None:
+            mark('update')
+        for r in live:
+            self.es[r]._tell_step(state[r])
+        self.gen += 1
+        if mark is not None:
+            mark('eigh')
+
+    def stop(self, r):
+        """Run r trains no more: its C and dC leave the stacked tensors, frozen as they are."""
+        self.running[r] = False
+        es = self.es[r]
+        es.C, es.dC = es.C.clone(), es.dC.clone()
 
 
 class Worker:
@@ -231,6 +326,206 @@ def train(config, worker=None, es=None):
         es.tell(solutions, shaped)                                                          # :90
         worker.merge_obs_stats(es)                                                          # :92-96
     return [training_rewards, training_steps, training_timestamps]
+
+
+# ---- sweeps: R CMA-ES runs of different configs trained together on one GPU -------------------------------------------
+# The fields every config of a CMA-ES sweep shares (closed-loop, or host-stepped with state_dim / action_dim for task).
+# seed, sigma (sigma0), action_noise_std and initial_weight (x0) may differ, and host-stepped configs may have their own
+# env_fn and batch_env_fn; learning_rate and weight_decay are not read by CMA-ES.
+SWEEP_SHARED = ('task', 'hidden_size', 'pop_size', 'repetitions', 'test_repetitions', 'clip', 'normalize_obs', 'max_steps',
+                'max_generations')
+SWEEP_HOST_SHARED = ('hidden_size', 'pop_size', 'state_dim', 'action_dim', 'repetitions', 'test_repetitions', 'clip',
+                     'normalize_obs', 'max_steps', 'max_generations')
+MAX_SWEEP_POP = 2048      # the counting rank of des_centered_rank_runs (larger runs are DES_ERR_UNSUPPORTED)
+
+
+def check_sweep_configs(configs):
+    """Raises ValueError unless train_sweep can train `configs` as one sweep: all closed-loop (ClosedLoopPendulumConfig)
+    or all host-stepped (HostEnvConfig) configs of 2 .. 2048 members, in one process, that agree on every field of
+    SWEEP_SHARED (closed-loop) or SWEEP_HOST_SHARED (host-stepped).  The first field that differs is named."""
+    from .natural_es import _field, _host_sweep
+    if not len(configs):
+        raise ValueError('cma_es.train_sweep: no configs')
+    host = _host_sweep(configs)
+    for i, c in enumerate(configs):
+        if not host and not getattr(c, 'closed_loop', False):
+            raise ValueError('cma_es.train_sweep: configs[%d] is a tape config; tape configs are not batched over runs '
+                             '(closed-loop ClosedLoopPendulumConfig or host-stepped HostEnvConfig only); use train()' % i)
+        if int(c.pop_size) < 2:
+            raise ValueError('cma_es.train_sweep: pop_size %d < 2: the centered rank of des_centered_rank_runs divides by '
+                             'pop_size - 1' % c.pop_size)
+        if int(c.pop_size) > MAX_SWEEP_POP:
+            raise ValueError('cma_es.train_sweep: pop_size %d > %d: the runs of a sweep are ranked by the counting rank of '
+                             'des_centered_rank_runs, which takes up to %d members (DES_ERR_UNSUPPORTED); use train()'
+                             % (c.pop_size, MAX_SWEEP_POP, MAX_SWEEP_POP))
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError('cma_es.train_sweep: a sweep trains on one GPU; the process group has world size %d'
+                         % dist.get_world_size())
+    for i, c in enumerate(configs[1:], 1):
+        for name in SWEEP_HOST_SHARED if host else SWEEP_SHARED:
+            a, b = _field(configs[0], name), _field(c, name)
+            if a != b:
+                raise ValueError('cma_es.train_sweep: configs differ in %s (%r in configs[0], %r in configs[%d]); the runs '
+                                 'of a CMA-ES sweep may differ only in seed, sigma, action_noise_std and initial_weight%s'
+                                 % (name, a, b, i, ' (and, host-stepped, their own env_fn and batch_env_fn)' if host
+                                    else ''))
+
+
+class SweepWorker:
+    """Worker for every run of a sweep: evaluates each run's solutions through one sweep source (fitness.DeviceSweep
+    closed-loop, fitness.HostSweep host-stepped) under its row of the table `hp` (its seed and action noise), and holds
+    each run's statistics obs_stats and observation totals obs_totals [R, 2*d0+1].  tests_run counts the test() calls,
+    the generation word of the next test episodes, as Worker's does."""
+
+    def __init__(self, configs, device=None, kernels=None):
+        from . import ops_runs
+        self.kn, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
+        c, R = configs[0], len(configs)
+        self.R, self.host = R, bool(getattr(c, 'host_env', False))
+        self.hp = self.kn.run_table([x.seed for x in configs], [x.sigma for x in configs], 0.0, 0.0,
+                                    [float(x.action_noise_std) for x in configs], self.device, runs=R)
+        shared = dict(hidden=c.hidden_size, repetitions=c.repetitions, clip=c.clip, normalize_obs=c.normalize_obs)
+        if self.host:
+            self.source = fitness.HostSweep(self.kn, self.device, state_dim=c.state_dim, action_dim=c.action_dim,
+                                            test_repetitions=c.test_repetitions,
+                                            runs=[dict(env_fn=x.env_fn, batch_env_fn=getattr(x, 'batch_env_fn', None),
+                                                       seed=x.seed, sigma=None,
+                                                       action_noise_std=float(x.action_noise_std)) for x in configs],
+                                            **shared)
+        else:
+            self.source = fitness.DeviceSweep(self.kn, self.device, runs=R, task=c.task, **shared)
+        self.obs_stats, self.obs_totals = self.source.obs_stats, self.source.obs_totals
+        self.tests_run = 0
+        self.fitness = None
+
+    def run(self, rows, generation, running):
+        """cost [R, lambda] (-mean return, cma_es.py:28) of every run's solutions rows [R * lambda, n]."""
+        lam = rows.shape[0] // self.R
+        if self.fitness is None or self.fitness.shape[1] != lam:
+            self.fitness = torch.zeros((self.R, lam), dtype=torch.float32, device=self.device)
+        self.source.solutions(rows, self.hp, generation=generation, running=running, out=self.fitness)
+        return -self.fitness
+
+    def steps(self, lam):
+        """[R] environment steps of the last run() (cma_es.py:73: the episodes' real lengths)."""
+        return self.source.steps(lam) if not self.host else np.asarray(self.source.last_steps, dtype=np.int64)
+
+    def test_returns(self, solutions, repetitions, running):
+        """[R, repetitions] returns of noiseless episodes of solutions[r] (Worker.test_returns of every running run)."""
+        ret = self.source.test_returns(solutions, self.hp, int(repetitions), self.tests_run, running)
+        self.tests_run += 1
+        return ret
+
+    def merge_obs_stats(self, running):
+        """Worker.merge_obs_stats of every running run; a stopped run's statistics stay as they were at its stop."""
+        if self.obs_stats is None:
+            return
+        stopped = torch.as_tensor(np.flatnonzero(~np.asarray(running)), device=self.device)
+        frozen = self.obs_stats[stopped].clone()
+        self.kn.obs_stats_merge_totals_runs(self.obs_stats, self.obs_totals, self.source.d0)
+        self.obs_stats[stopped] = frozen
+
+
+def build_sweep(configs, *, kernels=None, device=None):
+    """The (SweepWorker, CMASweep) pair of train_sweep(configs): run r has configs[r]'s seed, sigma0, action noise, x0
+    and, host-stepped, its own environments."""
+    check_sweep_configs(configs)
+    worker = SweepWorker(configs, device=device, kernels=kernels)
+    es = CMASweep([x.initial_weight for x in configs], [x.sigma for x in configs], configs[0].pop_size, worker.hp,
+                  device=worker.device, kernels=worker.kn)
+    return worker, es
+
+
+def train_sweep(configs, worker=None, es=None):
+    """train(configs[r]) for every r, trained together on one GPU: one [training_rewards, training_steps,
+    training_timestamps] triple per config, whose rewards and steps are those of train(configs[r]), bit for bit (and so
+    is each run's final strategy state es.es[r] and statistics worker.obs_stats[r]).  The runs share one clock.  The
+    configs may differ only in seed, sigma, action_noise_std and initial_weight (check_sweep_configs); host-stepped ones
+    also in env_fn and batch_env_fn.  Closed-loop runs all take the same steps and stop together; host-stepped runs
+    count their own steps and each stops where its train() would, its environments never reset or stepped again."""
+    check_sweep_configs(configs)
+    if worker is None or es is None:
+        worker, es = build_sweep(configs)
+    c, R, lam = configs[0], len(configs), es.lam
+    out = [[[], [], []] for _ in range(R)]
+    total_steps = np.zeros(R, dtype=np.int64)
+    initial_time = time.time()
+    x0 = torch.from_numpy(np.stack([np.asarray(x.initial_weight, dtype=np.float32).reshape(-1) for x in configs]))
+    returns = worker.test_returns(x0.to(worker.device), c.test_repetitions, es.running)           # :56
+    for r in range(R):
+        for log, value in zip(out[r], (np.mean(returns[r]), 0, 0)):
+            log.append(value)
+    logger.info('total steps 0, mean over %d runs %f' % (R, float(np.mean([o[0][-1] for o in out]))))
+    generation = 0
+    while True:
+        live = np.flatnonzero(es.running)
+        rows = es.ask()                                                                     # :62
+        cost = worker.run(rows, es.gen, es.running)                                         # :63-72, [R, lambda]
+        total_steps[live] += worker.steps(lam)[live]                                        # :73
+        best = torch.argmin(cost, dim=1)                                                    # :75
+        elapsed_time = time.time() - initial_time
+        best_rows = rows.reshape(R, lam, -1)[torch.arange(R, device=rows.device), best].contiguous()
+        returns = worker.test_returns(best_rows, c.test_repetitions, es.running)           # :77
+        for r in live:
+            for log, value in zip(out[r], (np.mean(returns[r]), int(total_steps[r]), elapsed_time)):
+                log.append(value)
+        logger.info('%d runs running, total steps %s, mean test %f, elapased time %f'
+                    % (len(live), total_steps[live].tolist(), float(np.mean([out[r][0][-1] for r in live])),
+                       elapsed_time))
+        generation += 1
+        for r in live:                                                                      # :85-87, where train() breaks
+            if (c.max_steps and total_steps[r] > c.max_steps) or \
+                    (getattr(c, 'max_generations', 0) and generation >= c.max_generations):
+                es.stop(r)
+        if not es.running.any():
+            break
+        shaped = worker.kn.centered_rank_runs(cost.to(torch.float32).contiguous())          # :89 fitness_shift(cost)
+        es.tell(shaped)                                                                     # :90
+        worker.merge_obs_stats(es.running)                                                  # :92-96
+    return out
+
+
+def multi_runs(config, runs=10, log_dir='log', data_dir='data', batched=False):
+    """The reference's CMA-ES driver (cma_es.py:113-152, natural_es.py:113-124's bookkeeping): `runs` train() runs, a
+    per-task log file and the pickle of [[rewards, steps, timestamps], ...] rewritten after every run, with the file names
+    and on-disk format of natural_es.multi_runs (data/<tag>-stats-<task>.bin).  Run r uses seed config.seed + r, so the
+    runs are independent, as the reference's OS-seeded ones are.  batched=True trains them together through train_sweep
+    and writes the same files once: the rewards and steps are those of batched=False, bit for bit; the timestamps come
+    from the sweep's one clock.  Unlike natural_es.multi_runs(batched=True), whose runs 1.. are further streams of one
+    seed that no single train() reproduces, every run here is a sweep run of its own seed, and so reproducible alone."""
+    import copy
+    import logging
+    import os
+    import pickle
+    os.makedirs(log_dir, exist_ok=True)
+    os.makedirs(data_dir, exist_ok=True)
+    configs = []
+    for r in range(runs):
+        c = copy.copy(config)
+        c.seed = config.seed + r
+        configs.append(c)
+    if batched:
+        check_sweep_configs(configs)
+    fh = logging.FileHandler(os.path.join(log_dir, '%s-%s.txt' % (config.tag, config.task)))
+    fh.setLevel(logging.DEBUG)
+    logger.addHandler(fh)
+    stats = []
+    path = os.path.join(data_dir, '%s-stats-%s.bin' % (config.tag, config.task))
+    try:
+        if batched:
+            logger.info('Runs 0-%d, batched' % (runs - 1))
+            stats = train_sweep(configs)
+            with open(path, 'wb') as f:
+                pickle.dump(stats, f)
+        for run in range(0 if batched else runs):
+            logger.info('Run %d' % (run))
+            stats.append(train(configs[run]))
+            with open(path, 'wb') as f:
+                pickle.dump(stats, f)
+    finally:
+        logger.removeHandler(fh)
+        fh.close()
+    return stats
 
 
 def _fetch_member(es, solutions_local, index):

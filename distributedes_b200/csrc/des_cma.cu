@@ -17,9 +17,10 @@ static_assert(cma_packed_tile(kCmaTcMinN - 1) == kCmaTile, "packed output of the
 // 64 x 64 outputs per CTA, 256 threads as 16 x 16.  Each thread owns a 4 x 4 block (rows ty*4 + {0..3}, columns
 // tx*4 + {0..3}), so every shared-memory operand read is one conflict-free LDS.128.  k-panels of 16 members are double
 // buffered: the next panel's global loads are in flight while the current one is multiplied.
-__global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restrict__ dC, const float *__restrict__ Y,
-                                                                  const float *__restrict__ w, int64_t lambda, int64_t n,
-                                                                  int tiles_per_side, int packed) {
+// The body of the kernel, shared with the run-batched kernel (des_cma_rank_mu_runs): dC, Y and w are the CTA's run's.
+__device__ __forceinline__ void cma_rank_mu_tile(float *__restrict__ dC, const float *__restrict__ Y,
+                                                 const float *__restrict__ w, int64_t lambda, int64_t n, int tiles_per_side,
+                                                 int packed) {
     constexpr int MT = 4;
     constexpr int LD = kCmaKP * kCmaTile / kCmaThreads;   // elements each thread stages per operand and panel
     __shared__ __align__(16) float As[2][kCmaKP][kCmaTile];   // w_k * Y[k][i0 + i]
@@ -123,14 +124,42 @@ __global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restr
     }
 }
 
-__global__ void cma_cov_apply_kernel(float *__restrict__ C, const float *__restrict__ dC, const float *__restrict__ pc,
-                                     int64_t n, float decay, float c1, float cmu) {
+__global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_kernel(float *__restrict__ dC, const float *__restrict__ Y,
+                                                                  const float *__restrict__ w, int64_t lambda, int64_t n,
+                                                                  int tiles_per_side, int packed) {
+    cma_rank_mu_tile(dC, Y, w, lambda, n, tiles_per_side, packed);
+}
+
+// A batch of runs (des_cma_rank_mu_runs): CTA row y is run y's cma_rank_mu_kernel, full matrix, on its rows of dC, Y, w.
+__global__ void __launch_bounds__(kCmaThreads) cma_rank_mu_runs_kernel(float *__restrict__ dC, const float *__restrict__ Y,
+                                                                       const float *__restrict__ w, int64_t lambda,
+                                                                       int64_t n, int tiles_per_side) {
+    const int64_t run = blockIdx.y;
+    cma_rank_mu_tile(dC + run * n * n, Y + run * lambda * n, w + run * lambda, lambda, n, tiles_per_side, 0);
+}
+
+// The covariance update of one entry, shared with the run-batched kernel (des_cma_cov_apply_runs).
+__device__ __forceinline__ void cma_cov_apply_at(float *__restrict__ C, const float *__restrict__ dC,
+                                                 const float *__restrict__ pc, int64_t n, float decay, float c1, float cmu) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= n * n) return;
     const int64_t i = idx / n, j = idx - i * n;
     float v = decay * C[idx];
     if (pc) v = __fmaf_rn(c1 * __ldg(pc + i), __ldg(pc + j), v);
     C[idx] = __fmaf_rn(cmu, dC[idx], v);
+}
+
+__global__ void cma_cov_apply_kernel(float *__restrict__ C, const float *__restrict__ dC, const float *__restrict__ pc,
+                                     int64_t n, float decay, float c1, float cmu) {
+    cma_cov_apply_at(C, dC, pc, n, decay, c1, cmu);
+}
+
+// A batch of runs (des_cma_cov_apply_runs): CTA row y updates run y's C with its dC, pc and decay; decay is converted to
+// fp32 as the host converts the single call's.
+__global__ void cma_cov_runs_kernel(float *__restrict__ C, const float *__restrict__ dC, const float *__restrict__ pc,
+                                          const double *__restrict__ decay, int64_t n, float c1, float cmu) {
+    const int64_t run = blockIdx.y;
+    cma_cov_apply_at(C + run * n * n, dC + run * n * n, pc ? pc + run * n : nullptr, n, (float)decay[run], c1, cmu);
 }
 
 // C <- decay*C + c1 pc pc^T + cmu*dC with dC given as packed upper-triangular tiles (cma_rank_mu_kernel, packed = 1).
@@ -237,5 +266,72 @@ extern "C" DES_API int des_cma_cov_apply(float *C_dev, const float *dC_dev, cons
     cma_cov_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(C_dev, dC_dev, pc_dev, n,
                                                                                           (float)decay, (float)c1, (float)cmu);
     DES_LAUNCH_CHECK("cma_cov_apply_kernel");
+    return DES_OK;
+}
+
+// ---- batches of runs: run r's Y, w, C, dC and pc are row r of [n_runs][...] arrays ----------------------------------------
+
+extern "C" DES_API size_t des_cma_rank_mu_runs_workspace_bytes(int64_t n_runs, int64_t lambda, int64_t n) {
+    return n_runs > 0 ? des_cma_rank_mu_workspace_bytes(n, lambda) : 0;      // the tensor-core runs reuse one workspace
+}
+
+extern "C" DES_API int des_cma_rank_mu_runs(float *out_dev, const float *Y_dev, const float *w_dev, int64_t n_runs,
+                                            int64_t lambda, int64_t n, void *workspace_dev, size_t workspace_bytes,
+                                            void *stream) {
+    using namespace des;
+    const char *who = "des_cma_rank_mu_runs";
+    DES_REQUIRE(n_runs >= 0 && lambda >= 0 && n > 0, "%s: bad sizes n_runs=%lld lambda=%lld n=%lld", who,
+                (long long)n_runs, (long long)lambda, (long long)n);
+    DES_REQUIRE(n <= 46340 * 16, "%s: n too large", who);
+    DES_REQUIRE(n_runs <= ((int64_t)1 << 40) / (n * n) && lambda <= ((int64_t)1 << 40) / n / (n_runs > 0 ? n_runs : 1),
+                "%s: n_runs x n x n or n_runs x lambda x n (%lld, %lld, %lld) floats past 2^40", who, (long long)n_runs,
+                (long long)lambda, (long long)n);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(out_dev && (lambda == 0 || (Y_dev && w_dev)), "%s: NULL pointer", who);
+    const size_t need = des_cma_rank_mu_runs_workspace_bytes(n_runs, lambda, n);
+    if (need && (!workspace_dev || workspace_bytes < need)) {
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (lambda == 0) {
+        DES_CUDA(cudaMemsetAsync(out_dev, 0, (size_t)n_runs * n * n * sizeof(float), st));
+        return DES_OK;
+    }
+    if (n >= kCmaTcMinN) {                 // one tensor-core SYRK per run, one workspace reused in stream order
+        for (int64_t r = 0; r < n_runs; ++r) {
+            const int rc = cma_rank_mu_tc(out_dev + r * n * n, Y_dev + r * lambda * n, w_dev + r * lambda, lambda, n, 0,
+                                          workspace_dev, st);
+            if (rc != DES_OK) return rc;
+        }
+        return DES_OK;
+    }
+    const int t = (int)((n + kCmaTile - 1) / kCmaTile);
+    for (int64_t r0 = 0; r0 < n_runs; r0 += 65535) {            // grid y: up to 65535 runs per launch
+        const int64_t nr = n_runs - r0 < 65535 ? n_runs - r0 : 65535;
+        cma_rank_mu_runs_kernel<<<dim3((unsigned)(t * (t + 1) / 2), (unsigned)nr), kCmaThreads, 0, st>>>(
+            out_dev + r0 * n * n, Y_dev + r0 * lambda * n, w_dev + r0 * lambda, lambda, n, t);
+        DES_LAUNCH_CHECK("cma_rank_mu_runs_kernel");
+    }
+    return DES_OK;
+}
+
+extern "C" DES_API int des_cma_cov_apply_runs(float *C_dev, const float *dC_dev, const float *pc_dev,
+                                              const double *decay_dev, double c1, double cmu, int64_t n_runs, int64_t n,
+                                              void *stream) {
+    using namespace des;
+    const char *who = "des_cma_cov_apply_runs";
+    DES_REQUIRE(n_runs >= 0 && n > 0, "%s: bad sizes n_runs=%lld n=%lld", who, (long long)n_runs, (long long)n);
+    DES_REQUIRE(n <= 46340 * 16 && n_runs <= ((int64_t)1 << 40) / (n * n), "%s: n_runs x n x n past 2^40", who);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(C_dev && dC_dev && decay_dev, "%s: NULL pointer", who);
+    const int64_t blocks = (n * n + 255) / 256;
+    for (int64_t r0 = 0; r0 < n_runs; r0 += 65535) {            // grid y: up to 65535 runs per launch
+        const int64_t nr = n_runs - r0 < 65535 ? n_runs - r0 : 65535;
+        cma_cov_runs_kernel<<<dim3((unsigned)blocks, (unsigned)nr), 256, 0, (cudaStream_t)stream>>>(
+            C_dev + r0 * n * n, dC_dev + r0 * n * n, pc_dev ? pc_dev + r0 * n : nullptr, decay_dev + r0, n, (float)c1,
+            (float)cmu);
+        DES_LAUNCH_CHECK("cma_cov_runs_kernel");
+    }
     return DES_OK;
 }

@@ -102,7 +102,54 @@ __global__ void perturb_sweep_kernel(float *__restrict__ out, const float *__res
     }
 }
 
+// A sweep's normals (des_noise_fill_sweep): CTA row y takes run y, whose run_size rows are noise_rows_kernel<false>'s rows
+// under the seed of its table row, member_offset 0 (CMA-ES's z of every run, stream kStreamCmaZ).
+__global__ void noise_sweep_kernel(float *__restrict__ out, int64_t run_size, int64_t P, const des_run_hp *__restrict__ hp,
+                                   uint32_t gen, uint32_t tag) {
+    const int64_t nq = (P + 3) >> 2;
+    const int64_t total = run_size * nq;
+    PhiloxKey key;
+    philox_round_keys(hp[blockIdx.y].seed, key);
+    out += (int64_t)blockIdx.y * run_size * P;
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t m = idx / nq;
+        const int64_t q = idx - m * nq;
+        const float4 z = noise_quad((uint32_t)q, (uint32_t)m, gen, tag, key);
+        const float zz[4] = {z.x, z.y, z.z, z.w};
+        float *row = out + m * P;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int64_t j = 4 * q + e;
+            if (j < P) row[j] = zz[e];
+        }
+    }
+}
+
 }  // namespace des
+
+extern "C" DES_API int des_noise_fill_sweep(float *z_out_dev, int64_t n_runs, int64_t run_size, int64_t P,
+                                            const des_run_hp *hp_dev, uint64_t generation, uint32_t stream_tag,
+                                            void *stream) {
+    using namespace des;
+    const char *who = "des_noise_fill_sweep";
+    const int rc = check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(P > 0 && P <= ((int64_t)1 << 34), "%s: bad size P=%lld", who, (long long)P);
+    if (n_runs == 0) return DES_OK;
+    DES_REQUIRE(z_out_dev && hp_dev, "%s: NULL pointer", who);
+    const int threads = 256;
+    const int64_t per_run = (run_size * ((P + 3) / 4) + threads - 1) / threads;
+    for (int64_t r0 = 0; r0 < n_runs; r0 += 65535) {            // grid y: up to 65535 runs per launch
+        const int64_t nr = n_runs - r0 < 65535 ? n_runs - r0 : 65535;
+        const int64_t cap = 132 * 64 / nr > 0 ? 132 * 64 / nr : 1;     // about launch_rows' 132 x 64 CTAs in all
+        noise_sweep_kernel<<<dim3((unsigned)(per_run < cap ? per_run : cap), (unsigned)nr), threads, 0,
+                             (cudaStream_t)stream>>>(z_out_dev + r0 * run_size * P, run_size, P, hp_dev + r0,
+                                                     (uint32_t)generation, stream_tag);
+        DES_LAUNCH_CHECK("noise_sweep_kernel");
+    }
+    return DES_OK;
+}
 
 extern "C" DES_API int des_nes_perturb(float *theta_out_dev, const float *theta_dev, int64_t n_members, int64_t P,
                                double sigma, uint64_t seed, uint64_t generation, int64_t member_offset,

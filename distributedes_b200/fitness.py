@@ -1,6 +1,8 @@
 """Fitness sources, one per kind of environment: the tape (Tape), episodes stepped on the device (DeviceRollouts) and
 episodes stepped on the host (HostRollouts).  engine.NESEngine and cma_es.Worker evaluate through one and never ask
-which.  HostSweep is HostRollouts for every run of a sweep at once (engine.HostEnvSweepEngine).  A source evaluates NES members theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
+which.  HostSweep is HostRollouts for every run of a sweep at once (engine.HostEnvSweepEngine, cma_es.SweepWorker), and
+DeviceSweep DeviceRollouts' evaluation of explicit rows for every run of a CMA-ES sweep.  A source evaluates NES members
+theta + sigma*eps (`members`) or explicit rows (`solutions`), runs test episodes,
 holds the normaliser statistics `obs_stats` [m | v | n] (or None) and the fp64 observation totals `obs_totals` of its
 last evaluation, shares and merges them over an engine.RankGroup, counts its environment steps and says whether a CUDA
 graph may capture it.  from_config builds the source a config describes, for both trainers."""
@@ -435,16 +437,26 @@ class HostSweep:
     def members(self, theta, hp, *, generation, run_size, running, out):
         """fitness out[R, N] of every run's members theta_r + sigma_r eps (one des_nes_perturb_sweep), its steps in
         last_steps and, normalising, its observation totals in obs_totals."""
-        N, w = int(run_size), 2 * self.d0 + 1
-        self.obs_totals.zero_()
+        N = int(run_size)
         if self.rows is None:
             self.rows = torch.empty((self.R * N, theta.shape[1]), dtype=torch.float32, device=self.device)
+        self.k.nes_perturb_sweep(theta, hp, N, generation, out=self.rows)
+        self._episodes(self.rows, hp, N, generation, running, out)
+
+    def solutions(self, rows, hp, *, generation, running, out):
+        """members without the perturbation (CMA-ES): rows [R * N, P] are every run's explicit solutions, run r's N rows
+        r*N .. r*N + N - 1 of them, evaluated as HostRollouts.solutions evaluates one run's at offset 0."""
+        self._episodes(rows, hp, rows.shape[0] // self.R, generation, running, out)
+
+    def _episodes(self, rows, hp, N, generation, running, out):
+        w = 2 * self.d0 + 1
+        self.obs_totals.zero_()
+        if self.stat_part is None or self.stat_part.shape[0] != self.R * N:
             self.stat_part = torch.zeros((self.R * N, w), dtype=torch.float64, device=self.device)
         else:
             self.stat_part.zero_()
-        self.k.nes_perturb_sweep(theta, hp, N, generation, out=self.rows)
         part = self.stat_part if self.normalize_obs else None
-        ret, self.last_steps = self._bridge(N, self.repetitions).run(self.rows, hp, generation=generation,
+        ret, self.last_steps = self._bridge(N, self.repetitions).run(rows, hp, generation=generation,
                                                                      running=running, obs_stats=self.obs_stats,
                                                                      stat_part=part)
         out.copy_(torch.from_numpy(np.stack([ret[r].mean(axis=1).astype(np.float32) for r in range(self.R)])))
@@ -457,6 +469,56 @@ class HostSweep:
         ret, _ = self._bridge(1, int(repetitions)).run(theta, hp, generation=generation, running=running,
                                                        key_member=TEST_MEMBER, obs_stats=self.obs_stats)
         return ret[:, 0]
+
+
+class DeviceSweep:
+    """DeviceRollouts.solutions for every run of a CMA-ES sweep (cma_es.SweepWorker): run r is the DeviceRollouts of its
+    own seed and action noise evaluating its rows at offset 0, all runs in one des_rollout_eval_solutions_sweep per
+    generation and their test episodes in one noiseless des_rollout_eval_sweep.  The seeds and action noise are the rows
+    of the sweep table `hp` the caller passes; the rest is shared.  Holds the statistics obs_stats and the observation
+    totals obs_totals [R, 2*d0+1]."""
+
+    def __init__(self, kernels, device, *, runs, task, hidden, repetitions, clip=None, normalize_obs, horizon=None):
+        one = DeviceRollouts(kernels, device, task=task, hidden=hidden, repetitions=repetitions, clip=clip,
+                             horizon=horizon, action_noise_std=0.0, seed=0, normalize_obs=normalize_obs, sigma=None,
+                             mirrored=False)                      # the checks and the shared settings of every run
+        self.k, self.device, self.R = kernels, one.device, int(runs)
+        self.d0, self.H, self.A, self.clip, self.env_id, self.horizon = one.d0, one.H, one.A, one.clip, one.env_id, one.horizon
+        self.repetitions, self.test_repetitions, self.normalize_obs = one.repetitions, one.test_repetitions, one.normalize_obs
+        w = 2 * self.d0 + 1
+        self.obs_stats = torch.zeros((self.R, w), dtype=torch.float32, device=self.device) if self.normalize_obs else None
+        self.obs_totals = torch.zeros((self.R, w), dtype=torch.float64, device=self.device)
+        self.roll_ws = self.fitness = None
+
+    def _env(self):
+        return dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip)
+
+    def solutions(self, rows, hp, *, generation, running, out):
+        """fitness out[R, N] of every run's rows [R * N, P] (run r's N rows r*N ..), and, normalising, each run's
+        observation totals in obs_totals.  Closed-loop runs stop together: `running` is not read."""
+        N, w = rows.shape[0] // self.R, 2 * self.d0 + 1
+        if self.roll_ws is None or self.roll_ws.numel() < self.R * N * w:
+            self.roll_ws = torch.empty(self.R * N * w, dtype=torch.float64, device=self.device)
+        self.obs_totals.zero_()
+        self.k.rollout_eval_solutions_sweep(rows, hp, repetitions=self.repetitions, generation=generation, run_size=N,
+                                            obs_stats=self.obs_stats,
+                                            totals_out=self.obs_totals if self.normalize_obs else None,
+                                            workspace=self.roll_ws, out=out, **self._env())
+
+    def test_returns(self, theta, hp, repetitions, generation, running):
+        """[R, repetitions] fp64: run r's noiseless episodes of theta[r] from the test stream keyed by `generation`, with
+        its statistics: DeviceRollouts.test_returns under run r's seed and action noise."""
+        reps = int(repetitions)
+        if self.fitness is None:
+            self.fitness = torch.empty((self.R, 1), dtype=torch.float32, device=self.device)
+        episodes = torch.empty((self.R, 1, reps), dtype=torch.float32, device=self.device)
+        self.k.rollout_eval_sweep(theta, hp, repetitions=reps, generation=generation, run_size=1, noiseless=True,
+                                  obs_stats=self.obs_stats, out=self.fitness, episodes_out=episodes, **self._env())
+        return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
+
+    def steps(self, N):
+        """[R] environment steps of the last evaluation: every episode runs its whole horizon."""
+        return np.full(self.R, N * self.repetitions * self.horizon, dtype=np.int64)
 
 
 def from_config(config, kernels, device, *, sigma=None, mirrored=False):

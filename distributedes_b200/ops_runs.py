@@ -104,3 +104,6 @@ def nes_apply_runs(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learn
 # whole set of device ops engine.RolloutRunsEngine and engine.HostEnvSweepEngine call.
 from .ops_sweep import (nes_apply_sweep, nes_grad_partial_sweep, nes_perturb_sweep, obs_parts_reduce_runs,  # noqa: E402,F401
                         policy_act_sweep, rollout_eval_sweep, run_table)
+# The CMA-ES sweep ops (cma_es.CMASweep, fitness.DeviceSweep): defined in ops_cma_sweep, on the same table.
+from .ops_cma_sweep import (cma_cov_apply_runs, cma_rank_mu_runs, noise_fill_sweep,  # noqa: E402,F401
+                            rollout_eval_solutions_sweep)

@@ -229,7 +229,7 @@ DES_API int des_obs_stats_merge_totals_runs(float *stats_dev, const double *obs_
  * are identical.  Shared: the generation word and Adam's t and beta^t (state_dev), the dims, repetitions, horizon, clip
  * and Adam's beta1, beta2 and epsilon.  The library cannot read the table's values (they are on the device): a sigma
  * <= 0 is the caller's to refuse.  Ranking and the statistics merge need no table: use des_centered_rank_runs and
- * des_obs_stats_merge_totals_runs.
+ * des_obs_stats_merge_totals_runs.  CMA-ES sweeps read the same table (seed and action_noise_std): "CMA-ES sweeps" below.
  *
  * des_rollout_eval_sweep       des_rollout_eval(theta_r, obs_stats_r, seed = s_r, sigma = sigma_r, action_noise_std =
  *                              a_r, member_offset = 0, n_local = run_size), outputs as des_rollout_eval_runs.
@@ -321,6 +321,41 @@ DES_API int des_policy_act_sweep(float *actions_out_dev, double *stat_part_dev, 
                                  int64_t n_runs, int64_t run_size, int64_t t, void *stream);
 DES_API int des_obs_parts_reduce_runs(double *obs_totals_out_dev, const double *parts_dev, int64_t n_runs,
                                       int64_t run_size, int32_t state_dim, void *stream);
+
+/* ---- CMA-ES sweeps: n_runs strategies of lambda (= run_size) members each, one launch per step for all of them --------
+ *
+ * A sweep of CMA-ES runs whose seeds, step sizes, action noise and start points differ per run (des_run_hp: the seed and
+ * action_noise_std fields are read; sigma, learning_rate and weight_decay are not).  Run r's member i is row
+ * r * lambda + i and member i of a standalone population under hp_dev[r].seed (member_offset 0).  Each entry point
+ * equals, for every run r, the call named beside it, bit for bit; n_runs == 0 does nothing and accepts NULL pointers.
+ *
+ * des_noise_fill_sweep              z_out [n_runs * run_size][P]: run r's rows are des_noise_fill(run_size, P, s_r,
+ *                                   generation, member_offset = 0, stream_tag); the shapes of a batch of runs (above).
+ * des_rollout_eval_solutions_sweep  des_rollout_eval_solutions(rows_r, obs_stats_r, seed = s_r, action_noise_std = a_r,
+ *                                   member_offset = 0, n_local = run_size) for rows [n_runs * run_size][P], fitness
+ *                                   [n_runs][run_size], episode returns [n_runs][run_size][repetitions], statistics and
+ *                                   observation totals [n_runs][2*state_dim+1] (workspace: n_runs * run_size *
+ *                                   (2*state_dim+1) * 8 bytes); the limits of des_rollout_eval_runs.
+ * des_cma_rank_mu_runs              out [n_runs][n][n]: run r's is des_cma_rank_mu(Y_r, w_r, lambda, n, packed = 0) of
+ *                                   Y [n_runs][lambda][n] and w [n_runs][lambda].  Below n = 2048 one launch of the FFMA
+ *                                   kernel for every run; from 2048 the tensor-core path once per run, reusing one
+ *                                   workspace of des_cma_rank_mu_runs_workspace_bytes in stream order.
+ * des_cma_cov_apply_runs            des_cma_cov_apply(C_r, dC_r, pc_r, decay_r, c1, cmu) for C, dC [n_runs][n][n], pc
+ *                                   [n_runs][n] (NULL: no rank-one term) and decay_dev [n_runs] fp64 in DEVICE memory,
+ *                                   converted to fp32 as the single call converts its decay.  c1 and cmu depend on
+ *                                   (n, lambda) only, so they are shared. */
+DES_API int des_noise_fill_sweep(float *z_out_dev, int64_t n_runs, int64_t run_size, int64_t P, const des_run_hp *hp_dev,
+                                 uint64_t generation, uint32_t stream_tag, void *stream);
+DES_API int des_rollout_eval_solutions_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
+                                             double *obs_totals_out_dev, const float *rows_dev, const float *obs_stats_dev,
+                                             int env, des_dims dims, int32_t repetitions, double clip,
+                                             const des_run_hp *hp_dev, uint64_t generation, int64_t n_runs,
+                                             int64_t run_size, void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API size_t des_cma_rank_mu_runs_workspace_bytes(int64_t n_runs, int64_t lambda, int64_t n);
+DES_API int des_cma_rank_mu_runs(float *out_dev, const float *Y_dev, const float *w_dev, int64_t n_runs, int64_t lambda,
+                                 int64_t n, void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API int des_cma_cov_apply_runs(float *C_dev, const float *dC_dev, const float *pc_dev, const double *decay_dev,
+                                   double c1, double cmu, int64_t n_runs, int64_t n, void *stream);
 
 /* ---- fused sample + forward + fitness ------------------------------------------------------ */
 
