@@ -279,6 +279,29 @@ class Worker:
         self.tests_run += 1
         return ret
 
+    def _recorder(self):
+        if not isinstance(self.source, fitness.DeviceRollouts):
+            raise TypeError('%s: episodes are recorded on the device\'s closed-loop environments only (DeviceRollouts); '
+                            'a host-stepped environment\'s own code sees every step, and a tape has no episodes'
+                            % type(self.source).__name__)
+        return self.source
+
+    def record_test_episodes(self, solution, repetitions=None):
+        """fitness.Trajectories [repetitions, horizon, ...] of the test episodes the next test_returns(solution,
+        repetitions) runs (generation word tests_run; repetitions default to the config's test_repetitions, as test()
+        runs them): its returns are that call's.  Advances nothing, tests_run included."""
+        src = self._recorder()
+        sol = torch.as_tensor(np.asarray(solution.detach().cpu() if isinstance(solution, torch.Tensor) else solution,
+                                         dtype=np.float32)).reshape(-1).to(self.device)
+        reps = repetitions or getattr(self.config, 'test_repetitions', None) or src.test_repetitions
+        return src.record(sol, repetitions=int(reps), noiseless=True, generation=self.tests_run).episode(0)
+
+    def record_solutions(self, solutions, member_offset=0, generation=0):
+        """fitness.Trajectories [n, repetitions, horizon, ...] of the episodes run(solutions, member_offset, generation)
+        runs: -mean of each row's returns, summed in fp64, is its cost bit for bit.  Advances nothing."""
+        rows = torch.as_tensor(solutions).to(device=self.device, dtype=torch.float32).contiguous()
+        return self._recorder().record(rows, member_offset=member_offset, generation=generation)
+
     def merge_obs_stats(self, es):
         """cma_es.py:92-96: the statistics of this generation's observations, summed over ranks, merged into [m|v|n]."""
         self.source.share_totals(es.group)
@@ -397,6 +420,8 @@ class SweepWorker:
         self.obs_stats, self.obs_totals = self.source.obs_stats, self.source.obs_totals
         self.tests_run = 0
         self.fitness = None
+        self.task, self.run_keys = getattr(c, 'task', None), [(x.seed, float(x.action_noise_std)) for x in configs]
+        self.test_repetitions = c.test_repetitions
 
     def run(self, rows, generation, running):
         """cost [R, lambda] (-mean return, cma_es.py:28) of every run's solutions rows [R * lambda, n]."""
@@ -415,6 +440,27 @@ class SweepWorker:
         ret = self.source.test_returns(solutions, self.hp, int(repetitions), self.tests_run, running)
         self.tests_run += 1
         return ret
+
+    def record_test_episodes(self, solution, run, repetitions=None):
+        """fitness.Trajectories [repetitions, horizon, ...] of run `run`'s test episodes of `solution` as the next
+        test_returns runs them: Worker.record_test_episodes under the run's seed and action noise, at member offset 0,
+        with its statistics.  Its returns are that call's row `run`.  Advances nothing."""
+        if self.host:
+            raise TypeError('SweepWorker: episodes are recorded on the device\'s closed-loop environments only; a '
+                            'host-stepped environment\'s own code sees every step')
+        r = int(run)
+        if not 0 <= r < self.R:
+            raise ValueError('record_test_episodes: run %r is not in [0, %d)' % (run, self.R))
+        s = self.source
+        seed, noise = self.run_keys[r]
+        src = fitness.DeviceRollouts(self.kn, self.device, task=self.task, hidden=s.H, repetitions=s.repetitions,
+                                     clip=s.clip, horizon=s.horizon, action_noise_std=noise, seed=seed,
+                                     normalize_obs=s.normalize_obs, sigma=None, mirrored=False)
+        src.obs_stats = None if self.obs_stats is None else self.obs_stats[r]      # a view: the run's statistics now
+        sol = torch.as_tensor(np.asarray(solution.detach().cpu() if isinstance(solution, torch.Tensor) else solution,
+                                         dtype=np.float32)).reshape(-1).to(self.device)
+        return src.record(sol, repetitions=int(repetitions or self.test_repetitions), noiseless=True,
+                          generation=self.tests_run).episode(0)
 
     def merge_obs_stats(self, running):
         """Worker.merge_obs_stats of every running run; a stopped run's statistics stay as they were at its stop."""
@@ -533,6 +579,21 @@ def _fetch_member(es, solutions_local, index):
     i = index - es.offset
     mine = solutions_local[i:i + 1] if 0 <= i < es.n_local else solutions_local[:0]
     return es.group.gather(mine, 0, 1)[0]
+
+
+def record(config, solution, stats, worker=None):
+    """test() recorded: fitness.Trajectories [test_repetitions, horizon, ...] of the test episodes whose mean test(config,
+    solution, stats, worker) reports, with the same statistics (`stats`, if given, replaces the worker's first, as in
+    test()).  Closed-loop device configs only.  Without a worker the episodes are keyed as the first test() of train()
+    keys them.  Advances nothing."""
+    if not getattr(config, 'closed_loop', False):
+        raise ValueError('cma_es.record: episodes are recorded on the device\'s closed-loop environments only '
+                         '(ClosedLoopPendulumConfig); a host-stepped environment\'s own code sees every step, and a tape '
+                         'has no episodes')
+    worker = worker if worker is not None else Worker(0, StaticNormalizer(config.state_dim), None, None, None, config)
+    if stats is not None and worker.obs_stats is not None:
+        worker.obs_stats.copy_(torch.as_tensor(np.asarray(stats, dtype=np.float32)))
+    return worker.record_test_episodes(solution, config.test_repetitions)
 
 
 def test(config, solution, stats, worker=None):

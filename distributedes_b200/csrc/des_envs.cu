@@ -18,14 +18,15 @@ namespace des {
 // makes the n_local members a batch of runs of run_size (des_rollout_eval_runs, member_offset 0): `weights` and
 // `obs_stats_dev` hold one row per run, and the observation totals are reduced per run.  A table hp_dev makes that batch a
 // sweep (des_rollout_eval_sweep, or des_rollout_eval_solutions_sweep in rows_mode): seed, sigma and action_noise_std are
-// then each run's row of the table.
+// then each run's row of the table.  A non-NULL `record` makes the launch a recording (des_rollout_record[_solutions]): its
+// four trajectory pointers, each optional, are written beside the evaluation's outputs by the RecordArgs kernels.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                           double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
-                          const des_run_hp *hp_dev, cudaStream_t st) {
+                          const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -35,6 +36,14 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     DES_REQUIRE(repetitions >= 1 && repetitions <= 10, "%s: repetitions must be in [1, 10] (one warp each)", who);
     DES_REQUIRE(dims.tape_len >= 1, "%s: episode length (dims.tape_len) must be >= 1", who);
     DES_REQUIRE(member_range_ok(member_offset, n_local, 28), "%s: bad member range", who);
+    if (record) {           // each trajectory's element count n_local * reps * horizon * width within int64
+        const void *traj[4] = {record->states, record->obs, record->actions, record->rewards};
+        const int width[4] = {2, 3, 1, 1};
+        for (int k = 0; k < 4; ++k)
+            DES_REQUIRE(!traj[k] || n_local == 0 || dims.tape_len <= INT64_MAX / (n_local * repetitions * width[k]),
+                        "%s: trajectories of %lld members x %d episodes x %d steps exceed int64 elements", who,
+                        (long long)n_local, repetitions, dims.tape_len);
+    }
     if (n_local == 0) return DES_OK;
     DES_REQUIRE(fitness_out_dev && weights_dev, "%s: NULL pointer", who);
     RollArgs a;
@@ -61,6 +70,13 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
     const int H = dims.hidden;
     const size_t smem = sizeof(float) * ((size_t)H * H + 2 * (size_t)H * kHS + 8 + 40 + (size_t)H * 4 + 3 * (size_t)H + 4) +
                         sizeof(double) * 80;
+    if (record) {
+        RecordArgs ra = *record;
+        static_cast<RollArgs &>(ra) = a;
+        const int rc = rollout_record_launch(ra, H, rows_mode, (unsigned)n_local, smem, st);
+        if (rc != DES_OK || !obs_totals_out_dev) return rc;
+        return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
+    }
     if (run_size > 0) {
         RunArgs ra;
         static_cast<RollArgs &>(ra) = a;
@@ -119,7 +135,7 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
     return des::rollout_launch("des_rollout_eval", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               false, 0, nullptr, (cudaStream_t)stream);
+                               false, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -132,7 +148,7 @@ extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *
     return des::rollout_launch("des_rollout_eval_mirrored", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                theta_dev, false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
-                               true, 0, nullptr, (cudaStream_t)stream);
+                               true, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -144,7 +160,7 @@ extern "C" DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float 
     return des::rollout_launch("des_rollout_eval_solutions", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
                                solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip, action_noise_std,
                                seed, generation, nullptr, member_offset, n_local, 0, workspace_dev, workspace_bytes,
-                               false, 0, nullptr, (cudaStream_t)stream);
+                               false, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -161,7 +177,7 @@ extern "C" DES_API int des_rollout_eval_runs(float *fitness_out_dev, float *epis
     return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
                                obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
                                state_dev, 0, n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size,
-                               nullptr, (cudaStream_t)stream);
+                               nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -179,7 +195,7 @@ extern "C" DES_API int des_rollout_eval_sweep(float *fitness_out_dev, float *epi
     return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
                                obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, state_dev, 0,
                                n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size, hp_dev,
-                               (cudaStream_t)stream);
+                               nullptr, (cudaStream_t)stream);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
@@ -195,5 +211,37 @@ extern "C" DES_API int des_rollout_eval_solutions_sweep(float *fitness_out_dev, 
     return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, rows_dev, true,
                                obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, nullptr, 0,
                                n_runs * run_size, 0, workspace_dev, workspace_bytes, false, run_size, hp_dev,
-                               (cudaStream_t)stream);
+                               nullptr, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_record(float *fitness_out_dev, float *episode_returns_out_dev,
+                                          double *obs_totals_out_dev, const float *theta_dev, const float *obs_stats_dev,
+                                          int env, des_dims dims, int32_t repetitions, double sigma, double clip,
+                                          double action_noise_std, uint64_t seed, uint64_t generation,
+                                          const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
+                                          int mirrored, double *states_out_dev, float *obs_out_dev, float *actions_out_dev,
+                                          double *rewards_out_dev, void *workspace_dev, size_t workspace_bytes,
+                                          void *stream) {
+    des::RecordArgs rec;
+    rec.states = states_out_dev; rec.obs = obs_out_dev; rec.actions = actions_out_dev; rec.rewards = rewards_out_dev;
+    return des::rollout_launch("des_rollout_record", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev,
+                               false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
+                               generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
+                               mirrored != 0, 0, nullptr, &rec, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_record_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
+                                                    double *obs_totals_out_dev, const float *solutions_dev,
+                                                    const float *obs_stats_dev, int env, des_dims dims,
+                                                    int32_t repetitions, double clip, double action_noise_std,
+                                                    uint64_t seed, uint64_t generation, int64_t member_offset,
+                                                    int64_t n_local, double *states_out_dev, float *obs_out_dev,
+                                                    float *actions_out_dev, double *rewards_out_dev, void *workspace_dev,
+                                                    size_t workspace_bytes, void *stream) {
+    des::RecordArgs rec;
+    rec.states = states_out_dev; rec.obs = obs_out_dev; rec.actions = actions_out_dev; rec.rewards = rewards_out_dev;
+    return des::rollout_launch("des_rollout_record_solutions", fitness_out_dev, episode_returns_out_dev,
+                               obs_totals_out_dev, solutions_dev, true, obs_stats_dev, env, dims, repetitions, 0.0, clip,
+                               action_noise_std, seed, generation, nullptr, member_offset, n_local, 0, workspace_dev,
+                               workspace_bytes, false, 0, nullptr, &rec, (cudaStream_t)stream);
 }

@@ -2,7 +2,8 @@
 // des_envs.cu instantiates every kernel of des_rollout_eval[_mirrored|_solutions|_runs|_sweep], and des_envs_sweep.cu the
 // row-mode sweep kernels of des_rollout_eval_solutions_sweep: one unit of their own keeps ptxas's code for the others
 // exactly what it was before CMA-ES sweeps existed (instantiated together, rollout_pendulum_kernel<8, true, RollArgs>
-// came out scheduled differently).
+// came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
+// (RecordArgs) in a unit of their own for the same reason.
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -40,6 +41,16 @@ struct RunArgs : RollArgs {
 // of the device table hp.  The key, sigma and act_noise of the RollArgs part are unused: each CTA sets them from its row.
 struct SweepArgs : RunArgs {
     const des_run_hp *hp;              // [n_runs]
+};
+
+// The arguments of a recording (des_rollout_record[_solutions]): an evaluation that also writes, for each member i, each
+// episode e < reps and each step t < horizon, the step's row of four trajectories [n_local][reps][horizon][...].  Each
+// pointer may be NULL (not written).
+struct RecordArgs : RollArgs {
+    double *states;                    // [..][2] gym's self.state before the step: (th unwrapped, thdot)
+    float *obs;                        // [..][3] the raw observation the policy was given (what stat_part sums)
+    float *actions;                    // [..][1] the action passed to env.step: after noise and the clip, before the +-2
+    double *rewards;                   // [..]    the reward Pendulum::step returned
 };
 
 // The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
@@ -95,7 +106,9 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // population under its run's seed, with the run's sigma and action noise; the round keys are set up from that seed.
 // kRows with SweepArgs (des_rollout_eval_solutions_sweep): CTA b evaluates row b of a.rows as member b % run_size of its
 // run, under the run's seed and action noise.
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs or SweepArgs
+// Args = RecordArgs (des_rollout_record[_solutions]): RollArgs, and the lane that publishes episode ep (< reps) writes
+// each step's state, observation, action and reward; the ones of the episodes past reps, stepped all the same, are not.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs or RecordArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
@@ -177,10 +190,19 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     Pendulum env;
     env.reset((uint32_t)ep, a.reset_member_base + (a.noiseless ? 0u : (uint32_t)member_slot(a)), gen, a.key);
     double total = 0.0, osum[3] = {0, 0, 0}, osq[3] = {0, 0, 0};
+    constexpr bool kRecord = std::is_same<Args, RecordArgs>::value;
+    // a recording's row of episode ep at step t, ((member * reps + ep) * horizon + t), and whether this lane writes it;
+    // the kernels of the evaluations compile none of it
+    auto row_at = [&](int t) { return ((int64_t)blockIdx.x * a.reps + ep) * a.horizon + t; };
     for (int t = 0; t < a.horizon; ++t) {
         {
             float o[3];
-            env.observe(o);
+            env.observe(o);                                              // leaves th and thdot as they were
+            if constexpr (kRecord) {
+                const int64_t at = row_at(t);
+                if (writer && ep < a.reps && a.states) { a.states[2 * at] = env.th; a.states[2 * at + 1] = env.thdot; }
+                if (writer && ep < a.reps && a.obs) { a.obs[3 * at] = o[0]; a.obs[3 * at + 1] = o[1]; a.obs[3 * at + 2] = o[2]; }
+            }
 #pragma unroll
             for (int k = 0; k < 3; ++k) { osum[k] += (double)o[k]; osq[k] += (double)o[k] * (double)o[k]; }
             if (writer)
@@ -265,7 +287,15 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
             act = __fmaf_rn(z0, a.act_noise, act);
         }
         act = clip_keep_nan(act, a.clip);                                // config.action_clip, utils.py:134
-        total += env.step((double)act);                                  // utils.py:135-137
+        if constexpr (kRecord) {
+            const double reward = env.step((double)act);
+            total += reward;
+            const int64_t at = row_at(t);
+            if (writer && ep < a.reps && a.actions) a.actions[at] = act;
+            if (writer && ep < a.reps && a.rewards) a.rewards[at] = reward;
+        } else {
+            total += env.step((double)act);                              // utils.py:135-137
+        }
     }
     if (writer) {
         red[ep * 8] = total;
@@ -292,5 +322,8 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
 // rollout_pendulum_kernel<H / 16, true, SweepArgs> over `blocks` CTAs (des_rollout_eval_solutions_sweep), defined in
 // des_envs_sweep.cu
 int rollout_rows_sweep_launch(const SweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, rows_mode, RecordArgs> over `blocks` CTAs (des_rollout_record[_solutions]), defined in
+// des_envs_record.cu
+int rollout_record_launch(const RecordArgs &a, int H, bool rows_mode, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

@@ -280,6 +280,33 @@ class NESEngine:
         return self.source.test_returns(theta, int(repetitions or self.source.test_repetitions), self.generation_index,
                                         state=self.state)
 
+    # -- recorded episodes (closed-loop sources only) -------------------------------------------------------------
+    def _recorder(self):
+        if not isinstance(self.source, DeviceRollouts):
+            raise TypeError('%s: episodes are recorded on the device\'s closed-loop environments only (DeviceRollouts); '
+                            'a host-stepped environment\'s own code sees every step, and a tape has no episodes'
+                            % type(self.source).__name__)
+        return self.source
+
+    def record_test_episodes(self, repetitions=None, solution=None):
+        """fitness.Trajectories [repetitions, horizon, ...] of the test episodes test_returns(solution, repetitions) runs
+        now: the same launch recorded, so its returns are test_returns()'s.  Advances nothing."""
+        src = self._recorder()
+        theta = self.theta if solution is None else torch.as_tensor(
+            np.ascontiguousarray(solution, dtype=np.float32)).to(self.device)
+        return src.record(theta, repetitions=int(repetitions or src.test_repetitions), noiseless=True,
+                          state=self.state).episode(0)
+
+    def record_members(self, first, count):
+        """fitness.Trajectories [count, repetitions, horizon, ...] of members [first, first + count) of the population
+        as the next evaluate() runs them (mirrored pairs whole when the engine is mirrored): the returns give that
+        evaluate()'s fitness of these members bit for bit.  Advances nothing; obs_totals stay as they are."""
+        first, count = int(first), int(count)
+        if not (0 <= first and 0 <= count and first + count <= self.N):
+            raise ValueError('record_members: members [%d, %d) are not in the population of %d' % (first, first + count,
+                                                                                                  self.N))
+        return self._recorder().record(self.theta, state=self.state, member_offset=first, n_local=count)
+
     def noiseless_fitness(self, solution=None):
         return float(self.test_returns(solution).mean())
 
@@ -386,7 +413,7 @@ class RolloutRunsEngine(_RunsUpdate):
         self.k, self.device = kernels_and_device(ops_runs if kernels is None else kernels, device)
         if self.k is ops_runs and self.device.type != 'cuda':
             raise RuntimeError('distributedes_b200 needs a CUDA device, got %s: there is no CPU fallback' % self.device)
-        self.R, self.N = int(runs), int(pop_size)
+        self.R, self.N, self.task = int(runs), int(pop_size), task
         if self.R < 1:
             raise ValueError('runs must be >= 1; got %r' % (runs,))
         if not 2 <= self.N <= self.MAX_RUN_SIZE:
@@ -500,6 +527,24 @@ class RolloutRunsEngine(_RunsUpdate):
         self._rollout(repetitions=reps, sigma=0.0, state=self.state, run_size=1, noiseless=True, obs_stats=self.obs_stats,
                       out=self.test_fitness, episodes_out=episodes)
         return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
+
+    def record_test_episodes(self, run, repetitions=None):
+        """fitness.Trajectories [repetitions, horizon, ...] of run `run`'s test episodes as test_returns() runs them now,
+        from one single-population launch on its theta and statistics: its returns are test_returns()[run].  In a
+        sweep the run is RolloutEngine(seed=seeds[run]) at member offset 0; in a batch without seeds the run-batched
+        launch keys run r's action noise by member r, so the recording does too.  Advances nothing."""
+        r = int(run)
+        if not 0 <= r < self.R:
+            raise ValueError('record_test_episodes: run %r is not in [0, %d)' % (run, self.R))
+        sweep = self.hp is not None
+        src = DeviceRollouts(self.k, self.device, task=self.task, hidden=self.H, repetitions=self.repetitions,
+                             horizon=self.horizon, clip=self.clip,
+                             action_noise_std=self.action_noise_std[r] if sweep else self.action_noise_std,
+                             seed=self.seed[r] if sweep else self.seed, normalize_obs=self.normalize_obs,
+                             sigma=self.sigma[r] if sweep else self.sigma, mirrored=False)
+        src.obs_stats = None if self.obs_stats is None else self.obs_stats[r]      # a view: the run's statistics now
+        return src.record(self.theta[r], repetitions=int(repetitions or self.test_repetitions), noiseless=True,
+                          state=self.state, member_offset=0 if sweep else r).episode(0)
 
 
 class HostEnvSweepEngine(_RunsUpdate):

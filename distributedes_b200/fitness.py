@@ -8,6 +8,8 @@ last evaluation, shares and merges them over an engine.RankGroup, counts its env
 graph may capture it.  from_config builds the source a config describes, for both trainers."""
 from __future__ import annotations
 
+from typing import NamedTuple
+
 import numpy as np
 import torch
 
@@ -128,6 +130,24 @@ class _Episodes:
             self.k.obs_stats_merge_totals(self.obs_stats, self.obs_totals, self.d0)
 
 
+class Trajectories(NamedTuple):
+    """Recorded closed-loop episodes (DeviceRollouts.record): for each member, episode and step, row-major
+    [members, repetitions, horizon, ...] (the surfaces that record test episodes drop the members axis):
+    states fp64 [.., 2], gym's (th, thdot) before the step, th unwrapped; obs fp32 [.., d0], the raw observation the
+    policy was given; actions fp32 [.., A], after action noise and the clip, before the environment's own clamp; rewards
+    fp64 [..], what the step returned; returns fp32 [members, repetitions], the episode returns the evaluation writes,
+    each the fp32 of the fp64 sum of its rewards in step order."""
+    states: np.ndarray
+    obs: np.ndarray
+    actions: np.ndarray
+    rewards: np.ndarray
+    returns: np.ndarray
+
+    def episode(self, i):
+        """The trajectories of member i (a test recording's one member)."""
+        return Trajectories(*(x[i] for x in self))
+
+
 class DeviceRollouts(_Episodes):
     """Closed-loop episodes stepped on the device (SURVEY 8f row 3): Evaluator.eval utils.py:116-124 runs `repetitions`
     episodes per member, every member seeing its own observations.  Environment: a DeviceEnv task."""
@@ -182,6 +202,35 @@ class DeviceRollouts(_Episodes):
         self.k.rollout_eval(sol, repetitions=int(repetitions), sigma=0.0, member_offset=0, n_local=1, noiseless=True,
                             obs_stats=self.obs_stats, episodes_out=episodes, **word, **self._env())
         return episodes.cpu().numpy().astype(np.float64)
+
+    def record(self, weights, *, repetitions=None, noiseless=False, state=None, generation=0, member_offset=0,
+               n_local=1):
+        """Trajectories of the episodes an evaluation runs, from one des_rollout_record[_solutions] launch with this
+        source's statistics: explicit rows weights[n, P] as solutions() evaluates them, or members [member_offset,
+        member_offset + n_local) of theta as members() does (noiseless: test episodes as test_returns() runs them, keyed
+        by the generation word in `state` if given, else `generation`).  Reads the statistics and writes nothing else:
+        obs_totals stay as they are."""
+        reps, T, dev = int(repetitions or self.repetitions), self.horizon, self.device
+        rows = weights.dim() == 2
+        n = int(weights.shape[0]) if rows else int(n_local)
+        f32, f64 = torch.float32, torch.float64
+        traj = dict(states_out=torch.empty((n, reps, T, 2), dtype=f64, device=dev),
+                    obs_out=torch.empty((n, reps, T, self.d0), dtype=f32, device=dev),
+                    actions_out=torch.empty((n, reps, T, self.A), dtype=f32, device=dev),
+                    rewards_out=torch.empty((n, reps, T), dtype=f64, device=dev))
+        episodes = torch.empty((n, reps), dtype=f32, device=dev)
+        if rows:
+            self.k.rollout_record_solutions(weights, repetitions=reps, generation=generation, member_offset=member_offset,
+                                            obs_stats=self.obs_stats, episodes_out=episodes, **traj, **self._env())
+        else:
+            word = dict(state=state) if state is not None else dict(generation=generation)
+            theta = weights.reshape(-1).to(device=dev, dtype=f32).contiguous()
+            self.k.rollout_record(theta, repetitions=reps, sigma=0.0 if noiseless else self.sigma,
+                                  mirrored=self.mirrored and not noiseless, member_offset=member_offset, n_local=n,
+                                  noiseless=noiseless, obs_stats=self.obs_stats, episodes_out=episodes, **word, **traj,
+                                  **self._env())
+        return Trajectories(*(traj[k].cpu().numpy() for k in ('states_out', 'obs_out', 'actions_out', 'rewards_out')),
+                            returns=episodes.cpu().numpy())
 
     def steps(self, N, group):
         return N * self.repetitions * self.horizon

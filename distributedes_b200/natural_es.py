@@ -297,6 +297,29 @@ def test(config, solution, stats, engine=None):
     return np.mean(rewards), np.std(rewards) / config.test_repetitions
 
 
+def record(config, solution, stats, engine=None):
+    """test() recorded: fitness.Trajectories [test_repetitions, horizon, ...] of the test episodes whose mean
+    test(config, solution, stats, engine) reports (solution None = the engine's theta).  Closed-loop device configs only.
+    Without an engine the episodes are keyed as the first test() of train() keys them (generation word 0), with the
+    statistics `stats` (a SharedStats, its state_dict, or None for none yet); with one, `stats` is not read, as in
+    test().  Advances nothing."""
+    if not getattr(config, 'closed_loop', False):
+        raise ValueError('natural_es.record: episodes are recorded on the device\'s closed-loop environments only '
+                         '(ClosedLoopPendulumConfig); a host-stepped environment\'s own code sees every step, and a tape '
+                         'has no episodes')
+    if engine is not None:
+        return engine.record_test_episodes(config.test_repetitions, solution)
+    k, dev = kernels_and_device()
+    src = from_config(config, k, dev, sigma=float(config.sigma), mirrored=config.mirrored)
+    if stats is not None and src.obs_stats is not None:
+        st = stats.state_dict() if hasattr(stats, 'state_dict') else stats
+        src.obs_stats.copy_(torch.from_numpy(np.concatenate([np.asarray(st[x], dtype=np.float32).reshape(-1)
+                                                             for x in ('m', 'v', 'n')])))
+    theta = config.initial_weight if solution is None else solution
+    theta = torch.as_tensor(np.ascontiguousarray(theta, dtype=np.float32).reshape(-1)).to(dev)
+    return src.record(theta, repetitions=config.test_repetitions, noiseless=True, generation=0).episode(0)
+
+
 def _launch_entry(rank, world_size, config_fn, port, result_path):
     torch.cuda.set_device(rank)
     dist.init_process_group('nccl', init_method='tcp://127.0.0.1:%d' % port, rank=rank, world_size=world_size)

@@ -187,9 +187,10 @@ def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions
 
 
 def _rollout(fn, weights, name, noise, env, hidden, horizon, repetitions, clip, action_noise_std, seed, generation,
-             member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out):
+             member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out, record=None):
     """The launch of rollout_eval[_mirrored] (weights = theta[P], noise = (sigma, state, noiseless)) and of
-    rollout_eval_solutions (weights = solutions[n_local, P], noise = None)."""
+    rollout_eval_solutions (weights = solutions[n_local, P], noise = None); `record` = (mirrored, states_out, obs_out,
+    actions_out, rewards_out) makes it the launch of rollout_record[_solutions]."""
     d0, A = _env_dims(env)
     P, mlp = _mlp(d0, int(hidden), A)
     n_local, reps, w, dev = int(n_local), int(repetitions), 2 * d0 + 1, weights.device
@@ -202,12 +203,20 @@ def _rollout(fn, weights, name, noise, env, hidden, horizon, repetitions, clip, 
             _ptr(weights, name, F32, P, need=mlp) if noise else _ptr(weights, name, F32, n_local * P, need=mlp + ' n x P ='),
             _ptr(obs_stats, 'obs_stats', F32, w, dev, True), int(env), Dims(d0, hidden, A, horizon), reps)
     tail = (float(clip), float(action_noise_std), int(seed), int(generation))
+    traj = ()
+    if record is not None:    # the four trajectories [n_local, reps, horizon, width], after the evaluation's arguments
+        steps = n_local * reps * int(horizon)
+        traj = tuple(_ptr(t, nm, dt, steps * width, dev, True) for t, (nm, dt, width) in zip(
+            record[1:], (('states_out', F64, 2), ('obs_out', F32, d0), ('actions_out', F32, A), ('rewards_out', F64, 1))))
     if noise:     # des_rollout_eval[_mirrored]: sigma before clip, state after the generation, noiseless after n_local
         sigma, state, noiseless = noise
         args = head + (float(sigma),) + tail + (_ptr(state, 'state', U8, STATE_BYTES, dev, True), int(member_offset),
                                                 n_local, 1 if noiseless else 0)
+        if record is not None:
+            args += (1 if record[0] else 0,)
     else:
         args = head + tail + (int(member_offset), n_local)
+    args += traj
     _launch(fn, weights, name, *args, *_ws(workspace, dev))
     return out
 
@@ -427,3 +436,8 @@ def _cov_apply(fn, Cmat, dC, name, packed, pc, decay, c1, cmu):
     _launch(fn, Cmat, 'Cmat', _ptr(Cmat, 'Cmat', F32, n * n), _ptr(dC, name, F32, cma_packed_elems(n) if packed else n * n, dev),
             _ptr(pc, 'pc', F32, n, dev, True), n, decay, c1, cmu)
     return Cmat
+
+
+# The recordings of closed-loop episodes: defined in ops_record on this module's launcher, listed here so that ops is
+# the whole set of single-population ops.
+from .ops_record import rollout_record, rollout_record_solutions  # noqa: E402,F401

@@ -100,6 +100,8 @@ def nes_apply_runs(theta, adam_m, adam_v, partial_sum, N, state, *, sigma, learn
             int(N), Opt(sigma, learning_rate, weight_decay, beta1, beta2, epsilon),
             _ptr(state, 'state', U8, STATE_BYTES, dev))
 
+# The recordings of one population (RolloutRunsEngine.record_test_episodes records one run at a time): ops.py's.
+from .ops import rollout_record, rollout_record_solutions  # noqa: E402,F401
 # The sweep ops (seeds and NES hyper-parameters per run): defined in ops_sweep, listed here so that this module stays the
 # whole set of device ops engine.RolloutRunsEngine and engine.HostEnvSweepEngine call.
 from .ops_sweep import (nes_apply_sweep, nes_grad_partial_sweep, nes_perturb_sweep, obs_parts_reduce_runs,  # noqa: E402,F401

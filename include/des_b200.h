@@ -173,6 +173,44 @@ DES_API int des_rollout_eval_solutions(float *fitness_out_dev, float *episode_re
                                        uint64_t generation, int64_t member_offset, int64_t n_local, void *workspace_dev,
                                        size_t workspace_bytes, void *stream);
 
+/* ---- recorded episodes: what a closed-loop evaluation did, step by step ---------------------------------------------
+ *
+ * A recording takes exactly the arguments of the evaluation it records and writes that evaluation's fitness, episode
+ * returns and observation totals bit for bit as it does, plus, for member i < n_local, episode e < repetitions and step
+ * t < dims.tape_len, row (i, e, t) of four trajectories laid out row-major [n_local][repetitions][tape_len][width]:
+ *
+ *   states_out_dev   fp64, width 2   gym's self.state before the step: (th, thdot), th unwrapped as the kernel keeps it
+ *   obs_out_dev      fp32, width 3   the raw observation the policy was given, before the normaliser
+ *   actions_out_dev  fp32, width 1   the action passed to env.step: after action noise and the clip to +-clip (NaN kept),
+ *                                    before Pendulum's own +-2 clamp (utils.py:133-135)
+ *   rewards_out_dev  fp64, width 1   the reward env.step returned (-cost)
+ *
+ * Each trajectory pointer may be NULL (not written).  Two identities hold bit for bit:
+ *   returns  episode return (i, e) = fp32 of the fp64 sum of rewards[i][e][t] over t in order, from 0.0;
+ *   totals   member i's observation totals are the fp64 sums over e in order of (the sums over t in order of
+ *            (double)obs and of its square), and its count is repetitions * tape_len; obs_totals_out_dev sums the
+ *            members' in member order.
+ * Both make every check of their evaluation counterpart before any CUDA work, and refuse a trajectory whose element
+ * count n_local * repetitions * tape_len * width exceeds INT64_MAX.  n_local == 0 does nothing and accepts NULL pointers.
+ *
+ * des_rollout_record            des_rollout_eval (mirrored == 0) or des_rollout_eval_mirrored (mirrored != 0; with
+ *                               noiseless != 0 refused as there): members, or with noiseless test episodes.
+ * des_rollout_record_solutions  des_rollout_eval_solutions: explicit rows. */
+DES_API int des_rollout_record(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                               const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                               int32_t repetitions, double sigma, double clip, double action_noise_std, uint64_t seed,
+                               uint64_t generation, const des_state *state_dev, int64_t member_offset, int64_t n_local,
+                               int noiseless, int mirrored, double *states_out_dev, float *obs_out_dev,
+                               float *actions_out_dev, double *rewards_out_dev, void *workspace_dev,
+                               size_t workspace_bytes, void *stream);
+DES_API int des_rollout_record_solutions(float *fitness_out_dev, float *episode_returns_out_dev,
+                                         double *obs_totals_out_dev, const float *solutions_dev,
+                                         const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
+                                         double clip, double action_noise_std, uint64_t seed, uint64_t generation,
+                                         int64_t member_offset, int64_t n_local, double *states_out_dev,
+                                         float *obs_out_dev, float *actions_out_dev, double *rewards_out_dev,
+                                         void *workspace_dev, size_t workspace_bytes, void *stream);
+
 /* Chan merge (utils.py:85-96) of a batch given by obs_totals_dev = [sum (d0) | sum of squares (d0) | count] into
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
 DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim, void *stream);
