@@ -64,6 +64,8 @@ constexpr uint32_t kStreamNesEps = 0u;
 constexpr uint32_t kStreamCmaZ = 1u;
 constexpr uint32_t kStreamEnvReset = 2u;
 constexpr uint32_t kStreamActNoise = 3u;
+// Stream 4 is the host's episode seed (envs.py).  Stream 5: the genetic algorithm's parent draws (ga_parent).
+constexpr uint32_t kStreamGaParent = 5u;
 // Member word of the test episodes' resets (test(), natural_es.py:101-110): no member of a population reaches it.
 constexpr uint32_t kTestEpisodeMember = 0x40000000u;
 
@@ -213,6 +215,13 @@ __device__ __forceinline__ float4 noise_quad(uint32_t q, uint32_t member, uint32
     box_muller(x.x, x.y, z.x, z.y);
     box_muller(x.z, x.w, z.z, z.w);
     return z;
+}
+
+// The genetic algorithm's parent of member m at generation `gen` in a table of n_parents rows (include/des_b200.h,
+// "genetic algorithm"): (x * n_parents) >> 32 of the first word x of Philox(0, m, gen, 5).  For members past the elites.
+__device__ __forceinline__ uint32_t ga_parent(uint32_t member, uint32_t gen, uint32_t n_parents, const PhiloxKey &key) {
+    const uint32_t x = philox4x32(0u, member, gen, kStreamGaParent, key).x;
+    return (uint32_t)(((uint64_t)x * n_parents) >> 32);
 }
 
 // The generation word of the counters: des_state's generation when the caller passes one (graph replay), else `gen`,

@@ -19,14 +19,16 @@ namespace des {
 // `obs_stats_dev` hold one row per run, and the observation totals are reduced per run.  A table hp_dev makes that batch a
 // sweep (des_rollout_eval_sweep, or des_rollout_eval_solutions_sweep in rows_mode): seed, sigma and action_noise_std are
 // then each run's row of the table.  A non-NULL `record` makes the launch a recording (des_rollout_record[_solutions]): its
-// four trajectory pointers, each optional, are written beside the evaluation's outputs by the RecordArgs kernels.
+// four trajectory pointers, each optional, are written beside the evaluation's outputs by the RecordArgs kernels.  A
+// non-NULL `ga` makes it a genetic-algorithm generation (des_rollout_eval_ga): `weights` is then its parents table.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
                           double clip, double action_noise_std, uint64_t seed, uint64_t generation,
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
-                          const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st) {
+                          const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st,
+                          const GaArgs *ga = nullptr) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -74,6 +76,15 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
         RecordArgs ra = *record;
         static_cast<RollArgs &>(ra) = a;
         const int rc = rollout_record_launch(ra, H, rows_mode, (unsigned)n_local, smem, st);
+        if (rc != DES_OK || !obs_totals_out_dev) return rc;
+        return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
+    }
+    if (ga) {
+        GaArgs g = *ga;
+        static_cast<RollArgs &>(g) = a;
+        g.theta = nullptr;
+        g.parents = weights_dev;
+        const int rc = rollout_ga_launch(g, H, (unsigned)n_local, smem, st);
         if (rc != DES_OK || !obs_totals_out_dev) return rc;
         return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
     }
@@ -136,6 +147,27 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
                                false, 0, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_ga(float *fitness_out_dev, float *episode_returns_out_dev,
+                                           double *obs_totals_out_dev, const float *parents_dev, int64_t n_parents,
+                                           int64_t n_elites, const float *obs_stats_dev, int env, des_dims dims,
+                                           int32_t repetitions, double sigma, double clip, double action_noise_std,
+                                           uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                           int64_t member_offset, int64_t n_local, int noiseless, void *workspace_dev,
+                                           size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_ga";
+    DES_REQUIRE(!noiseless, "%s: test episodes (noiseless) evaluate one row; use des_rollout_eval on it", who);
+    DES_REQUIRE(n_parents >= 1 && n_parents <= INT32_MAX, "%s: n_parents must be in [1, 2^31) (got %lld)", who,
+                (long long)n_parents);
+    DES_REQUIRE(n_elites >= 0 && n_elites <= n_parents, "%s: n_elites must be in [0, n_parents = %lld] (got %lld)", who,
+                (long long)n_parents, (long long)n_elites);
+    des::GaArgs ga;
+    ga.n_parents = (int)n_parents; ga.n_elites = (int)n_elites;
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, parents_dev, false,
+                               obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
+                               state_dev, member_offset, n_local, 0, workspace_dev, workspace_bytes, false, 0, nullptr,
+                               nullptr, (cudaStream_t)stream, &ga);
 }
 
 extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,

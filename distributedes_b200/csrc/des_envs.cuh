@@ -3,7 +3,8 @@
 // row-mode sweep kernels of des_rollout_eval_solutions_sweep: one unit of their own keeps ptxas's code for the others
 // exactly what it was before CMA-ES sweeps existed (instantiated together, rollout_pendulum_kernel<8, true, RollArgs>
 // came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
-// (RecordArgs) in a unit of their own for the same reason.
+// (RecordArgs) in a unit of their own for the same reason, and des_envs_ga.cu the genetic algorithm's kernels of
+// des_rollout_eval_ga (GaArgs).
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -51,6 +52,14 @@ struct RecordArgs : RollArgs {
     float *obs;                        // [..][3] the raw observation the policy was given (what stat_part sums)
     float *actions;                    // [..][1] the action passed to env.step: after noise and the clip, before the +-2
     double *rewards;                   // [..]    the reward Pendulum::step returned
+};
+
+// The arguments of a genetic-algorithm generation (des_rollout_eval_ga): member m's weights are row m of the parents
+// table for m < n_elites, else fmaf(sigma, eps_m, parents[ga_parent(m)]) (include/des_b200.h, "genetic algorithm").
+// theta is unused.
+struct GaArgs : RollArgs {
+    const float *parents;              // [n_parents][P]
+    int n_parents, n_elites;
 };
 
 // The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
@@ -108,7 +117,9 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // run, under the run's seed and action noise.
 // Args = RecordArgs (des_rollout_record[_solutions]): RollArgs, and the lane that publishes episode ep (< reps) writes
 // each step's state, observation, action and reward; the ones of the episodes past reps, stepped all the same, are not.
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs or RecordArgs
+// Args = GaArgs (des_rollout_eval_ga, kRows false): the member's weights are built from its row of the parents table:
+// an elite's row as it is, any other member's parent row plus sigma*eps of the member, through the same stage().
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs or GaArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
@@ -152,6 +163,24 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
         // ---- explicit solution row (cma_es.py:27-28).  P is odd, so rows are not 16-byte aligned: coalesced scalar loads
         const float *row = a.rows + (int64_t)blockIdx.x * L.P;
         for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
+    } else if constexpr (std::is_same<Args, GaArgs>::value) {
+        // ---- an elite's parent row as it is, any other member's parent row + sigma*eps (P is odd: scalar loads)
+        if (member < (uint32_t)a.n_elites) {
+            const float *row = a.parents + (int64_t)member * L.P;
+            for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
+        } else {
+            const float *row = a.parents + (int64_t)ga_parent(member, gen, (uint32_t)a.n_parents, a.key) * L.P;
+            for (int q = lane; q < (L.P + 3) / 4; q += 32) {
+                const float4 z = noise_quad((uint32_t)q, member, gen, kStreamNesEps, a.key);
+                const float zz[4] = {z.x, z.y, z.z, z.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int j = 4 * q + e;
+                    if (j >= L.P) break;
+                    stage(j, __fmaf_rn(a.sigma, zz[e], __ldg(row + j)));
+                }
+            }
+        }
     } else {
         // ---- theta' = theta + sigma*eps for this member -> shared memory (natural_es.py:28-30)
         const uint32_t word = noise_word(member, a.mirrored);
@@ -325,5 +354,7 @@ int rollout_rows_sweep_launch(const SweepArgs &a, int H, unsigned blocks, size_t
 // rollout_pendulum_kernel<H / 16, rows_mode, RecordArgs> over `blocks` CTAs (des_rollout_record[_solutions]), defined in
 // des_envs_record.cu
 int rollout_record_launch(const RecordArgs &a, int H, bool rows_mode, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, false, GaArgs> over `blocks` CTAs (des_rollout_eval_ga), defined in des_envs_ga.cu
+int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

@@ -194,6 +194,18 @@ class DeviceRollouts(_Episodes):
                                           workspace=self._workspace(n), out=out, **self._env())
         return out
 
+    def ga_members(self, parents, n_elites, generation, offset, n_local, out):
+        """The genetic algorithm's members [offset, offset + n_local) of `generation`, whose table is parents[T_g, P]
+        with n_elites elites, evaluated by des_rollout_eval_ga: solutions() of genetic.GeneticAlgorithm.ask()'s rows, bit
+        for bit, with each member's weights built on the device.  The sigma is this source's."""
+        self.obs_totals.zero_()
+        if n_local:
+            self.k.rollout_eval_ga(parents, n_elites, repetitions=self.repetitions, sigma=self.sigma,
+                                   generation=generation, member_offset=offset, n_local=n_local,
+                                   obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                                   workspace=self._workspace(n_local), out=out, **self._env())
+        return out
+
     def test_returns(self, solution, repetitions, generation, state=None):
         """Noiseless episodes from the test stream, keyed by the generation word in `state` if given, else `generation`."""
         sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()

@@ -441,3 +441,5 @@ def _cov_apply(fn, Cmat, dC, name, packed, pc, decay, c1, cmu):
 # The recordings of closed-loop episodes: defined in ops_record on this module's launcher, listed here so that ops is
 # the whole set of single-population ops.
 from .ops_record import rollout_record, rollout_record_solutions  # noqa: E402,F401
+# The genetic algorithm's ops (genetic.py): defined in ops_ga on this module's checks.
+from .ops_ga import ga_order, ga_order_workspace, ga_rows, rollout_eval_ga  # noqa: E402,F401

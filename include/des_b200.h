@@ -33,6 +33,7 @@
  *     N must be even and every shard holds whole pairs: member_offset and n_local (n_members) even, or
  *     DES_ERR_INVALID_ARGUMENT before any CUDA work.  Reset states (stream 2), action noise (stream 3) and episode seeds
  *     (stream 4) stay keyed by the global member m: the two members of a pair see different episodes.
+ *   - Stream 5 draws the genetic algorithm's parents ("genetic algorithm" below).
  */
 #ifndef DES_B200_H
 #define DES_B200_H
@@ -210,6 +211,51 @@ DES_API int des_rollout_record_solutions(float *fitness_out_dev, float *episode_
                                          int64_t member_offset, int64_t n_local, double *states_out_dev,
                                          float *obs_out_dev, float *actions_out_dev, double *rewards_out_dev,
                                          void *workspace_dev, size_t workspace_bytes, void *stream);
+
+/* ---- genetic algorithm: truncation selection, elites and Gaussian mutation (Such et al. 2017) -------------------------
+ *
+ * Population N >= 2, truncation T (1 <= T <= N), elites E (0 <= E <= T), mutation power sigma, P = des_param_count.
+ *   Parents table  generation g has parents[T_g][P] fp32: generation 0 one row (the start point, T_0 = 1), every later
+ *                  generation T_g = T rows.  E_g = min(E, T_g) is the n_elites the entry points take.
+ *   Member m of g  m < E_g: its weights are parents[m] as they are.  Otherwise its parent is p = (x * T_g) >> 32, x the
+ *                  first word of Philox(0, m, g, stream 5) (noise contract above: counter (0, m, g, 5), key = seed), and
+ *                  its weights are fmaf(fp32(sigma), eps_m[j], parents[p][j]), eps_m the stream-0 row of member m of
+ *                  generation g (des_noise_fill's row).  So with a one-row table [theta] and E_g = 0 the members are
+ *                  des_nes_perturb(theta)'s rows, bit for bit.
+ *   Episodes       resets (stream 2) and action noise (stream 3) are keyed by the global member m and g, exactly as
+ *                  des_rollout_eval_solutions keys row m; fitness is the mean return over `repetitions`.
+ *   Selection      members ordered by fitness, descending: ties to the lower index, NaN last, -0 == +0.  The next
+ *                  table's row k (k < T) is the weights of the member in position k, regenerated bit-identically to what
+ *                  was evaluated (des_ga_rows with members = des_ga_order's order).  Elites are re-evaluated each
+ *                  generation on fresh episodes.
+ *
+ * des_ga_rows            rows_out[n_local][P]: row i is member members_dev[i] (int32, device; the caller keeps them below
+ *                        2^31), or member_offset + i when members_dev is NULL (then member_offset + n_local <= 2^32), of
+ *                        the generation whose table is parents[n_parents][P] with n_elites elites.  rows_out may not
+ *                        overlap parents (DES_ERR_INVALID_ARGUMENT): the table is double-buffered.  The rows of a
+ *                        generation for host-stepped environments and the tape, and the gather of the next table.
+ * des_rollout_eval_ga    des_rollout_eval's closed-loop evaluation of members [member_offset, member_offset + n_local) of
+ *                        the generation whose table is parents_dev[n_parents][P], each member's weights built in shared
+ *                        memory (no rows in memory): fitness, episode returns and observation totals equal those of
+ *                        des_rollout_eval_solutions on des_ga_rows' rows at the same member_offset, bit for bit.  The
+ *                        checks of des_rollout_eval, and noiseless != 0, n_parents < 1 and n_elites outside
+ *                        [0, n_parents] are refused.
+ * des_ga_order           order_out[T] int32: the members in positions 0 .. T-1 of the selection order of fitness_dev[N]
+ *                        (N >= 2, 1 <= T <= N); workspace: des_ga_order_workspace_bytes(N) bytes, or DES_ERR_WORKSPACE.
+ *                        It ranks -fitness with des_centered_rank (counting up to N = 2048, bucketed above).
+ * n_local == 0 does nothing and accepts NULL pointers. */
+DES_API int des_ga_rows(float *rows_out_dev, const float *parents_dev, int64_t n_parents, int64_t n_elites, int64_t P,
+                        double sigma, uint64_t seed, uint64_t generation, int64_t member_offset, int64_t n_local,
+                        const int32_t *members_dev, void *stream);
+DES_API int des_rollout_eval_ga(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                const float *parents_dev, int64_t n_parents, int64_t n_elites, const float *obs_stats_dev,
+                                int env, des_dims dims, int32_t repetitions, double sigma, double clip,
+                                double action_noise_std, uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                int64_t member_offset, int64_t n_local, int noiseless, void *workspace_dev,
+                                size_t workspace_bytes, void *stream);
+DES_API size_t des_ga_order_workspace_bytes(int64_t N);
+DES_API int des_ga_order(int32_t *order_out_dev, const float *fitness_dev, int64_t N, int64_t T, void *workspace_dev,
+                         size_t workspace_bytes, void *stream);
 
 /* Chan merge (utils.py:85-96) of a batch given by obs_totals_dev = [sum (d0) | sum of squares (d0) | count] into
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
