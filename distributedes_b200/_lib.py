@@ -37,6 +37,11 @@ class RunHp(C.Structure):
                 ('weight_decay', C.c_double), ('action_noise_std', C.c_double)]
 
 
+class GaRun(C.Structure):
+    """des_ga_run: one run's row of a genetic-algorithm sweep's count table (16 bytes, kept in device memory)."""
+    _fields_ = [('n_parents', C.c_int32), ('n_elites', C.c_int32), ('truncation', C.c_int32), ('pad', C.c_int32)]
+
+
 _P, _I64, _U64, _U32, _I32, _D, _SZ = C.c_void_p, C.c_int64, C.c_uint64, C.c_uint32, C.c_int32, C.c_double, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol include/des_b200.h declares (tests check this)
@@ -89,6 +94,11 @@ SIGNATURES = {
     'des_cma_rank_mu_runs_workspace_bytes': (_SZ, [_I64, _I64, _I64]),
     'des_cma_rank_mu_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
     'des_cma_cov_apply_runs': (C.c_int, [_P, _P, _P, _P, _D, _D, _I64, _I64, _P]),
+    'des_rollout_eval_ga_sweep': (C.c_int, [_P, _P, _P, _P, _P, _I64, _P, C.c_int, Dims, _I32, _D, _P, _U64, _P, _I64,
+                                            _I64, _P, C.c_size_t, _P]),
+    'des_ga_rows_sweep': (C.c_int, [_P, _P, _P, _I64, _I64, _P, _U64, _I64, _I64, _P, _P]),
+    'des_ga_order_runs_workspace_bytes': (_SZ, [_I64, _I64]),
+    'des_ga_order_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_nes_eval_mirrored': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),

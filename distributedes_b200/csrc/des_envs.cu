@@ -20,7 +20,9 @@ namespace des {
 // sweep (des_rollout_eval_sweep, or des_rollout_eval_solutions_sweep in rows_mode): seed, sigma and action_noise_std are
 // then each run's row of the table.  A non-NULL `record` makes the launch a recording (des_rollout_record[_solutions]): its
 // four trajectory pointers, each optional, are written beside the evaluation's outputs by the RecordArgs kernels.  A
-// non-NULL `ga` makes it a genetic-algorithm generation (des_rollout_eval_ga): `weights` is then its parents table.
+// non-NULL `ga` makes it a genetic-algorithm generation (des_rollout_eval_ga): `weights` is then its parents table.  A
+// non-NULL `ga_sweep` with a table hp_dev makes the sweep one of genetic-algorithm runs (des_rollout_eval_ga_sweep):
+// `weights` is then the buffer of every run's parents table.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
@@ -28,7 +30,7 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
                           const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st,
-                          const GaArgs *ga = nullptr) {
+                          const GaArgs *ga = nullptr, const GaSweepArgs *ga_sweep = nullptr) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -96,6 +98,15 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
             SweepArgs sa;
             static_cast<RunArgs &>(sa) = ra;
             sa.hp = hp_dev;
+            if (ga_sweep) {
+                GaSweepArgs g = *ga_sweep;
+                static_cast<SweepArgs &>(g) = sa;
+                g.theta = nullptr;
+                g.parents = weights_dev;
+                const int rc = rollout_ga_sweep_launch(g, H, (unsigned)n_local, smem, st);
+                if (rc != DES_OK || !obs_totals_out_dev) return rc;
+                return obs_parts_reduce_runs(obs_totals_out_dev, a.stat_part, n_local / run_size, run_size, 7, st);
+            }
             void (*sweep_kernel)(SweepArgs);
             switch (H / 16) {
                 case 1: sweep_kernel = rollout_pendulum_kernel<1, false, SweepArgs>; break;
@@ -168,6 +179,28 @@ extern "C" DES_API int des_rollout_eval_ga(float *fitness_out_dev, float *episod
                                obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
                                state_dev, member_offset, n_local, 0, workspace_dev, workspace_bytes, false, 0, nullptr,
                                nullptr, (cudaStream_t)stream, &ga);
+}
+
+extern "C" DES_API int des_rollout_eval_ga_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
+                                                 double *obs_totals_out_dev, const float *parents_dev,
+                                                 const des_ga_run *ga_dev, int64_t table_rows, const float *obs_stats_dev,
+                                                 int env, des_dims dims, int32_t repetitions, double clip,
+                                                 const des_run_hp *hp_dev, uint64_t generation, const des_state *state_dev,
+                                                 int64_t n_runs, int64_t run_size, void *workspace_dev,
+                                                 size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_ga_sweep";
+    const int rc = des::check_runs(who, n_runs, run_size, 2);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(table_rows >= 1 && table_rows <= run_size, "%s: table_rows must be in [1, run_size = %lld] (got %lld)", who,
+                (long long)run_size, (long long)table_rows);
+    DES_REQUIRE(n_runs == 0 || (hp_dev && ga_dev), "%s: NULL pointer", who);
+    des::GaSweepArgs ga;
+    ga.ga = ga_dev; ga.table_rows = (int)table_rows;
+    ga.n_parents = 1; ga.n_elites = 0;                  // each CTA sets its run's
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, parents_dev, false,
+                               obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, state_dev, 0,
+                               n_runs * run_size, 0, workspace_dev, workspace_bytes, false, run_size, hp_dev, nullptr,
+                               (cudaStream_t)stream, nullptr, &ga);
 }
 
 extern "C" DES_API int des_rollout_eval_mirrored(float *fitness_out_dev, float *episode_returns_out_dev,

@@ -3,8 +3,8 @@
 // row-mode sweep kernels of des_rollout_eval_solutions_sweep: one unit of their own keeps ptxas's code for the others
 // exactly what it was before CMA-ES sweeps existed (instantiated together, rollout_pendulum_kernel<8, true, RollArgs>
 // came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
-// (RecordArgs) in a unit of their own for the same reason, and des_envs_ga.cu the genetic algorithm's kernels of
-// des_rollout_eval_ga (GaArgs).
+// (RecordArgs) in a unit of their own for the same reason, des_envs_ga.cu the genetic algorithm's kernels of
+// des_rollout_eval_ga (GaArgs) and des_envs_ga_sweep.cu those of its sweeps, des_rollout_eval_ga_sweep (GaSweepArgs).
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -62,11 +62,26 @@ struct GaArgs : RollArgs {
     int n_parents, n_elites;
 };
 
+// The arguments of a genetic-algorithm sweep (des_rollout_eval_ga_sweep): a sweep (SweepArgs: the run's seed, sigma and
+// action noise from its hp row) whose CTA builds its member as a GaArgs kernel does, from its run's table of the buffer
+// parents [n_runs][table_rows][P] and the counts of its des_ga_run row, clamped so that no table read leaves the buffer.
+// The CTA sets parents, n_parents and n_elites itself; theta is unused.
+struct GaSweepArgs : SweepArgs {
+    const float *parents;              // [n_runs][table_rows][P], then the CTA's run's table
+    int n_parents, n_elites;
+    const des_ga_run *ga;              // [n_runs]
+    int table_rows;                    // >= 1
+};
+
+// The Args whose members are built from a parents table (the genetic algorithm's fill stage).
+template <typename Args>
+constexpr bool kGaFill = std::is_same<Args, GaArgs>::value || std::is_same<Args, GaSweepArgs>::value;
+
 // The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
 // except in a sweep, where every run is a population of its own.
 template <typename Args>
 __device__ __forceinline__ unsigned member_slot(const Args &a) {
-    if constexpr (std::is_same<Args, SweepArgs>::value) return blockIdx.x % (unsigned)a.run_size;
+    if constexpr (std::is_base_of<SweepArgs, Args>::value) return blockIdx.x % (unsigned)a.run_size;
     else return blockIdx.x;
 }
 
@@ -119,18 +134,27 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // each step's state, observation, action and reward; the ones of the episodes past reps, stepped all the same, are not.
 // Args = GaArgs (des_rollout_eval_ga, kRows false): the member's weights are built from its row of the parents table:
 // an elite's row as it is, any other member's parent row plus sigma*eps of the member, through the same stage().
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs or GaArgs
+// Args = GaSweepArgs (des_rollout_eval_ga_sweep, kRows false): a sweep CTA that fills as GaArgs does, from its run's
+// table and counts.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs or GaSweepArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
         const unsigned run = blockIdx.x / (unsigned)a.run_size;
-        if constexpr (!kRows) a.theta += (size_t)run * a.L.P;     // row mode: theta is NULL, CTA b reads row b of rows
+        if constexpr (!kRows && !kGaFill<Args>) a.theta += (size_t)run * a.L.P;   // NULL otherwise
         if (a.obs_stats) a.obs_stats += (size_t)run * 7;
-        if constexpr (std::is_same<Args, SweepArgs>::value) {
+        if constexpr (std::is_base_of<SweepArgs, Args>::value) {
             const des_run_hp hp = a.hp[run];
             philox_round_keys(hp.seed, a.key);                  // make_philox_key's words, as the host makes them
             a.sigma = a.noiseless ? 0.f : (float)hp.sigma;      // the host's conversions of the single call
             a.act_noise = (float)hp.action_noise_std;
+        }
+        if constexpr (std::is_same<Args, GaSweepArgs>::value) {
+            // the run's table and counts, clamped to the buffer: n_parents in [1, table_rows], n_elites in [0, n_parents]
+            const des_ga_run g = a.ga[run];
+            a.n_parents = min(max(g.n_parents, 1), a.table_rows);
+            a.n_elites = min(max(g.n_elites, 0), a.n_parents);
+            a.parents += (size_t)run * (size_t)a.table_rows * a.L.P;
         }
     }
     extern __shared__ __align__(16) float sm[];
@@ -163,7 +187,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
         // ---- explicit solution row (cma_es.py:27-28).  P is odd, so rows are not 16-byte aligned: coalesced scalar loads
         const float *row = a.rows + (int64_t)blockIdx.x * L.P;
         for (int j = lane; j < L.P; j += 32) stage(j, __ldg(row + j));
-    } else if constexpr (std::is_same<Args, GaArgs>::value) {
+    } else if constexpr (kGaFill<Args>) {
         // ---- an elite's parent row as it is, any other member's parent row + sigma*eps (P is odd: scalar loads)
         if (member < (uint32_t)a.n_elites) {
             const float *row = a.parents + (int64_t)member * L.P;
@@ -356,5 +380,8 @@ int rollout_rows_sweep_launch(const SweepArgs &a, int H, unsigned blocks, size_t
 int rollout_record_launch(const RecordArgs &a, int H, bool rows_mode, unsigned blocks, size_t smem, cudaStream_t st);
 // rollout_pendulum_kernel<H / 16, false, GaArgs> over `blocks` CTAs (des_rollout_eval_ga), defined in des_envs_ga.cu
 int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, false, GaSweepArgs> over `blocks` CTAs (des_rollout_eval_ga_sweep), defined in
+// des_envs_ga_sweep.cu
+int rollout_ga_sweep_launch(const GaSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

@@ -3,7 +3,7 @@
 //                 plus sigma*eps of the member: a generation's rows (host-stepped and tape sources), or, with a members
 //                 list, the next parents table gathered from the selected members
 //   des_ga_order  order_out[T]: the members of the T best fitnesses, best first (truncation selection)
-#include "des_common.cuh"
+#include "des_ga.cuh"
 
 namespace des {
 
@@ -18,24 +18,7 @@ __global__ void ga_rows_kernel(float *__restrict__ out, const float *__restrict_
         const int64_t i = idx / nq;
         const int64_t q = idx - i * nq;
         const uint32_t m = members ? (uint32_t)__ldg(members + i) : (uint32_t)(member_offset + i);
-        float *row = out + i * P;
-        if (m < n_elites) {
-            const float *src = parents + (int64_t)m * P;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int64_t j = 4 * q + e;
-                if (j < P) row[j] = src[j];
-            }
-        } else {
-            const float *src = parents + (int64_t)ga_parent(m, gen, n_parents, key) * P;
-            const float4 z = noise_quad((uint32_t)q, m, gen, kStreamNesEps, key);
-            const float zz[4] = {z.x, z.y, z.z, z.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int64_t j = 4 * q + e;
-                if (j < P) row[j] = __fmaf_rn(sigma, zz[e], src[j]);
-            }
-        }
+        ga_row_quad(out + i * P, parents, n_parents, n_elites, P, q, sigma, key, gen, m);
     }
 }
 

@@ -566,6 +566,20 @@ class DeviceSweep:
                                             totals_out=self.obs_totals if self.normalize_obs else None,
                                             workspace=self.roll_ws, out=out, **self._env())
 
+    def ga_members(self, parents, ga, hp, *, generation, out):
+        """fitness out[R, N] of every genetic-algorithm run's generation, whose tables are parents[R, table_rows, P] with
+        the counts of the table `ga` (des_rollout_eval_ga_sweep: each member's weights built on the device), and,
+        normalising, each run's observation totals in obs_totals: DeviceRollouts.ga_members of every run under its seed,
+        sigma and action noise, at offset 0."""
+        N, w = out.shape[1], 2 * self.d0 + 1
+        if self.roll_ws is None or self.roll_ws.numel() < self.R * N * w:
+            self.roll_ws = torch.empty(self.R * N * w, dtype=torch.float64, device=self.device)
+        self.obs_totals.zero_()
+        self.k.rollout_eval_ga_sweep(parents, ga, hp, repetitions=self.repetitions, generation=generation, run_size=N,
+                                     obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                                     workspace=self.roll_ws, out=out, **self._env())
+        return out
+
     def test_returns(self, theta, hp, repetitions, generation, running):
         """[R, repetitions] fp64: run r's noiseless episodes of theta[r] from the test stream keyed by `generation`, with
         its statistics: DeviceRollouts.test_returns under run r's seed and action noise."""

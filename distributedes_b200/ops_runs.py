@@ -109,3 +109,7 @@ from .ops_sweep import (nes_apply_sweep, nes_grad_partial_sweep, nes_perturb_swe
 # The CMA-ES sweep ops (cma_es.CMASweep, fitness.DeviceSweep): defined in ops_cma_sweep, on the same table.
 from .ops_cma_sweep import (cma_cov_apply_runs, cma_rank_mu_runs, noise_fill_sweep,  # noqa: E402,F401
                             rollout_eval_solutions_sweep)
+# The genetic-algorithm sweep ops (genetic.GASweep, fitness.DeviceSweep.ga_members): defined in ops_ga_sweep, on the same
+# table and a count table of their own.
+from .ops_ga_sweep import (ga_order_runs, ga_order_runs_workspace, ga_rows_sweep, ga_table,  # noqa: E402,F401
+                           rollout_eval_ga_sweep)

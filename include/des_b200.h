@@ -441,6 +441,62 @@ DES_API int des_cma_rank_mu_runs(float *out_dev, const float *Y_dev, const float
 DES_API int des_cma_cov_apply_runs(float *C_dev, const float *dC_dev, const float *pc_dev, const double *decay_dev,
                                    double c1, double cmu, int64_t n_runs, int64_t n, void *stream);
 
+/* ---- genetic-algorithm sweeps: R runs of N members, one launch per step for all of them -------------------------------
+ *
+ * A GA sweep is R = n_runs runs of N = run_size members (2 <= N <= 2048, R * N <= 2^28; N above 2048 is
+ * DES_ERR_UNSUPPORTED), in one process on one GPU.  Run r owns:
+ *   - its seed s_r, mutation power sigma_r and action-noise std a_r: row r of the sweep table hp_dev (des_run_hp above;
+ *     learning_rate and weight_decay are not read);
+ *   - its truncation T_r and elites E_r, and its start point x0_r (row 0 of its generation-0 table).
+ * Run r's member i is member i of a standalone GA population under s_r at member offset 0: its parent draw (stream 5), its
+ * eps (stream 0), its resets (stream 2) and its action noise (stream 3) are keyed by s_r.  So run r of a sweep is the
+ * single genetic algorithm of its own seed, sigma, action noise, T_r, E_r and x0_r, bit for bit; runs with equal entries
+ * are identical.  Shared: the generation word, N, dims, repetitions, horizon and clip.
+ *
+ * Tables.  Every run's parents table sits in one buffer [R][table_rows][P] fp32, table_rows = max_r T_r >= 1 (a host
+ * scalar, 1 <= table_rows <= N): generation 0 has one row per run (x0_r), every later generation T_r rows.  Run r's
+ * current n_parents and n_elites, and its T_r, are row r of ga_dev, a des_ga_run table in DEVICE memory.  The library
+ * cannot read that table: a count out of range is the caller's to refuse.  Whatever it holds, no kernel reads or writes
+ * outside the [R][table_rows][P] buffers: n_parents is clamped to [1, table_rows], n_elites to [0, n_parents] and the
+ * truncation to [1, min(N, table_rows)].
+ *
+ * des_rollout_eval_ga_sweep   des_rollout_eval_ga(parents_r, n_parents_r, n_elites_r, obs_stats_r, seed = s_r, sigma =
+ *                             sigma_r, action_noise_std = a_r, member_offset = 0, n_local = N) of every run: fitness
+ *                             [R][N], episode returns [R][N][repetitions], statistics and observation totals
+ *                             [R][2*state_dim+1] (workspace: R * N * (2*state_dim+1) * 8 bytes).  The checks of
+ *                             des_rollout_eval_runs, and table_rows outside [1, N].
+ * des_ga_rows_sweep           Rows mode (members_dev NULL): rows_out [R * N][P], run r's rows those of
+ *                             des_ga_rows(parents_r, n_parents_r, n_elites_r, P, sigma_r, s_r, generation, member_offset =
+ *                             0, n_local = N): a generation's rows for host-stepped environments.  Gather mode: members_dev
+ *                             [R][table_rows] int32, rows_out [R][table_rows][P], row (r, k) the weights of member
+ *                             members_dev[r][k] of run r (des_ga_rows with members); a negative entry (-1: none) leaves its
+ *                             row unwritten.  rows_out may not overlap the parents buffer (DES_ERR_INVALID_ARGUMENT).
+ * des_ga_order_runs           order_out [R][table_rows] int32: run r's first T_r entries are des_ga_order(fitness_r, T_r),
+ *                             the later ones -1, for fitness [R][N]; workspace: des_ga_order_runs_workspace_bytes(R, N)
+ *                             bytes, or DES_ERR_WORKSPACE.  It ranks -fitness with des_centered_rank_runs' counting rank.
+ * Test episodes need no entry point of their own: row 0 of each run's table is its best member; copy those rows to
+ * theta [R][P] and run des_rollout_eval_sweep with noiseless != 0 and run_size 1.
+ * n_runs == 0 does nothing and accepts NULL pointers. */
+typedef struct des_ga_run {
+    int32_t n_parents;          /* T_g of the run's current table      offset 0  */
+    int32_t n_elites;           /* E_g = min(E_r, T_g)                 offset 4  */
+    int32_t truncation;         /* T_r                                 offset 8  */
+    int32_t pad;                /*                                     offset 12 */
+} des_ga_run;                   /* 16 bytes */
+DES_API int des_rollout_eval_ga_sweep(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                      const float *parents_dev, const des_ga_run *ga_dev, int64_t table_rows,
+                                      const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double clip,
+                                      const des_run_hp *hp_dev, uint64_t generation, const des_state *state_dev,
+                                      int64_t n_runs, int64_t run_size, void *workspace_dev, size_t workspace_bytes,
+                                      void *stream);
+DES_API int des_ga_rows_sweep(float *rows_out_dev, const float *parents_dev, const des_ga_run *ga_dev, int64_t table_rows,
+                              int64_t P, const des_run_hp *hp_dev, uint64_t generation, int64_t n_runs, int64_t run_size,
+                              const int32_t *members_dev, void *stream);
+DES_API size_t des_ga_order_runs_workspace_bytes(int64_t n_runs, int64_t run_size);
+DES_API int des_ga_order_runs(int32_t *order_out_dev, const float *fitness_dev, const des_ga_run *ga_dev,
+                              int64_t table_rows, int64_t n_runs, int64_t run_size, void *workspace_dev,
+                              size_t workspace_bytes, void *stream);
+
 /* ---- fused sample + forward + fitness ------------------------------------------------------ */
 
 /* fitness_out_dev[i] (i < n_local) = sum_t -|| clip(pi_{theta+sigma*eps_m}(obs_t), -clip, clip) - target_t ||^2
