@@ -22,7 +22,8 @@ namespace des {
 // four trajectory pointers, each optional, are written beside the evaluation's outputs by the RecordArgs kernels.  A
 // non-NULL `ga` makes it a genetic-algorithm generation (des_rollout_eval_ga): `weights` is then its parents table.  A
 // non-NULL `ga_sweep` with a table hp_dev makes the sweep one of genetic-algorithm runs (des_rollout_eval_ga_sweep):
-// `weights` is then the buffer of every run's parents table.
+// `weights` is then the buffer of every run's parents table.  A non-NULL `bc` makes it an evaluation that also writes
+// each member's behaviour characterisation (des_rollout_eval_bc).
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
@@ -30,7 +31,8 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           const des_state *state_dev, int64_t member_offset, int64_t n_local, int noiseless,
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
                           const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st,
-                          const GaArgs *ga = nullptr, const GaSweepArgs *ga_sweep = nullptr) {
+                          const GaArgs *ga = nullptr, const GaSweepArgs *ga_sweep = nullptr,
+                          const BcArgs *bc = nullptr) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -49,7 +51,7 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                         (long long)n_local, repetitions, dims.tape_len);
     }
     if (n_local == 0) return DES_OK;
-    DES_REQUIRE(fitness_out_dev && weights_dev, "%s: NULL pointer", who);
+    DES_REQUIRE(fitness_out_dev && weights_dev && (!bc || bc->bc_out), "%s: NULL pointer", who);
     RollArgs a;
     a.fitness = fitness_out_dev; a.ep_ret = episode_returns_out_dev;
     a.theta = rows_mode ? nullptr : weights_dev; a.rows = rows_mode ? weights_dev : nullptr;
@@ -78,6 +80,13 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
         RecordArgs ra = *record;
         static_cast<RollArgs &>(ra) = a;
         const int rc = rollout_record_launch(ra, H, rows_mode, (unsigned)n_local, smem, st);
+        if (rc != DES_OK || !obs_totals_out_dev) return rc;
+        return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
+    }
+    if (bc) {
+        BcArgs b = *bc;
+        static_cast<RollArgs &>(b) = a;
+        const int rc = rollout_bc_launch(b, H, (unsigned)n_local, smem, st);
         if (rc != DES_OK || !obs_totals_out_dev) return rc;
         return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
     }
@@ -158,6 +167,21 @@ extern "C" DES_API int des_rollout_eval(float *fitness_out_dev, float *episode_r
                                false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
                                generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
                                false, 0, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_bc(float *fitness_out_dev, float *episode_returns_out_dev,
+                                           double *obs_totals_out_dev, const float *theta_dev, const float *obs_stats_dev,
+                                           int env, des_dims dims, int32_t repetitions, double sigma, double clip,
+                                           double action_noise_std, uint64_t seed, uint64_t generation,
+                                           const des_state *state_dev, int64_t member_offset, int64_t n_local,
+                                           int noiseless, float *bc_out_dev, void *workspace_dev, size_t workspace_bytes,
+                                           void *stream) {
+    des::BcArgs bc;
+    bc.bc_out = bc_out_dev;
+    return des::rollout_launch("des_rollout_eval_bc", fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev,
+                               theta_dev, false, obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed,
+                               generation, state_dev, member_offset, n_local, noiseless, workspace_dev, workspace_bytes,
+                               false, 0, nullptr, nullptr, (cudaStream_t)stream, nullptr, nullptr, &bc);
 }
 
 extern "C" DES_API int des_rollout_eval_ga(float *fitness_out_dev, float *episode_returns_out_dev,

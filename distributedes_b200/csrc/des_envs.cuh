@@ -5,6 +5,7 @@
 // came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
 // (RecordArgs) in a unit of their own for the same reason, des_envs_ga.cu the genetic algorithm's kernels of
 // des_rollout_eval_ga (GaArgs) and des_envs_ga_sweep.cu those of its sweeps, des_rollout_eval_ga_sweep (GaSweepArgs).
+// des_envs_bc.cu instantiates the behaviour-writing kernels of des_rollout_eval_bc (BcArgs) for novelty search.
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -73,6 +74,13 @@ struct GaSweepArgs : SweepArgs {
     int table_rows;                    // >= 1
 };
 
+// The arguments of an evaluation that also writes each member's behaviour characterisation (des_rollout_eval_bc): the
+// raw observation after the last step of each of its episodes, averaged over the repetitions (fp64 sum in episode
+// order, stored as fp32).
+struct BcArgs : RollArgs {
+    float *bc_out;                     // [n_local][d0]
+};
+
 // The Args whose members are built from a parents table (the genetic algorithm's fill stage).
 template <typename Args>
 constexpr bool kGaFill = std::is_same<Args, GaArgs>::value || std::is_same<Args, GaSweepArgs>::value;
@@ -136,7 +144,9 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // an elite's row as it is, any other member's parent row plus sigma*eps of the member, through the same stage().
 // Args = GaSweepArgs (des_rollout_eval_ga_sweep, kRows false): a sweep CTA that fills as GaArgs does, from its run's
 // table and counts.
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs or GaSweepArgs
+// Args = BcArgs (des_rollout_eval_bc, kRows false): RollArgs, and after the last step each episode's publishing lane
+// observes its state once more; lane 0 writes the member's mean of those raw observations.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs, GaSweepArgs or BcArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
@@ -247,6 +257,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     // a recording's row of episode ep at step t, ((member * reps + ep) * horizon + t), and whether this lane writes it;
     // the kernels of the evaluations compile none of it
     auto row_at = [&](int t) { return ((int64_t)blockIdx.x * a.reps + ep) * a.horizon + t; };
+    constexpr bool kBc = std::is_same<Args, BcArgs>::value;    // a behaviour-writing evaluation (after the loop)
     for (int t = 0; t < a.horizon; ++t) {
         {
             float o[3];
@@ -370,6 +381,26 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
         }
         if (lane == 6) a.stat_part[(int64_t)blockIdx.x * 7 + 6] = (double)a.reps * a.horizon;
     }
+    if constexpr (kBc) {
+        // the behaviour: the raw observation after the last step, in the reduction area once every read above is done.
+        // Observed here, after the step loop, so that the loop is the evaluation's own code and schedule
+        float bc[3];
+        env.observe(bc);
+        __syncwarp();
+        if (writer) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) red[ep * 8 + 1 + k] = (double)bc[k];
+        }
+        __syncwarp();
+        if (lane == 0) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                double s = 0.0;
+                for (int r = 0; r < a.reps; ++r) s += red[r * 8 + 1 + k];
+                a.bc_out[(int64_t)blockIdx.x * 3 + k] = (float)(s / a.reps);
+            }
+        }
+    }
 }
 
 // rollout_pendulum_kernel<H / 16, true, SweepArgs> over `blocks` CTAs (des_rollout_eval_solutions_sweep), defined in
@@ -383,5 +414,7 @@ int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cuda
 // rollout_pendulum_kernel<H / 16, false, GaSweepArgs> over `blocks` CTAs (des_rollout_eval_ga_sweep), defined in
 // des_envs_ga_sweep.cu
 int rollout_ga_sweep_launch(const GaSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, false, BcArgs> over `blocks` CTAs (des_rollout_eval_bc), defined in des_envs_bc.cu
+int rollout_bc_launch(const BcArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

@@ -193,9 +193,12 @@ class NESEngine:
         self.source.seed = int(value)
 
     # -- the three phases around the two collectives -------------------------------------------------------
-    def evaluate(self):
+    def evaluate(self, bc_out=None):
+        """Evaluates the generation's members; bc_out [n_local, d0], when given, also receives their behaviours from the
+        same episodes (closed-loop and host-stepped sources; novelty.py)."""
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
         self.source.members(self.theta, state=self.state, generation=self.generation_index, offset=self.offset,
-                            n_local=self.n_local, out=self.fitness_shard_out)
+                            n_local=self.n_local, out=self.fitness_shard_out, **bc)
         self._gather_fitness()
         self.source.share_totals(self.group)
         self.steps_taken = self.source.steps(self.N, self.group)
@@ -213,10 +216,14 @@ class NESEngine:
         else:
             self.group.gather(self.fitness_shard_out, self.offset, self.N, out=self.fitness_all)
 
-    def rank_and_reduce(self):
-        self.k.centered_rank(self.fitness_all, self.offset, self.n_local, workspace=self.rank_ws, out=self.shaped)
+    def rank_and_reduce(self, shaped=None):
+        """The shard's partial sum of shaped fitness x noise, all-reduced.  `shaped` [n_local], when given, replaces the
+        centered ranks of the fitness (novelty search's blend, novelty.py)."""
+        if shaped is None:
+            self.k.centered_rank(self.fitness_all, self.offset, self.n_local, workspace=self.rank_ws, out=self.shaped)
+            shaped = self.shaped
         grad = self.k.nes_grad_partial_mirrored if self.mirrored else self.k.nes_grad_partial
-        grad(self.shaped, self.P, seed=self.seed, state=self.state, member_offset=self.offset, workspace=self.grad_ws,
+        grad(shaped, self.P, seed=self.seed, state=self.state, member_offset=self.offset, workspace=self.grad_ws,
              out=self.partial_local if self.comm is not None else self.partial)
         if self.comm is not None:
             self.comm.allreduce_partial(self.partial_local, self.partial)   # slots over NVLink, summed in rank order
@@ -271,14 +278,16 @@ class NESEngine:
             torch.cuda.current_stream(self.device).synchronize()
 
     # -- test episodes (test(), natural_es.py:101-110) ----------------------------------------------------------
-    def test_returns(self, solution=None, repetitions=None):
-        """Returns of `repetitions` noiseless episodes of `solution` (None = theta) with the current statistics."""
+    def test_returns(self, solution=None, repetitions=None, bc_out=None):
+        """Returns of `repetitions` noiseless episodes of `solution` (None = theta) with the current statistics; bc_out
+        [1, d0], when given, also receives the solution's behaviour from the same episodes (novelty.py)."""
         theta = self.theta if solution is None else torch.as_tensor(
             np.ascontiguousarray(solution, dtype=np.float32)).to(self.device)
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
         # the generation word of the test episodes: device rollouts read it from des_state, host episodes need it on
         # the host (generation_index); the tape ignores it
         return self.source.test_returns(theta, int(repetitions or self.source.test_repetitions), self.generation_index,
-                                        state=self.state)
+                                        state=self.state, **bc)
 
     # -- recorded episodes (closed-loop sources only) -------------------------------------------------------------
     def _recorder(self):

@@ -175,13 +175,21 @@ class DeviceRollouts(_Episodes):
         return dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip,
                     action_noise_std=self.action_noise_std, seed=self.seed)
 
-    def members(self, theta, *, state, generation, offset, n_local, out):
+    def members(self, theta, *, state, generation, offset, n_local, out, bc_out=None):
+        """Fitness of members [offset, offset + n_local) into out; with bc_out [n_local, d0], also their behaviours
+        (des_rollout_eval_bc: the same fitness, bit for bit).  Behaviours of mirrored members are refused."""
+        if bc_out is not None and self.mirrored:
+            raise ValueError('DeviceRollouts: behaviours (bc_out) are written for plain members only; this source samples '
+                             'mirrored pairs')
         self.obs_totals.zero_()
         if n_local:
-            (self.k.rollout_eval_mirrored if self.mirrored else self.k.rollout_eval)(
-                theta, repetitions=self.repetitions, sigma=self.sigma, state=state, member_offset=offset, n_local=n_local,
-                obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
-                workspace=self._workspace(n_local), out=out, **self._env())
+            kw = dict(repetitions=self.repetitions, sigma=self.sigma, state=state, member_offset=offset, n_local=n_local,
+                      obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
+                      workspace=self._workspace(n_local), out=out, **self._env())
+            if bc_out is not None:
+                self.k.rollout_eval_bc(theta, bc_out=bc_out, **kw)
+            else:
+                (self.k.rollout_eval_mirrored if self.mirrored else self.k.rollout_eval)(theta, **kw)
 
     def solutions(self, solutions, *, offset, generation, out=None):
         n = int(solutions.shape[0])
@@ -206,13 +214,18 @@ class DeviceRollouts(_Episodes):
                                    workspace=self._workspace(n_local), out=out, **self._env())
         return out
 
-    def test_returns(self, solution, repetitions, generation, state=None):
-        """Noiseless episodes from the test stream, keyed by the generation word in `state` if given, else `generation`."""
+    def test_returns(self, solution, repetitions, generation, state=None, bc_out=None):
+        """Noiseless episodes from the test stream, keyed by the generation word in `state` if given, else `generation`;
+        with bc_out [1, d0], the same launch writes the solution's behaviour (des_rollout_eval_bc)."""
         sol = solution.reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
         episodes = torch.empty(int(repetitions), dtype=torch.float32, device=self.device)
         word = dict(state=state) if state is not None else dict(generation=generation)
-        self.k.rollout_eval(sol, repetitions=int(repetitions), sigma=0.0, member_offset=0, n_local=1, noiseless=True,
-                            obs_stats=self.obs_stats, episodes_out=episodes, **word, **self._env())
+        kw = dict(repetitions=int(repetitions), sigma=0.0, member_offset=0, n_local=1, noiseless=True,
+                  obs_stats=self.obs_stats, episodes_out=episodes, **word, **self._env())
+        if bc_out is not None:
+            self.k.rollout_eval_bc(sol, bc_out=bc_out, **kw)
+        else:
+            self.k.rollout_eval(sol, **kw)
         return episodes.cpu().numpy().astype(np.float64)
 
     def record(self, weights, *, repetitions=None, noiseless=False, state=None, generation=0, member_offset=0,
@@ -251,6 +264,15 @@ class DeviceRollouts(_Episodes):
         return world == 1 or not self.normalize_obs      # sharded, the observation totals travel through NCCL
 
 
+def behaviour(final_obs):
+    """[n, d0] fp32 behaviours from final_obs [n, repetitions, d0] fp32: each member's fp64 sum in episode order over
+    its episodes, divided by the repetitions (des_rollout_eval_bc's contract, on the host)."""
+    s = np.zeros(final_obs.shape[::2], dtype=np.float64)
+    for r in range(final_obs.shape[1]):
+        s += final_obs[:, r].astype(np.float64)
+    return (s / final_obs.shape[1]).astype(np.float32)
+
+
 class HostEpisodes:
     """The bridge between environments stepped on the host and the population's policy on the device: runs the episodes
     of `n` weight rows x `repetitions` in lockstep until every slot is done (Evaluator.eval / single_run,
@@ -278,10 +300,11 @@ class HostEpisodes:
         self.alive_d = torch.empty(B, dtype=torch.uint8, device=self.device)
         self.act_d = torch.empty((B, self.A), dtype=torch.float32, device=self.device)
 
-    def run(self, rows, *, generation, member_offset=0, key_member=None, obs_stats=None, stat_part=None):
+    def run(self, rows, *, generation, member_offset=0, key_member=None, obs_stats=None, stat_part=None, final_obs=None):
         """Returns (returns[n, repetitions] fp64, environment steps taken).  Episode (i, r) resets with the key
         (generation, member_offset + i, r), or (generation, key_member, r) when key_member is given (test episodes,
-        whose action noise then uses member 0 as des_rollout_eval's test episodes do)."""
+        whose action noise then uses member 0 as des_rollout_eval's test episodes do).  final_obs, an fp32 array
+        [n, repetitions, d0], receives the observation returned by the step that ended each episode."""
         n, reps, B = self.n, self.reps, self.n * self.reps
         if B == 0:
             return np.zeros((n, reps)), 0
@@ -311,6 +334,9 @@ class HostEpisodes:
             obs, reward, done = self.env.step(act_h, alive)
             returns[alive] += np.asarray(reward, dtype=np.float64)[alive]      # utils.py:137
             steps += int(alive.sum())
+            if final_obs is not None:
+                ended = alive & np.asarray(done, dtype=bool)
+                final_obs.reshape(B, self.d0)[ended] = np.asarray(obs, dtype=np.float32).reshape(B, self.d0)[ended]
             alive &= ~np.asarray(done, dtype=bool)
             t += 1
         return returns.reshape(n, reps), steps
@@ -351,7 +377,10 @@ class HostRollouts(_Episodes):
             self._bridges[(n, reps)] = ep
         return ep
 
-    def members(self, theta, *, state, generation, offset, n_local, out):
+    def members(self, theta, *, state, generation, offset, n_local, out, bc_out=None):
+        """Fitness of members [offset, offset + n_local) into out; with bc_out [n_local, d0], also their behaviours: each
+        member's observations after its episodes' last steps, averaged over the repetitions (behaviour()).  Mirrored
+        members have them too: their rows are the mirrored perturbations."""
         self.obs_totals.zero_()
         self.last_steps = 0
         if n_local:
@@ -359,7 +388,7 @@ class HostRollouts(_Episodes):
                 self.rows = torch.empty((n_local, theta.numel()), dtype=torch.float32, device=self.device)
             (self.k.nes_perturb_mirrored if self.mirrored else self.k.nes_perturb)(theta, n_local, self.sigma, self.seed, generation,
                                                       member_offset=offset, out=self.rows)
-            self._episodes(self.rows, offset, generation, out)
+            self._episodes(self.rows, offset, generation, out, bc_out)
 
     def solutions(self, solutions, *, offset, generation, out=None):
         n = int(solutions.shape[0])
@@ -370,24 +399,32 @@ class HostRollouts(_Episodes):
             self._episodes(solutions.to(device=self.device, dtype=torch.float32).contiguous(), offset, generation, out)
         return out
 
-    def _episodes(self, rows, offset, generation, out):
+    def _episodes(self, rows, offset, generation, out, bc_out=None):
         n = int(rows.shape[0])
         if self.stat_part is None or self.stat_part.shape[0] != n:
             self.stat_part = torch.zeros((n, 2 * self.d0 + 1), dtype=torch.float64, device=self.device)
         else:
             self.stat_part.zero_()
         part = self.stat_part if self.normalize_obs else None
+        final = None if bc_out is None else np.zeros((n, self.repetitions, self.d0), dtype=np.float32)
         ret, self.last_steps = self._bridge(n, self.repetitions).run(rows, generation=generation, member_offset=offset,
-                                                                     obs_stats=self.obs_stats, stat_part=part)
+                                                                     obs_stats=self.obs_stats, stat_part=part,
+                                                                     final_obs=final)
         out.copy_(torch.from_numpy(ret.mean(axis=1).astype(np.float32)))       # -cost, utils.py:124
         if part is not None:
             self.k.obs_parts_reduce(part, self.d0, out=self.obs_totals)
+        if bc_out is not None:
+            bc_out.copy_(torch.from_numpy(behaviour(final)).reshape(bc_out.shape))
 
-    def test_returns(self, solution, repetitions, generation, state=None):
-        """Episodes keyed (generation, TEST_MEMBER, repetition), which do not feed the statistics; `state` is not read."""
+    def test_returns(self, solution, repetitions, generation, state=None, bc_out=None):
+        """Episodes keyed (generation, TEST_MEMBER, repetition), which do not feed the statistics; `state` is not read.
+        With bc_out [1, d0], also the solution's behaviour from the same episodes."""
         row = solution.reshape(1, -1).to(device=self.device, dtype=torch.float32).contiguous()
+        final = None if bc_out is None else np.zeros((1, int(repetitions), self.d0), dtype=np.float32)
         ret, _ = self._bridge(1, int(repetitions)).run(row, generation=generation, key_member=TEST_MEMBER,
-                                                       obs_stats=self.obs_stats)
+                                                       obs_stats=self.obs_stats, final_obs=final)
+        if bc_out is not None:
+            bc_out.copy_(torch.from_numpy(behaviour(final)).reshape(bc_out.shape))
         return ret[0]
 
     def steps(self, N, group):

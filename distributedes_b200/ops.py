@@ -187,10 +187,11 @@ def rollout_eval_solutions(solutions, *, env=0, hidden, horizon=200, repetitions
 
 
 def _rollout(fn, weights, name, noise, env, hidden, horizon, repetitions, clip, action_noise_std, seed, generation,
-             member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out, record=None):
+             member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out, record=None, bc_out=None):
     """The launch of rollout_eval[_mirrored] (weights = theta[P], noise = (sigma, state, noiseless)) and of
     rollout_eval_solutions (weights = solutions[n_local, P], noise = None); `record` = (mirrored, states_out, obs_out,
-    actions_out, rewards_out) makes it the launch of rollout_record[_solutions]."""
+    actions_out, rewards_out) makes it the launch of rollout_record[_solutions], and `bc_out` [n_local, d0] that of
+    rollout_eval_bc (ops_novelty)."""
     d0, A = _env_dims(env)
     P, mlp = _mlp(d0, int(hidden), A)
     n_local, reps, w, dev = int(n_local), int(repetitions), 2 * d0 + 1, weights.device
@@ -217,6 +218,8 @@ def _rollout(fn, weights, name, noise, env, hidden, horizon, repetitions, clip, 
     else:
         args = head + tail + (int(member_offset), n_local)
     args += traj
+    if bc_out is not None:
+        args += (_ptr(bc_out, 'bc_out', F32, n_local * d0, dev),)
     _launch(fn, weights, name, *args, *_ws(workspace, dev))
     return out
 
@@ -443,3 +446,5 @@ def _cov_apply(fn, Cmat, dC, name, packed, pc, decay, c1, cmu):
 from .ops_record import rollout_record, rollout_record_solutions  # noqa: E402,F401
 # The genetic algorithm's ops (genetic.py): defined in ops_ga on this module's checks.
 from .ops_ga import ga_order, ga_order_workspace, ga_rows, rollout_eval_ga  # noqa: E402,F401
+# Novelty search's ops (novelty.py): defined in ops_novelty on this module's checks.
+from .ops_novelty import novelty, ns_shape, ns_shape_workspace, rollout_eval_bc  # noqa: E402,F401

@@ -257,6 +257,39 @@ DES_API size_t des_ga_order_workspace_bytes(int64_t N);
 DES_API int des_ga_order(int32_t *order_out_dev, const float *fitness_dev, int64_t N, int64_t T, void *workspace_dev,
                          size_t workspace_bytes, void *stream);
 
+/* ---- novelty search: NS-ES, NSR-ES and NSRA-ES (Conti et al. 2018) ------------------------------------------------------
+ *
+ *   Behaviour (BC)  a member's BC is the raw observation (before the normaliser) the environment returns after the last
+ *                   step of each of its episodes, averaged over its `repetitions` episodes: the fp64 sum of the fp32
+ *                   observations in episode order, divided by repetitions, stored as fp32.  d = state_dim.
+ *   Novelty         of a query row q[d] against an archive a[A][d]: for each archive row i, d2_i accumulates
+ *                   fmaf(diff_j, diff_j, d2_i) in j order from +0, with diff_j = q_j - a_ij in fp32.  Rows are ordered by
+ *                   (d2, i), a NaN d2 after every number.  The novelty is the mean, in fp64 in that order, of the fp32
+ *                   __fsqrt_rn(d2) of the first k_eff = min(k, A) rows, stored as fp32 (NaN when one of them is NaN).
+ *   Shaping         shaped = fmaf(w, s_f, fp32(1 - w) * s_n) in fp32, with s_f and s_n the des_centered_rank of the
+ *                   fitness and of the novelty, w the reward weight (w = 0: NS-ES, w = 0.5: NSR-ES) converted to fp32 and
+ *                   1 - w computed in fp64 then converted.  At w = 1 the shaped vector is s_f bit for bit.
+ *
+ * des_rollout_eval_bc  des_rollout_eval (NES members, or noiseless test episodes) that also writes bc_out_dev[n_local][3],
+ *                      each member's BC.  Fitness, episode returns and observation totals are des_rollout_eval's, bit for
+ *                      bit; its checks are des_rollout_eval's, and bc_out_dev may be NULL only when n_local == 0.
+ * des_novelty          novelty_out[n] of queries[n][d] against archive[A][d], both fp32 row-major.  1 <= d <= 32,
+ *                      1 <= k <= 32, 1 <= A < 2^31, 0 <= n < 2^31; n == 0 does nothing.  No workspace.
+ * des_ns_shape         shaped_out[N] from fitness[N] and novelty[N] (N >= 2), 0 <= reward_weight <= 1; shaped_out may not
+ *                      overlap either input.  workspace: des_ns_shape_workspace_bytes(N) bytes, or DES_ERR_WORKSPACE.  The
+ *                      ranks take des_centered_rank's counting path up to N = 2048 and its bucketed path above. */
+DES_API int des_rollout_eval_bc(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                int32_t repetitions, double sigma, double clip, double action_noise_std, uint64_t seed,
+                                uint64_t generation, const des_state *state_dev, int64_t member_offset, int64_t n_local,
+                                int noiseless, float *bc_out_dev, void *workspace_dev, size_t workspace_bytes,
+                                void *stream);
+DES_API int des_novelty(float *novelty_out_dev, const float *queries_dev, int64_t n, const float *archive_dev, int64_t A,
+                        int32_t d, int32_t k, void *stream);
+DES_API size_t des_ns_shape_workspace_bytes(int64_t N);
+DES_API int des_ns_shape(float *shaped_out_dev, const float *fitness_dev, const float *novelty_dev, int64_t N,
+                         double reward_weight, void *workspace_dev, size_t workspace_bytes, void *stream);
+
 /* Chan merge (utils.py:85-96) of a batch given by obs_totals_dev = [sum (d0) | sum of squares (d0) | count] into
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
 DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim, void *stream);
