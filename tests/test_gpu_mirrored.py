@@ -2,7 +2,8 @@
 
 * Tape forward: member 2p is bit-equal to plain member p on every kernel shape (fp32; f16 / f16x3 on 2-CTA clusters,
   single-CTA and multi-pass tapes, with and without the tile workspace); member 2p+1 matches the fp32 forward of the
-  des_nes_perturb_mirrored rows within the per-precision tolerances of test_gpu_ops.py.
+  des_nes_perturb_mirrored rows within the per-precision tolerances of test_gpu_ops.py.  Every action of member 2p+1,
+  on every eval kernel instantiation and against fp64, is checked in tests/test_gpu_forward_error.py.
 * Rows, the pair-form reduction (against an fp64 sum over the device's own normals), closed-loop and host-stepped
   Pendulum and graph capture.  natural_es.train against the reference's verbatim run on explicit +-eps pairs is in
   tests/test_gpu_goldens.py, two GPUs in tests/test_gpu_multi.py."""
