@@ -104,6 +104,11 @@ SIGNATURES = {
     'des_ga_rows_sweep': (C.c_int, [_P, _P, _P, _I64, _I64, _P, _U64, _I64, _I64, _P, _P]),
     'des_ga_order_runs_workspace_bytes': (_SZ, [_I64, _I64]),
     'des_ga_order_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, _SZ, _P]),
+    'des_rollout_eval_bc_sweep': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _P, _U64, _P, _I64, _I64,
+                                            C.c_int, _P, _P, C.c_size_t, _P]),
+    'des_novelty_runs': (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _I64, _I32, _I32, _P]),
+    'des_ns_shape_runs_workspace_bytes': (_SZ, [_I64, _I64]),
+    'des_ns_shape_runs': (C.c_int, [_P, _P, _P, _I64, _I64, _P, _P, _SZ, _P]),
     'des_nes_eval_workspace_bytes': (_SZ, [Dims, C.c_int]),
     'des_nes_eval': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),
     'des_nes_eval_mirrored': (C.c_int, [_P, _P, _P, _P, Dims, _D, _D, _U64, _U64, _P, _I64, _I64, C.c_int, _P, _SZ, _P]),

@@ -23,7 +23,8 @@ namespace des {
 // non-NULL `ga` makes it a genetic-algorithm generation (des_rollout_eval_ga): `weights` is then its parents table.  A
 // non-NULL `ga_sweep` with a table hp_dev makes the sweep one of genetic-algorithm runs (des_rollout_eval_ga_sweep):
 // `weights` is then the buffer of every run's parents table.  A non-NULL `bc` makes it an evaluation that also writes
-// each member's behaviour characterisation (des_rollout_eval_bc).
+// each member's behaviour characterisation (des_rollout_eval_bc), and a non-NULL `bc_sweep` with a table hp_dev a sweep
+// that does (des_rollout_eval_bc_sweep).
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
@@ -32,7 +33,7 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
                           const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st,
                           const GaArgs *ga = nullptr, const GaSweepArgs *ga_sweep = nullptr,
-                          const BcArgs *bc = nullptr) {
+                          const BcArgs *bc = nullptr, const BcSweepArgs *bc_sweep = nullptr) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -51,7 +52,8 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                         (long long)n_local, repetitions, dims.tape_len);
     }
     if (n_local == 0) return DES_OK;
-    DES_REQUIRE(fitness_out_dev && weights_dev && (!bc || bc->bc_out), "%s: NULL pointer", who);
+    DES_REQUIRE(fitness_out_dev && weights_dev && (!bc || bc->bc_out) && (!bc_sweep || bc_sweep->bc_out),
+                "%s: NULL pointer", who);
     RollArgs a;
     a.fitness = fitness_out_dev; a.ep_ret = episode_returns_out_dev;
     a.theta = rows_mode ? nullptr : weights_dev; a.rows = rows_mode ? weights_dev : nullptr;
@@ -113,6 +115,13 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                 g.theta = nullptr;
                 g.parents = weights_dev;
                 const int rc = rollout_ga_sweep_launch(g, H, (unsigned)n_local, smem, st);
+                if (rc != DES_OK || !obs_totals_out_dev) return rc;
+                return obs_parts_reduce_runs(obs_totals_out_dev, a.stat_part, n_local / run_size, run_size, 7, st);
+            }
+            if (bc_sweep) {
+                BcSweepArgs b = *bc_sweep;
+                static_cast<SweepArgs &>(b) = sa;
+                const int rc = rollout_bc_sweep_launch(b, H, (unsigned)n_local, smem, st);
                 if (rc != DES_OK || !obs_totals_out_dev) return rc;
                 return obs_parts_reduce_runs(obs_totals_out_dev, a.stat_part, n_local / run_size, run_size, 7, st);
             }
@@ -285,6 +294,27 @@ extern "C" DES_API int des_rollout_eval_sweep(float *fitness_out_dev, float *epi
                                obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, state_dev, 0,
                                n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size, hp_dev,
                                nullptr, (cudaStream_t)stream);
+}
+
+extern "C" DES_API int des_rollout_eval_bc_sweep(float *fitness_out_dev, float *episode_returns_out_dev,
+                                                 double *obs_totals_out_dev, const float *theta_dev,
+                                                 const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions,
+                                                 double clip, const des_run_hp *hp_dev, uint64_t generation,
+                                                 const des_state *state_dev, int64_t n_runs, int64_t run_size,
+                                                 int noiseless, float *bc_out_dev, void *workspace_dev,
+                                                 size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_bc_sweep";
+    const int rc = des::check_runs(who, n_runs, run_size, 1);
+    if (rc != DES_OK) return rc;
+    DES_REQUIRE(!noiseless || run_size == 1, "%s: test episodes (noiseless) evaluate one theta per run: run_size must be 1 "
+                "(got %lld)", who, (long long)run_size);
+    DES_REQUIRE(n_runs == 0 || hp_dev, "%s: NULL pointer", who);
+    des::BcSweepArgs bc;
+    bc.bc_out = bc_out_dev;
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, theta_dev, false,
+                               obs_stats_dev, env, dims, repetitions, 0.0, clip, 0.0, 0, generation, state_dev, 0,
+                               n_runs * run_size, noiseless, workspace_dev, workspace_bytes, false, run_size, hp_dev,
+                               nullptr, (cudaStream_t)stream, nullptr, nullptr, nullptr, &bc);
 }
 
 extern "C" DES_API int des_rollout_eval_solutions_sweep(float *fitness_out_dev, float *episode_returns_out_dev,

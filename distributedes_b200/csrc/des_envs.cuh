@@ -5,7 +5,8 @@
 // came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
 // (RecordArgs) in a unit of their own for the same reason, des_envs_ga.cu the genetic algorithm's kernels of
 // des_rollout_eval_ga (GaArgs) and des_envs_ga_sweep.cu those of its sweeps, des_rollout_eval_ga_sweep (GaSweepArgs).
-// des_envs_bc.cu instantiates the behaviour-writing kernels of des_rollout_eval_bc (BcArgs) for novelty search.
+// des_envs_bc.cu instantiates the behaviour-writing kernels of des_rollout_eval_bc (BcArgs) for novelty search, and
+// des_envs_bc_sweep.cu those of its sweeps, des_rollout_eval_bc_sweep (BcSweepArgs).
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -81,9 +82,20 @@ struct BcArgs : RollArgs {
     float *bc_out;                     // [n_local][d0]
 };
 
+// The arguments of a sweep evaluation that also writes each member's behaviour (des_rollout_eval_bc_sweep): a sweep
+// (SweepArgs: the run's seed, sigma and action noise from its hp row) whose CTA writes its behaviour as a BcArgs kernel
+// does, at row blockIdx.x of bc_out [n_runs * run_size][d0].
+struct BcSweepArgs : SweepArgs {
+    float *bc_out;                     // [n_runs * run_size][d0]
+};
+
 // The Args whose members are built from a parents table (the genetic algorithm's fill stage).
 template <typename Args>
 constexpr bool kGaFill = std::is_same<Args, GaArgs>::value || std::is_same<Args, GaSweepArgs>::value;
+
+// The Args of a behaviour-writing evaluation (after the step loop).
+template <typename Args>
+constexpr bool kBc = std::is_same<Args, BcArgs>::value || std::is_same<Args, BcSweepArgs>::value;
 
 // The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
 // except in a sweep, where every run is a population of its own.
@@ -146,7 +158,9 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // table and counts.
 // Args = BcArgs (des_rollout_eval_bc, kRows false): RollArgs, and after the last step each episode's publishing lane
 // observes its state once more; lane 0 writes the member's mean of those raw observations.
-template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs, GaSweepArgs or BcArgs
+// Args = BcSweepArgs (des_rollout_eval_bc_sweep, kRows false): a sweep CTA that writes its behaviour as BcArgs does.
+template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs, GaSweepArgs,
+                                              // BcArgs or BcSweepArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
@@ -257,7 +271,6 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     // a recording's row of episode ep at step t, ((member * reps + ep) * horizon + t), and whether this lane writes it;
     // the kernels of the evaluations compile none of it
     auto row_at = [&](int t) { return ((int64_t)blockIdx.x * a.reps + ep) * a.horizon + t; };
-    constexpr bool kBc = std::is_same<Args, BcArgs>::value;    // a behaviour-writing evaluation (after the loop)
     for (int t = 0; t < a.horizon; ++t) {
         {
             float o[3];
@@ -381,7 +394,7 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
         }
         if (lane == 6) a.stat_part[(int64_t)blockIdx.x * 7 + 6] = (double)a.reps * a.horizon;
     }
-    if constexpr (kBc) {
+    if constexpr (kBc<Args>) {
         // the behaviour: the raw observation after the last step, in the reduction area once every read above is done.
         // Observed here, after the step loop, so that the loop is the evaluation's own code and schedule
         float bc[3];
@@ -416,5 +429,8 @@ int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cuda
 int rollout_ga_sweep_launch(const GaSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 // rollout_pendulum_kernel<H / 16, false, BcArgs> over `blocks` CTAs (des_rollout_eval_bc), defined in des_envs_bc.cu
 int rollout_bc_launch(const BcArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, false, BcSweepArgs> over `blocks` CTAs (des_rollout_eval_bc_sweep), defined in
+// des_envs_bc_sweep.cu
+int rollout_bc_sweep_launch(const BcSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

@@ -370,13 +370,17 @@ class _RunsUpdate:
     Adam and the statistics merge.  With a sweep table `hp` each run has its own seed and hyper-parameters (ops_sweep);
     without one the runs share `seed`, `sigma`, `lr` and `wd`."""
 
-    def rank_and_reduce(self):
-        self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
+    def rank_and_reduce(self, shaped=None):
+        """Every run's partial sum of shaped fitness x noise.  `shaped` [R, N], when given, replaces the centered ranks of
+        the fitness (a novelty-search sweep's blend, novelty.py)."""
+        if shaped is None:
+            self.k.centered_rank_runs(self.fitness_all, workspace=self.rank_ws, out=self.shaped)
+            shaped = self.shaped
         if self.hp is not None:
-            self.k.nes_grad_partial_sweep(self.shaped, self.P, self.hp, state=self.state, workspace=self.grad_ws,
+            self.k.nes_grad_partial_sweep(shaped, self.P, self.hp, state=self.state, workspace=self.grad_ws,
                                           out=self.partial)
         else:
-            self.k.nes_grad_partial_runs(self.shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
+            self.k.nes_grad_partial_runs(shaped, self.P, seed=self.seed, state=self.state, workspace=self.grad_ws,
                                          out=self.partial)
         return self.partial
 
@@ -498,17 +502,25 @@ class RolloutRunsEngine(_RunsUpdate):
         env = dict(env=self.env_id, hidden=self.H, horizon=self.horizon, clip=self.clip)
         return env if self.hp is not None else dict(env, action_noise_std=self.action_noise_std, seed=self.seed)
 
-    def _rollout(self, **kw):
-        """rollout_eval_sweep with the table, or rollout_eval_runs with the shared seed and sigma."""
+    def _rollout(self, bc_out=None, **kw):
+        """rollout_eval_sweep with the table, or rollout_eval_runs with the shared seed and sigma; with bc_out,
+        rollout_eval_bc_sweep, which needs the table."""
         if self.hp is not None:
             kw.pop('sigma')
+            if bc_out is not None:
+                return self.k.rollout_eval_bc_sweep(self.theta, self.hp, bc_out=bc_out, **kw, **self._env())
             return self.k.rollout_eval_sweep(self.theta, self.hp, **kw, **self._env())
+        if bc_out is not None:
+            raise ValueError('RolloutRunsEngine: behaviours (bc_out) are written for sweeps only (seeds=); a batch of runs '
+                             'without seeds has none')
         return self.k.rollout_eval_runs(self.theta, **kw, **self._env())
 
-    def evaluate(self):
+    def evaluate(self, bc_out=None):
+        """Every run's fitness [R, N]; bc_out [R, N, d0], when given, also receives the members' behaviours from the same
+        episodes (a sweep only: rollout_eval_bc_sweep; novelty.py)."""
         self._rollout(repetitions=self.repetitions, sigma=self.sigma, state=self.state, run_size=self.N,
                       obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
-                      workspace=self.roll_ws, out=self.fitness_all)
+                      workspace=self.roll_ws, out=self.fitness_all, bc_out=bc_out)
         return self.fitness_all
 
     def _generation_eager(self):
@@ -527,14 +539,15 @@ class RolloutRunsEngine(_RunsUpdate):
             self._generation_eager()
         self.generation_index += 1
 
-    def test_returns(self, repetitions=None):
+    def test_returns(self, repetitions=None, bc_out=None):
         """[R, repetitions] fp64 returns of noiseless test episodes of every run's theta with its own statistics, from
         one launch: run r's are RolloutEngine.test_returns of theta[r] (the same resets and generation word; in a sweep,
-        under run r's seed)."""
+        under run r's seed).  bc_out [R, 1, d0], when given, also receives every run's behaviour from the same episodes
+        (a sweep only)."""
         reps = int(repetitions or self.test_repetitions)
         episodes = torch.empty((self.R, 1, reps), dtype=torch.float32, device=self.device)
         self._rollout(repetitions=reps, sigma=0.0, state=self.state, run_size=1, noiseless=True, obs_stats=self.obs_stats,
-                      out=self.test_fitness, episodes_out=episodes)
+                      out=self.test_fitness, episodes_out=episodes, bc_out=bc_out)
         return episodes.reshape(self.R, reps).cpu().numpy().astype(np.float64)
 
     def record_test_episodes(self, run, repetitions=None):
@@ -634,9 +647,12 @@ class HostEnvSweepEngine(_RunsUpdate):
         self.steps_taken = np.zeros(R, dtype=np.int64)      # per run, the episodes' real lengths (natural_es.py:75)
         self.running = np.ones(R, dtype=bool)
 
-    def evaluate(self):
+    def evaluate(self, bc_out=None):
+        """Every run's fitness [R, N]; bc_out [R, N, d0], when given, also receives the members' behaviours from the same
+        episodes (novelty.py)."""
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
         self.source.members(self.theta, self.hp, generation=self.generation_index, run_size=self.N,
-                            running=self.running, out=self.fitness_all)
+                            running=self.running, out=self.fitness_all, **bc)
         self.steps_taken = self.source.last_steps
         return self.fitness_all
 
@@ -647,9 +663,11 @@ class HostEnvSweepEngine(_RunsUpdate):
         self.apply()
         self.generation_index += 1
 
-    def test_returns(self, repetitions=None):
+    def test_returns(self, repetitions=None, bc_out=None):
         """[R, repetitions] fp64 returns of noiseless test episodes of every running run's theta with its own statistics,
         keyed (generation_index, TEST_MEMBER, repetition): run r's are HostEnvEngine.test_returns of theta[r].  The
-        runs `running` leaves out return zeros."""
+        runs `running` leaves out return zeros.  bc_out [R, 1, d0], when given, also receives every running run's
+        behaviour from the same episodes."""
         reps = int(repetitions or self.test_repetitions)
-        return self.source.test_returns(self.theta, self.hp, reps, self.generation_index, self.running)
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
+        return self.source.test_returns(self.theta, self.hp, reps, self.generation_index, self.running, **bc)

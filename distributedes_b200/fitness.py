@@ -459,10 +459,11 @@ class HostSweepEpisodes:
         self.alive_d = torch.zeros(RB, dtype=torch.uint8, device=self.device)
         self.act_d = torch.zeros((RB, self.A), dtype=torch.float32, device=self.device)
 
-    def run(self, rows, hp, *, generation, running, key_member=None, obs_stats=None, stat_part=None):
+    def run(self, rows, hp, *, generation, running, key_member=None, obs_stats=None, stat_part=None, final_obs=None):
         """Returns (returns[R, n, repetitions] fp64, environment steps[R]); the runs not `running` return zeros.  The
         episodes' keys are HostEpisodes.run's at member_offset 0, the same for every run (each env seeds with its run's
-        seed)."""
+        seed).  final_obs, an fp32 array [R, n, repetitions, d0], receives the observation returned by the step that
+        ended each episode, as HostEpisodes.run's does; the slots of runs not `running` are left as they are."""
         R, n, reps, B, d0 = self.R, self.n, self.reps, self.n * self.reps, self.d0
         members = (np.full(n, int(key_member), dtype=np.int64) if key_member is not None else np.arange(n, dtype=np.int64))
         keys = np.stack([np.full(B, int(generation) & 0xFFFFFFFF, dtype=np.int64), np.repeat(members, reps),
@@ -490,6 +491,9 @@ class HostSweepEpisodes:
                 obs_h[r], reward[r], done[r] = self.envs[r].step(act_h[r], alive[r])
             np.add(returns, reward, out=returns, where=alive)                   # utils.py:137, alive slots only
             steps += alive.sum(axis=1)
+            if final_obs is not None:
+                ended = alive & done
+                final_obs.reshape(R, B, d0)[ended] = obs_h[ended]
             alive &= ~done
             t += 1
         return returns.reshape(R, n, reps), steps
@@ -532,21 +536,22 @@ class HostSweep:
             self._bridges[(n, reps)] = ep
         return ep
 
-    def members(self, theta, hp, *, generation, run_size, running, out):
+    def members(self, theta, hp, *, generation, run_size, running, out, bc_out=None):
         """fitness out[R, N] of every run's members theta_r + sigma_r eps (one des_nes_perturb_sweep), its steps in
-        last_steps and, normalising, its observation totals in obs_totals."""
+        last_steps and, normalising, its observation totals in obs_totals.  With bc_out [R, N, d0], also their behaviours:
+        HostRollouts.members' of every running run (behaviour())."""
         N = int(run_size)
         if self.rows is None:
             self.rows = torch.empty((self.R * N, theta.shape[1]), dtype=torch.float32, device=self.device)
         self.k.nes_perturb_sweep(theta, hp, N, generation, out=self.rows)
-        self._episodes(self.rows, hp, N, generation, running, out)
+        self._episodes(self.rows, hp, N, generation, running, out, bc_out)
 
     def solutions(self, rows, hp, *, generation, running, out):
         """members without the perturbation (CMA-ES): rows [R * N, P] are every run's explicit solutions, run r's N rows
         r*N .. r*N + N - 1 of them, evaluated as HostRollouts.solutions evaluates one run's at offset 0."""
         self._episodes(rows, hp, rows.shape[0] // self.R, generation, running, out)
 
-    def _episodes(self, rows, hp, N, generation, running, out):
+    def _episodes(self, rows, hp, N, generation, running, out, bc_out=None):
         w = 2 * self.d0 + 1
         self.obs_totals.zero_()
         if self.stat_part is None or self.stat_part.shape[0] != self.R * N:
@@ -554,18 +559,31 @@ class HostSweep:
         else:
             self.stat_part.zero_()
         part = self.stat_part if self.normalize_obs else None
+        final = None if bc_out is None else np.zeros((self.R, N, self.repetitions, self.d0), dtype=np.float32)
         ret, self.last_steps = self._bridge(N, self.repetitions).run(rows, hp, generation=generation,
                                                                      running=running, obs_stats=self.obs_stats,
-                                                                     stat_part=part)
+                                                                     stat_part=part, final_obs=final)
         out.copy_(torch.from_numpy(np.stack([ret[r].mean(axis=1).astype(np.float32) for r in range(self.R)])))
         if part is not None:
             self.k.obs_parts_reduce_runs(part, self.d0, N, out=self.obs_totals)
+        if bc_out is not None:
+            self._behaviours(final, bc_out)
 
-    def test_returns(self, theta, hp, repetitions, generation, running):
+    def _behaviours(self, final, bc_out):
+        """bc_out [R, n, d0] from the final observations [R, n, repetitions, d0] (behaviour())."""
+        R, n, reps, d0 = final.shape
+        bc_out.copy_(torch.from_numpy(behaviour(final.reshape(R * n, reps, d0))).reshape(bc_out.shape))
+
+    def test_returns(self, theta, hp, repetitions, generation, running, bc_out=None):
         """[R, repetitions] fp64: every running run's episodes keyed (generation, TEST_MEMBER, repetition) of theta[r]
-        with its statistics, as HostRollouts.test_returns; they do not feed the statistics."""
+        with its statistics, as HostRollouts.test_returns; they do not feed the statistics.  With bc_out [R, 1, d0],
+        also every running run's behaviour from the same episodes."""
+        final = None if bc_out is None else np.zeros((self.R, 1, int(repetitions), self.d0), dtype=np.float32)
         ret, _ = self._bridge(1, int(repetitions)).run(theta, hp, generation=generation, running=running,
-                                                       key_member=TEST_MEMBER, obs_stats=self.obs_stats)
+                                                       key_member=TEST_MEMBER, obs_stats=self.obs_stats,
+                                                       final_obs=final)
+        if bc_out is not None:
+            self._behaviours(final, bc_out)
         return ret[:, 0]
 
 

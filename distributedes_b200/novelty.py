@@ -16,10 +16,17 @@ picks agent m with probability proportional to the novelty of its latest BC (one
 evaluates its population (fitness and BCs from one launch), shapes, steps it, then tests it: that BC joins the archive.
 
 Config attributes, read with defaults: ns_k (10), ns_reward_weight (0.5, or 'adaptive'), ns_agents (1).  Closed-loop and
-host-stepped configs only (a tape has no episodes), plain sampling, one process."""
+host-stepped configs only (a tape has no episodes), plain sampling, one process.
+
+train_sweep(configs) trains R one-agent configs as one batch on one GPU (NoveltySweep): run r is train(configs[r]), bit
+for bit, and each run has its own seed, hyper-parameters, start point, archive and reward weight.  multi_runs is the
+reference's driver of ten runs, sequential or batched."""
 from __future__ import annotations
 
 import copy
+import logging
+import os
+import pickle
 import time
 
 import numpy as np
@@ -74,6 +81,16 @@ def check_config(config):
         raise ValueError('novelty: the behaviour has state_dim = %d entries; des_novelty takes [1, %d]'
                          % (config.state_dim, MAX_D))
     settings(config)
+
+
+def _adapted(w, stall, improved):
+    """NSRA-ES after a generation's test: (w, stall) -> (w, stall)."""
+    if improved:
+        return min(1.0, w + ADAPT_STEP), 0
+    stall += 1
+    if stall >= ADAPT_PATIENCE:
+        return max(0.0, w - ADAPT_STEP), 0
+    return w, stall
 
 
 class NoveltySearch:
@@ -134,14 +151,8 @@ class NoveltySearch:
 
     def adapt(self, improved):
         """NSRA-ES's schedule of w after a generation's test; a fixed weight stays as it is."""
-        if not self.adaptive:
-            return
-        if improved:
-            self.reward_weight, self.stall = min(1.0, self.reward_weight + ADAPT_STEP), 0
-        else:
-            self.stall += 1
-            if self.stall >= ADAPT_PATIENCE:
-                self.reward_weight, self.stall = max(0.0, self.reward_weight - ADAPT_STEP), 0
+        if self.adaptive:
+            self.reward_weight, self.stall = _adapted(self.reward_weight, self.stall, improved)
 
     def select(self):
         """The agent of the next generation, drawn with probability proportional to the novelty of its latest behaviour
@@ -220,3 +231,242 @@ def test(config, solution, stats, ns=None, agent=0):
     """natural_es.test: the mean and std / test_repetitions of noiseless episodes of `solution` (None = the agent's
     current weights) with agent `agent`'s statistics; without `ns`, natural_es.test's host evaluation with `stats`."""
     return natural_es.test(config, solution, stats, engine=None if ns is None else ns.agents[agent])
+
+
+# ---- sweeps: R one-agent novelty searches of different configs trained together on one GPU ------------------------------
+def check_sweep_configs(configs):
+    """Raises ValueError unless train_sweep can train `configs` as one sweep, naming the config and the field: each
+    config passes check_config and has one agent, and the list passes natural_es.check_sweep_configs (all closed-loop or
+    all host-stepped, at most 2048 members each, shared fields equal) with ns_k shared too."""
+    from .natural_es import SWEEP_HOST_SHARED, SWEEP_SHARED, _field, _host_sweep, check_host_sweep_config, check_runs_config
+    if not len(configs):
+        raise ValueError('novelty.train_sweep: no configs')
+    for i, c in enumerate(configs):
+        try:
+            check_config(c)
+        except ValueError as e:
+            raise ValueError('novelty.train_sweep: configs[%d]: %s' % (i, e)) from None
+        M = settings(c)[3]
+        if M != 1:
+            raise ValueError('novelty.train_sweep: configs[%d] has ns_agents = %d; a sweep trains one agent per run (agents '
+                             'step in different generations, so each has its own Adam t, beta^t and generation word, '
+                             'and the runs of a sweep share one des_state)' % (i, M))
+    host = _host_sweep(configs)
+    for i, c in enumerate(configs):
+        try:
+            (check_host_sweep_config if host else check_runs_config)(c)
+        except ValueError as e:
+            raise ValueError('novelty.train_sweep: configs[%d]: %s' % (i, e)) from None
+    shared = (SWEEP_HOST_SHARED if host else SWEEP_SHARED) + ('ns_k',)
+    for i, c in enumerate(configs[1:], 1):
+        for name in shared:
+            a, b = ((settings(x)[0] for x in (configs[0], c)) if name == 'ns_k' else
+                    (_field(configs[0], name), _field(c, name)))
+            if a != b:
+                raise ValueError('novelty.train_sweep: configs differ in %s (%r in configs[0], %r in configs[%d]); the runs '
+                                 'of a novelty sweep may differ only in seed, sigma, learning_rate, weight_decay, '
+                                 'action_noise_std, initial_weight and ns_reward_weight%s'
+                                 % (name, a, b, i, ' (and, host-stepped, their own env_fn and batch_env_fn)' if host else ''))
+
+
+class NoveltySweep:
+    """R one-agent novelty searches trained as one batch (train_sweep): run r is the NoveltySearch of train(configs[r]).
+    `engine` is the sweep engine of natural_es.build_sweep_engine (closed-loop RolloutRunsEngine, host-stepped
+    HostEnvSweepEngine); each run has its own archive [A, d] (archive(r): a view of one [R, capacity, d] buffer whose
+    capacity doubles when full), reward weight (reward_weight[r], stall[r], weights[r]: the w of each generation it
+    shaped with), best test mean best[r] and best_theta[r].  Every live run adds one behaviour per generation, so the live
+    runs' archives have the same number of rows.
+
+    `running` [R] says which runs still train: a host-stepped run stops where its train() would, and its archive, theta,
+    Adam moments and statistics stay as they were then (theta(r), adam_m(r), adam_v(r), obs_stats(r)).  `kernels`
+    (default: distributedes_b200.ops_runs) exists so the host logic can run on CPU with a stand-in."""
+
+    def __init__(self, configs, *, kernels=None, device=None):
+        check_sweep_configs(configs)
+        self.engine = e = natural_es.build_sweep_engine(configs, kernels=kernels, device=device)
+        self.kn, self.device, self.R, self.N, self.d = e.k, e.device, e.R, e.N, e.d0
+        self.host = bool(getattr(configs[0], 'host_env', False))
+        self.k = settings(configs[0])[0]
+        self.adaptive = [settings(c)[2] for c in configs]
+        self.reward_weight = [1.0 if a else settings(c)[1] for a, c in zip(self.adaptive, configs)]
+        self.stall = [0] * self.R
+        self.best, self.best_theta = [-np.inf] * self.R, [None] * self.R
+        self.weights = [[] for _ in range(self.R)]
+        self.running = np.ones(self.R, dtype=bool)
+        R, N, d, dev = self.R, self.N, self.d, self.device
+        self._archive = torch.zeros((R, _INITIAL_CAPACITY, d), dtype=torch.float32, device=dev)
+        self.size = 0                                   # rows of every live run's archive
+        self.sizes = np.zeros(R, dtype=np.int64)        # rows of each run's archive (a stopped run's stays)
+        self.test_bc = torch.zeros((R, 1, d), dtype=torch.float32, device=dev)
+        self.bc = torch.zeros((R, N, d), dtype=torch.float32, device=dev)
+        self.novelty = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.shaped = torch.zeros((R, N), dtype=torch.float32, device=dev)
+        self.shape_ws = self.kn.ns_shape_runs_workspace(R, N, dev)
+        self.weight_table = self.kn.ns_weight_table(self.reward_weight, dev)
+        self._table_weights = list(self.reward_weight)
+        self._frozen = {}                               # r -> theta, Adam moments and statistics of a stopped run
+
+    def archive(self, r):
+        """Run r's archive [A_r, d]: the behaviours of its tests, in order."""
+        return self._archive[r, :int(self.sizes[r])]
+
+    def _state(self, r, name):
+        if r in self._frozen:
+            return self._frozen[r][name]
+        t = getattr(self.engine, name)
+        return None if t is None else t[r]
+
+    def theta(self, r):
+        return self._state(r, 'theta')
+
+    def adam_m(self, r):
+        return self._state(r, 'adam_m')
+
+    def adam_v(self, r):
+        return self._state(r, 'adam_v')
+
+    def obs_stats(self, r):
+        return self._state(r, 'obs_stats')
+
+    def test(self, repetitions):
+        """Every live run's test (mean, std / repetitions, improved), None for a stopped run; the same launch writes
+        each run's behaviour, which joins its archive.  Keeps each run's best test mean and its weights."""
+        e = self.engine
+        returns = e.test_returns(repetitions, bc_out=self.test_bc)
+        if self.size == self._archive.shape[1]:
+            grown = torch.zeros((self.R, 2 * self.size, self.d), dtype=torch.float32, device=self.device)
+            grown[:, :self.size].copy_(self._archive)
+            self._archive = grown
+        self._archive[:, self.size].copy_(self.test_bc[:, 0])
+        self.size += 1
+        self.sizes[self.running] = self.size
+        out, thetas = [None] * self.R, None
+        for r in np.flatnonzero(self.running):
+            mean, ste = np.mean(returns[r]), np.std(returns[r]) / repetitions
+            improved = bool(mean > self.best[r])
+            if improved:
+                thetas = e.theta_numpy() if thetas is None else thetas
+                self.best[r], self.best_theta[r] = mean, thetas[r].copy()
+            out[r] = (mean, ste, improved)
+        return out
+
+    def adapt(self, r, improved):
+        """NSRA-ES's schedule of run r's w after its test; a fixed weight stays as it is."""
+        if self.adaptive[r]:
+            self.reward_weight[r], self.stall[r] = _adapted(self.reward_weight[r], self.stall[r], improved)
+
+    def evaluate(self):
+        """Every run's generation: fitness (engine.fitness_all [R, N]) and the members' behaviours (self.bc) from one
+        launch (host-stepped: one policy launch per step)."""
+        return self.engine.evaluate(bc_out=self.bc)
+
+    def stop(self, r):
+        """Run r trains no more: its theta, Adam moments and statistics are kept as they are now."""
+        e = self.engine
+        self._frozen[r] = {n: None if getattr(e, n) is None else getattr(e, n)[r].clone()
+                           for n in ('theta', 'adam_m', 'adam_v', 'obs_stats')}
+        self.running[r] = False
+        if self.host:
+            e.running[r] = False
+
+    def step(self):
+        """Every run's novelty against its archive, the blend with its weight w_r (the weight table rewritten when a w
+        changed), and the gradient and Adam step of every run."""
+        e = self.engine
+        self.kn.novelty_runs(self.bc, self._archive, self.k, size=self.size, out=self.novelty)
+        if self.reward_weight != self._table_weights:
+            self.weight_table.copy_(self.kn.ns_weight_table(self.reward_weight, self.device))
+            self._table_weights = list(self.reward_weight)
+        self.kn.ns_shape_runs(e.fitness_all, self.novelty, self.weight_table, workspace=self.shape_ws, out=self.shaped)
+        for r in np.flatnonzero(self.running):
+            self.weights[r].append(self.reward_weight[r])
+        e.rank_and_reduce(shaped=self.shaped)
+        e.apply()
+        e.generation_index += 1
+
+
+def build_sweep(configs, *, kernels=None, device=None):
+    """The NoveltySweep of train_sweep(configs)."""
+    return NoveltySweep(configs, kernels=kernels, device=device)
+
+
+def train_sweep(configs, sweep=None):
+    """train(configs[r]) for every r, trained together on one GPU as one sweep: one [training_rewards, training_steps,
+    training_timestamps] triple per config, whose rewards and steps are those of train(configs[r]), bit for bit (and so
+    are run r's final theta, Adam moments, statistics, archive, weights, best and best_theta: NoveltySweep).  The runs
+    share one clock.  The configs may differ in seed, sigma, learning_rate, weight_decay, action_noise_std,
+    initial_weight and ns_reward_weight ('adaptive' included), host-stepped ones also in env_fn and batch_env_fn
+    (check_sweep_configs).  Closed-loop runs take the same steps and stop together; host-stepped runs count their own
+    steps and each stops where its train() would, its environments never reset or stepped again."""
+    check_sweep_configs(configs)
+    ns = sweep if sweep is not None else build_sweep(configs)
+    c, R = configs[0], len(configs)
+    reps = c.test_repetitions
+    out = [[[], [], []] for _ in range(R)]
+    total_steps = np.zeros(R, dtype=np.int64)
+    initial_time = time.time()
+    iteration = 0
+    while True:
+        live = np.flatnonzero(ns.running)
+        tests = ns.test(reps)
+        if iteration > 0:
+            for r in live:
+                ns.adapt(r, tests[r][2])
+        elapsed_time = time.time() - initial_time
+        for r in live:
+            for log, value in zip(out[r], (tests[r][0], int(total_steps[r]), elapsed_time)):
+                log.append(value)
+        logger.info('Test: %d runs running, mean %f, elapsed time %d'
+                    % (len(live), float(np.mean([out[r][0][-1] for r in live])), elapsed_time))
+        fitness = ns.evaluate()
+        total_steps[live] += np.broadcast_to(ns.engine.steps_taken, (R,))[live]
+        logger.info('Train: iteration %d, mean fitness over %d runs %f'
+                    % (iteration, len(live), float(fitness[torch.as_tensor(live)].mean())))
+        iteration += 1
+        for r in live:                                                  # where train(configs[r]) breaks
+            if (c.max_steps and total_steps[r] > c.max_steps) or \
+                    (getattr(c, 'max_generations', 0) and iteration > c.max_generations):
+                ns.stop(r)
+        if not ns.running.any():
+            break
+        ns.step()
+    return out
+
+
+def multi_runs(config, runs=10, log_dir='log', data_dir='data', batched=False, *, kernels=None, device=None):
+    """`runs` train() runs one after the other, run r with seed config.seed + r, with the log file and the pickle of
+    [[rewards, steps, timestamps], ...] of natural_es.multi_runs (data/<tag>-stats-<task>.bin, rewritten after every
+    run).  batched=True trains them together through train_sweep and writes the same files once: the rewards and steps
+    are those of batched=False, bit for bit; the timestamps come from the sweep's one clock.  `kernels` is a stand-in for
+    the device ops (ops, or ops_runs when batched)."""
+    check_config(config)
+    configs = []
+    for run in range(runs):
+        c = copy.copy(config)
+        c.seed = config.seed + run
+        configs.append(c)
+    if batched:
+        check_sweep_configs(configs)
+    os.makedirs(log_dir, exist_ok=True)
+    os.makedirs(data_dir, exist_ok=True)
+    fh = logging.FileHandler(os.path.join(log_dir, '%s-%s.txt' % (config.tag, config.task)))
+    fh.setLevel(logging.DEBUG)
+    logger.addHandler(fh)
+    stats = []
+    path = os.path.join(data_dir, '%s-stats-%s.bin' % (config.tag, config.task))
+    try:
+        if batched:
+            logger.info('Runs 0-%d, batched' % (runs - 1))
+            stats = train_sweep(configs, build_sweep(configs, kernels=kernels, device=device))
+            with open(path, 'wb') as f:
+                pickle.dump(stats, f)
+        for run in range(0 if batched else runs):
+            c = configs[run]
+            logger.info('Run %d' % run)
+            stats.append(train(c, build(c, kernels=kernels, device=device)))
+            with open(path, 'wb') as f:
+                pickle.dump(stats, f)
+    finally:
+        logger.removeHandler(fh)
+        fh.close()
+    return stats

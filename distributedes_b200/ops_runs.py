@@ -113,3 +113,7 @@ from .ops_cma_sweep import (cma_cov_apply_runs, cma_rank_mu_runs, noise_fill_swe
 # table and a count table of their own.
 from .ops_ga_sweep import (ga_order_runs, ga_order_runs_workspace, ga_rows_sweep, ga_table,  # noqa: E402,F401
                            rollout_eval_ga_sweep)
+# The novelty-search sweep ops (novelty.NoveltySweep): defined in ops_novelty_sweep, on the same table and a table of
+# reward weights of their own.
+from .ops_novelty_sweep import (novelty_runs, ns_shape_runs, ns_shape_runs_workspace,  # noqa: E402,F401
+                                ns_weight_table, rollout_eval_bc_sweep)

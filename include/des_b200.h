@@ -530,6 +530,41 @@ DES_API int des_ga_order_runs(int32_t *order_out_dev, const float *fitness_dev, 
                               int64_t table_rows, int64_t n_runs, int64_t run_size, void *workspace_dev,
                               size_t workspace_bytes, void *stream);
 
+/* ---- novelty-search sweeps: R runs of N members, each with its own archive and reward weight -------------------------
+ *
+ * A sweep (above: the des_run_hp table, the per-run rows, 1 <= run_size <= 2048 (2 for the ranks; above 2048
+ * DES_ERR_UNSUPPORTED), n_runs * run_size <= 2^28, and n_runs == 0 does nothing and accepts NULL pointers) of novelty
+ * searches (NS-ES, NSR-ES, NSRA-ES: "novelty search" above).  Each entry point equals, for every run r, the single-run
+ * call named beside it, bit for bit.
+ *
+ * des_rollout_eval_bc_sweep   des_rollout_eval_bc(theta_r, obs_stats_r, seed = s_r, sigma = sigma_r, action_noise_std =
+ *                             a_r, member_offset = 0, n_local = run_size) with the outputs of des_rollout_eval_sweep and
+ *                             bc_out_dev [n_runs][run_size][3]; noiseless != 0 needs run_size == 1 (run r's test
+ *                             episodes under s_r).  Fitness, episode returns and observation totals are
+ *                             des_rollout_eval_sweep's, bit for bit.
+ * des_novelty_runs            novelty_out [n_runs][n] of queries [n_runs][n][d] against archive [n_runs][capacity][d]:
+ *                             run r's row is des_novelty(queries_r, n, archive_r, A, d, k).  1 <= n <= 2048 (above:
+ *                             DES_ERR_UNSUPPORTED), n_runs * n <= 2^28, 1 <= A <= capacity < 2^31; every run's archive
+ *                             has A rows, and rows at index A or above are never read.  No workspace.
+ * des_ns_shape_runs           shaped_out [n_runs][run_size] of fitness and novelty [n_runs][run_size]: run r's row is
+ *                             des_ns_shape(fitness_r, novelty_r, run_size, w_r), the ranks des_centered_rank_runs'.
+ *                             weights_dev is a table in DEVICE memory, fp32 [n_runs][2], 8-byte aligned: row r is
+ *                             (fp32(w_r), fp32(1 - w_r)) with 1 - w_r computed in fp64, as des_ns_shape converts its
+ *                             weight.  The library cannot read it: a weight outside [0, 1] is the caller's to refuse.
+ *                             shaped_out may not overlap either input.  workspace: des_ns_shape_runs_workspace_bytes(
+ *                             n_runs, run_size) bytes, or DES_ERR_WORKSPACE. */
+DES_API int des_rollout_eval_bc_sweep(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                      const float *theta_dev, const float *obs_stats_dev, int env, des_dims dims,
+                                      int32_t repetitions, double clip, const des_run_hp *hp_dev, uint64_t generation,
+                                      const des_state *state_dev, int64_t n_runs, int64_t run_size, int noiseless,
+                                      float *bc_out_dev, void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API int des_novelty_runs(float *novelty_out_dev, const float *queries_dev, int64_t n_runs, int64_t n,
+                             const float *archive_dev, int64_t capacity, int64_t A, int32_t d, int32_t k, void *stream);
+DES_API size_t des_ns_shape_runs_workspace_bytes(int64_t n_runs, int64_t run_size);
+DES_API int des_ns_shape_runs(float *shaped_out_dev, const float *fitness_dev, const float *novelty_dev, int64_t n_runs,
+                              int64_t run_size, const float *weights_dev, void *workspace_dev, size_t workspace_bytes,
+                              void *stream);
+
 /* ---- fused sample + forward + fitness ------------------------------------------------------ */
 
 /* fitness_out_dev[i] (i < n_local) = sum_t -|| clip(pi_{theta+sigma*eps_m}(obs_t), -clip, clip) - target_t ||^2
