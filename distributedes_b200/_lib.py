@@ -75,6 +75,10 @@ SIGNATURES = {
     'des_novelty': (C.c_int, [_P, _P, _I64, _P, _I64, _I32, _I32, _P]),
     'des_ns_shape_workspace_bytes': (_SZ, [_I64]),
     'des_ns_shape': (C.c_int, [_P, _P, _P, _I64, _D, _P, _SZ, _P]),
+    'des_rollout_eval_ga_bc': (C.c_int, [_P, _P, _P, _P, _I64, _I64, _P, C.c_int, Dims, _I32, _D, _D, _D, _U64, _U64, _P,
+                                         _I64, _I64, C.c_int, _P, _P, C.c_size_t, _P]),
+    'des_ns_ga_order_workspace_bytes': (_SZ, [_I64]),
+    'des_ns_ga_order': (C.c_int, [_P, _P, _P, _I64, _I64, _D, _P, _SZ, _P]),
     'des_obs_stats_merge_totals': (C.c_int, [_P, _P, _I32, _P]),
     'des_rollout_eval_runs': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, Dims, _I32, _D, _D, _D, _U64, _U64, _P, _I64, _I64,
                                         C.c_int, _P, C.c_size_t, _P]),

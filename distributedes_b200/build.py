@@ -16,7 +16,7 @@ CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'build')
 LIB = os.path.join(PKG, 'libdes_b200.so')
 SOURCES = ['des_capi.cu', 'des_noise.cu', 'des_eval_ffma.cu', 'des_eval_tc.cu', 'des_rank.cu', 'des_update.cu',
-           'des_cma.cu', 'des_cma_tc.cu', 'des_envs.cu', 'des_envs_sweep.cu', 'des_envs_record.cu', 'des_envs_ga.cu', 'des_ga.cu', 'des_envs_ga_sweep.cu', 'des_ga_sweep.cu', 'des_envs_bc.cu', 'des_envs_bc_sweep.cu', 'des_novelty.cu', 'des_act.cu', 'des_act_sweep.cu', 'des_obs.cu', 'des_comm.cu']
+           'des_cma.cu', 'des_cma_tc.cu', 'des_envs.cu', 'des_envs_sweep.cu', 'des_envs_record.cu', 'des_envs_ga.cu', 'des_ga.cu', 'des_envs_ga_sweep.cu', 'des_ga_sweep.cu', 'des_envs_bc.cu', 'des_envs_bc_sweep.cu', 'des_envs_ga_bc.cu', 'des_novelty.cu', 'des_act.cu', 'des_act_sweep.cu', 'des_obs.cu', 'des_comm.cu']
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden']

@@ -24,7 +24,8 @@ namespace des {
 // non-NULL `ga_sweep` with a table hp_dev makes the sweep one of genetic-algorithm runs (des_rollout_eval_ga_sweep):
 // `weights` is then the buffer of every run's parents table.  A non-NULL `bc` makes it an evaluation that also writes
 // each member's behaviour characterisation (des_rollout_eval_bc), and a non-NULL `bc_sweep` with a table hp_dev a sweep
-// that does (des_rollout_eval_bc_sweep).
+// that does (des_rollout_eval_bc_sweep).  A non-NULL `ga_bc` makes it a genetic-algorithm generation that also writes each
+// member's behaviour (des_rollout_eval_ga_bc): `weights` is then its parents table.
 static int rollout_launch(const char *who, float *fitness_out_dev, float *episode_returns_out_dev,
                           double *obs_totals_out_dev, const float *weights_dev, bool rows_mode,
                           const float *obs_stats_dev, int env, des_dims dims, int32_t repetitions, double sigma,
@@ -33,7 +34,8 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                           void *workspace_dev, size_t workspace_bytes, bool mirrored, int64_t run_size,
                           const des_run_hp *hp_dev, const RecordArgs *record, cudaStream_t st,
                           const GaArgs *ga = nullptr, const GaSweepArgs *ga_sweep = nullptr,
-                          const BcArgs *bc = nullptr, const BcSweepArgs *bc_sweep = nullptr) {
+                          const BcArgs *bc = nullptr, const BcSweepArgs *bc_sweep = nullptr,
+                          const GaBcArgs *ga_bc = nullptr) {
     DES_REQUIRE(env == kEnvPendulum, "%s: unknown environment %d (0 = Pendulum-v0)", who, env);
     if (mirrored && !(member_offset >= 0 && n_local >= 0 && whole_pairs(member_offset, n_local)))
         return not_whole_pairs(who, "n_local", member_offset, n_local);
@@ -52,8 +54,8 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
                         (long long)n_local, repetitions, dims.tape_len);
     }
     if (n_local == 0) return DES_OK;
-    DES_REQUIRE(fitness_out_dev && weights_dev && (!bc || bc->bc_out) && (!bc_sweep || bc_sweep->bc_out),
-                "%s: NULL pointer", who);
+    DES_REQUIRE(fitness_out_dev && weights_dev && (!bc || bc->bc_out) && (!bc_sweep || bc_sweep->bc_out) &&
+                (!ga_bc || ga_bc->bc_out), "%s: NULL pointer", who);
     RollArgs a;
     a.fitness = fitness_out_dev; a.ep_ret = episode_returns_out_dev;
     a.theta = rows_mode ? nullptr : weights_dev; a.rows = rows_mode ? weights_dev : nullptr;
@@ -89,6 +91,15 @@ static int rollout_launch(const char *who, float *fitness_out_dev, float *episod
         BcArgs b = *bc;
         static_cast<RollArgs &>(b) = a;
         const int rc = rollout_bc_launch(b, H, (unsigned)n_local, smem, st);
+        if (rc != DES_OK || !obs_totals_out_dev) return rc;
+        return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
+    }
+    if (ga_bc) {
+        GaBcArgs g = *ga_bc;
+        static_cast<RollArgs &>(g) = a;
+        g.theta = nullptr;
+        g.parents = weights_dev;
+        const int rc = rollout_ga_bc_launch(g, H, (unsigned)n_local, smem, st);
         if (rc != DES_OK || !obs_totals_out_dev) return rc;
         return obs_parts_reduce(obs_totals_out_dev, a.stat_part, n_local, 7, st);
     }
@@ -212,6 +223,28 @@ extern "C" DES_API int des_rollout_eval_ga(float *fitness_out_dev, float *episod
                                obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
                                state_dev, member_offset, n_local, 0, workspace_dev, workspace_bytes, false, 0, nullptr,
                                nullptr, (cudaStream_t)stream, &ga);
+}
+
+extern "C" DES_API int des_rollout_eval_ga_bc(float *fitness_out_dev, float *episode_returns_out_dev,
+                                              double *obs_totals_out_dev, const float *parents_dev, int64_t n_parents,
+                                              int64_t n_elites, const float *obs_stats_dev, int env, des_dims dims,
+                                              int32_t repetitions, double sigma, double clip, double action_noise_std,
+                                              uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                              int64_t member_offset, int64_t n_local, int noiseless, float *bc_out_dev,
+                                              void *workspace_dev, size_t workspace_bytes, void *stream) {
+    const char *who = "des_rollout_eval_ga_bc";
+    DES_REQUIRE(!noiseless, "%s: test episodes (noiseless) evaluate one row; use des_rollout_eval_bc on it", who);
+    DES_REQUIRE(n_parents >= 1 && n_parents <= INT32_MAX, "%s: n_parents must be in [1, 2^31) (got %lld)", who,
+                (long long)n_parents);
+    DES_REQUIRE(n_elites >= 0 && n_elites <= n_parents, "%s: n_elites must be in [0, n_parents = %lld] (got %lld)", who,
+                (long long)n_parents, (long long)n_elites);
+    des::GaBcArgs ga;
+    ga.n_parents = (int)n_parents; ga.n_elites = (int)n_elites;
+    ga.bc_out = bc_out_dev;
+    return des::rollout_launch(who, fitness_out_dev, episode_returns_out_dev, obs_totals_out_dev, parents_dev, false,
+                               obs_stats_dev, env, dims, repetitions, sigma, clip, action_noise_std, seed, generation,
+                               state_dev, member_offset, n_local, 0, workspace_dev, workspace_bytes, false, 0, nullptr,
+                               nullptr, (cudaStream_t)stream, nullptr, nullptr, nullptr, nullptr, &ga);
 }
 
 extern "C" DES_API int des_rollout_eval_ga_sweep(float *fitness_out_dev, float *episode_returns_out_dev,

@@ -6,7 +6,8 @@
 // (RecordArgs) in a unit of their own for the same reason, des_envs_ga.cu the genetic algorithm's kernels of
 // des_rollout_eval_ga (GaArgs) and des_envs_ga_sweep.cu those of its sweeps, des_rollout_eval_ga_sweep (GaSweepArgs).
 // des_envs_bc.cu instantiates the behaviour-writing kernels of des_rollout_eval_bc (BcArgs) for novelty search, and
-// des_envs_bc_sweep.cu those of its sweeps, des_rollout_eval_bc_sweep (BcSweepArgs).
+// des_envs_bc_sweep.cu those of its sweeps, des_rollout_eval_bc_sweep (BcSweepArgs).  des_envs_ga_bc.cu instantiates the
+// genetic algorithm's behaviour-writing kernels of des_rollout_eval_ga_bc (GaBcArgs) for its novelty search.
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -89,13 +90,23 @@ struct BcSweepArgs : SweepArgs {
     float *bc_out;                     // [n_runs * run_size][d0]
 };
 
-// The Args whose members are built from a parents table (the genetic algorithm's fill stage).
+// The arguments of a genetic-algorithm generation that also writes each member's behaviour (des_rollout_eval_ga_bc): a
+// GaArgs generation whose CTA writes its behaviour as a BcArgs kernel does, at row blockIdx.x of bc_out.  It derives from
+// neither RunArgs nor SweepArgs, so the member is blockIdx.x and no run block applies.
+struct GaBcArgs : GaArgs {
+    float *bc_out;                     // [n_local][d0]
+};
+
+// The Args whose members are built from a parents table (the genetic algorithm's fill stage).  Named one by one, not by
+// base class, so that a new Args joins no other Args' code paths.
 template <typename Args>
-constexpr bool kGaFill = std::is_same<Args, GaArgs>::value || std::is_same<Args, GaSweepArgs>::value;
+constexpr bool kGaFill = std::is_same<Args, GaArgs>::value || std::is_same<Args, GaSweepArgs>::value ||
+                         std::is_same<Args, GaBcArgs>::value;
 
 // The Args of a behaviour-writing evaluation (after the step loop).
 template <typename Args>
-constexpr bool kBc = std::is_same<Args, BcArgs>::value || std::is_same<Args, BcSweepArgs>::value;
+constexpr bool kBc = std::is_same<Args, BcArgs>::value || std::is_same<Args, BcSweepArgs>::value ||
+                     std::is_same<Args, GaBcArgs>::value;
 
 // The CTA's member within its population: member_offset + member_slot(a) is the member in the counters.  blockIdx.x,
 // except in a sweep, where every run is a population of its own.
@@ -159,8 +170,9 @@ constexpr int kHS = 8;                 // row stride of an h1 panel (one panel p
 // Args = BcArgs (des_rollout_eval_bc, kRows false): RollArgs, and after the last step each episode's publishing lane
 // observes its state once more; lane 0 writes the member's mean of those raw observations.
 // Args = BcSweepArgs (des_rollout_eval_bc_sweep, kRows false): a sweep CTA that writes its behaviour as BcArgs does.
+// Args = GaBcArgs (des_rollout_eval_ga_bc, kRows false): fills as GaArgs does and writes its behaviour as BcArgs does.
 template <int R, bool kRows, typename Args>   // H = 16*R; Args: RollArgs, RunArgs, SweepArgs, RecordArgs, GaArgs, GaSweepArgs,
-                                              // BcArgs or BcSweepArgs
+                                              // BcArgs, BcSweepArgs or GaBcArgs
 __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     constexpr int H = 16 * R, C = kEpPerLane;
     if constexpr (std::is_base_of<RunArgs, Args>::value) {
@@ -432,5 +444,7 @@ int rollout_bc_launch(const BcArgs &a, int H, unsigned blocks, size_t smem, cuda
 // rollout_pendulum_kernel<H / 16, false, BcSweepArgs> over `blocks` CTAs (des_rollout_eval_bc_sweep), defined in
 // des_envs_bc_sweep.cu
 int rollout_bc_sweep_launch(const BcSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// rollout_pendulum_kernel<H / 16, false, GaBcArgs> over `blocks` CTAs (des_rollout_eval_ga_bc), defined in des_envs_ga_bc.cu
+int rollout_ga_bc_launch(const GaBcArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
 
 }  // namespace des

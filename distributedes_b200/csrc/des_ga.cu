@@ -3,6 +3,8 @@
 //                 plus sigma*eps of the member: a generation's rows (host-stepped and tape sources), or, with a members
 //                 list, the next parents table gathered from the selected members
 //   des_ga_order  order_out[T]: the members of the T best fitnesses, best first (truncation selection)
+//   des_ns_ga_order  order_out[T]: the members of the T smallest keys of the blend of the fitness and novelty ranks
+//                    (the genetic algorithm's novelty search), from des_ns_shape, the rank and des_ga_order's kernels
 #include "des_ga.cuh"
 
 namespace des {
@@ -110,6 +112,52 @@ extern "C" DES_API int des_ga_order(int32_t *order_out_dev, const float *fitness
                                      stream);
     if (rc != DES_OK) return rc;
     ga_scatter_kernel<<<blocks, 256, 0, st>>>(order_out_dev, w.rank, N, T);
+    DES_LAUNCH_CHECK("ga_scatter_kernel");
+    return DES_OK;
+}
+
+extern "C" DES_API size_t des_ns_ga_order_workspace_bytes(int64_t N) {
+    if (N < 2) return 0;
+    return 256 + 5 * des::al256((size_t)N * 4) + des_ns_shape_workspace_bytes(N);
+}
+
+// The negated fitness and novelty, their blend (des_ns_shape: both ranks, then fmaf(w, c_f, fp32(1 - w) * c_n)), the
+// ascending rank of that key (ties to the lower index) and des_ga_order's scatter.  The rank of the key and des_ns_shape
+// run one after the other on the stream, so they share the tail of the workspace.
+extern "C" DES_API int des_ns_ga_order(int32_t *order_out_dev, const float *fitness_dev, const float *novelty_dev,
+                                       int64_t N, int64_t T, double reward_weight, void *workspace_dev,
+                                       size_t workspace_bytes, void *stream) {
+    using namespace des;
+    const char *who = "des_ns_ga_order";
+    DES_REQUIRE(N >= 2 && N <= ((int64_t)1 << 24), "%s: N=%lld, need 2 <= N <= 2^24 (above, two centered ranks can round "
+                "to one fp32 key)", who, (long long)N);
+    DES_REQUIRE(T >= 1 && T <= N, "%s: T must be in [1, N = %lld] (got %lld)", who, (long long)N, (long long)T);
+    DES_REQUIRE(reward_weight >= 0.0 && reward_weight <= 1.0, "%s: reward_weight must be in [0, 1] (got %g)", who,
+                reward_weight);
+    DES_REQUIRE(order_out_dev && fitness_dev && novelty_dev, "%s: NULL pointer", who);
+    const size_t need = des_ns_ga_order_workspace_bytes(N);
+    if (!workspace_dev || workspace_bytes < need) {
+        set_error("%s: workspace %zu B < required %zu B", who, workspace_bytes, need);
+        return DES_ERR_WORKSPACE;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    uint8_t *p = (uint8_t *)(((uintptr_t)workspace_dev + 255) & ~(uintptr_t)255);
+    float *neg_f = (float *)p; p += al256((size_t)N * 4);
+    float *neg_n = (float *)p; p += al256((size_t)N * 4);
+    float *key = (float *)p; p += al256((size_t)N * 4);
+    float *shaped = (float *)p; p += al256((size_t)N * 4);
+    int32_t *rank = (int32_t *)p; p += al256((size_t)N * 4);
+    const size_t tail = (size_t)((const uint8_t *)workspace_dev + workspace_bytes - p);
+    const unsigned blocks = (unsigned)((N + 255) / 256);
+    ga_negate_kernel<<<blocks, 256, 0, st>>>(neg_f, fitness_dev, N);
+    DES_LAUNCH_CHECK("ga_negate_kernel");
+    ga_negate_kernel<<<blocks, 256, 0, st>>>(neg_n, novelty_dev, N);
+    DES_LAUNCH_CHECK("ga_negate_kernel");
+    int rc = des_ns_shape(key, neg_f, neg_n, N, reward_weight, p, tail, stream);
+    if (rc != DES_OK) return rc;
+    rc = des_centered_rank(shaped, rank, key, N, 0, N, p, tail, stream);
+    if (rc != DES_OK) return rc;
+    ga_scatter_kernel<<<blocks, 256, 0, st>>>(order_out_dev, rank, N, T);
     DES_LAUNCH_CHECK("ga_scatter_kernel");
     return DES_OK;
 }

@@ -202,16 +202,21 @@ class DeviceRollouts(_Episodes):
                                           workspace=self._workspace(n), out=out, **self._env())
         return out
 
-    def ga_members(self, parents, n_elites, generation, offset, n_local, out):
+    def ga_members(self, parents, n_elites, generation, offset, n_local, out, bc_out=None):
         """The genetic algorithm's members [offset, offset + n_local) of `generation`, whose table is parents[T_g, P]
         with n_elites elites, evaluated by des_rollout_eval_ga: solutions() of genetic.GeneticAlgorithm.ask()'s rows, bit
-        for bit, with each member's weights built on the device.  The sigma is this source's."""
+        for bit, with each member's weights built on the device.  The sigma is this source's.  With bc_out [n_local, d0],
+        also their behaviours (des_rollout_eval_ga_bc: the same fitness, bit for bit)."""
         self.obs_totals.zero_()
         if n_local:
-            self.k.rollout_eval_ga(parents, n_elites, repetitions=self.repetitions, sigma=self.sigma,
-                                   generation=generation, member_offset=offset, n_local=n_local,
-                                   obs_stats=self.obs_stats, totals_out=self.obs_totals if self.normalize_obs else None,
-                                   workspace=self._workspace(n_local), out=out, **self._env())
+            kw = dict(repetitions=self.repetitions, sigma=self.sigma, generation=generation, member_offset=offset,
+                      n_local=n_local, obs_stats=self.obs_stats,
+                      totals_out=self.obs_totals if self.normalize_obs else None, workspace=self._workspace(n_local),
+                      out=out, **self._env())
+            if bc_out is not None:
+                self.k.rollout_eval_ga_bc(parents, n_elites, bc_out=bc_out, **kw)
+            else:
+                self.k.rollout_eval_ga(parents, n_elites, **kw)
         return out
 
     def test_returns(self, solution, repetitions, generation, state=None, bc_out=None):
@@ -390,13 +395,16 @@ class HostRollouts(_Episodes):
                                                       member_offset=offset, out=self.rows)
             self._episodes(self.rows, offset, generation, out, bc_out)
 
-    def solutions(self, solutions, *, offset, generation, out=None):
+    def solutions(self, solutions, *, offset, generation, out=None, bc_out=None):
+        """Fitness of explicit rows solutions[n, P] as members offset.. into out; with bc_out [n, d0], also their
+        behaviours from the same episodes (behaviour())."""
         n = int(solutions.shape[0])
         self.obs_totals.zero_()
         self.last_steps = 0
         out = out if out is not None else torch.zeros(n, dtype=torch.float32, device=self.device)
         if n:
-            self._episodes(solutions.to(device=self.device, dtype=torch.float32).contiguous(), offset, generation, out)
+            self._episodes(solutions.to(device=self.device, dtype=torch.float32).contiguous(), offset, generation, out,
+                           bc_out)
         return out
 
     def _episodes(self, rows, offset, generation, out, bc_out=None):

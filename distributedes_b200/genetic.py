@@ -108,13 +108,21 @@ class GeneticAlgorithm:
         return self.kn.ga_rows(self.parents, self.n_elites, sigma=self.sigma, seed=self.seed, generation=self.gen,
                                member_offset=0, n_local=self.N, out=out)
 
-    def tell(self, fitness):
+    def tell(self, fitness, novelty=None, reward_weight=1.0):
         """Selects the T best of fitness [N] (higher is better; ties to the lower index, NaN last) and makes their
-        weights, regenerated, the next table.  Returns the order [T] (int32, best first)."""
+        weights, regenerated, the next table.  Returns the order [T] (int32, best first).  With novelty [N] the T first
+        are those of the smallest keys fmaf(w, rank(-fitness), (1 - w) * rank(-novelty)) instead (des_ns_ga_order, w =
+        reward_weight; at w = 1 the order is the fitness's, bit for bit), and the elites are the first E of them."""
         f = torch.as_tensor(fitness).to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
         if f.numel() != self.N:
             raise ValueError('tell() needs the fitness of all %d members (got %d)' % (self.N, f.numel()))
-        self.order = self.kn.ga_order(f, self.T)
+        if novelty is None:
+            self.order = self.kn.ga_order(f, self.T)
+        else:
+            nov = torch.as_tensor(novelty).to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
+            if nov.numel() != self.N:
+                raise ValueError('tell() needs the novelty of all %d members (got %d)' % (self.N, nov.numel()))
+            self.order = self.kn.ns_ga_order(f, nov, float(reward_weight), self.T)
         nxt = self.kn.ga_rows(self.parents, self.n_elites, sigma=self.sigma, seed=self.seed, generation=self.gen,
                               members=self.order, out=self._spare)
         self._spare = self.parents if self.parents.shape[0] == self.T else torch.empty_like(nxt)
@@ -141,25 +149,29 @@ class Worker:
         self.tests_run = 0
         self.fitness = self.rows = None
 
-    def run(self, ga):
-        """fitness [N] fp32 (mean return, higher is better) of generation ga.gen's members."""
+    def run(self, ga, bc_out=None):
+        """fitness [N] fp32 (mean return, higher is better) of generation ga.gen's members; with bc_out [N, d0], the same
+        evaluation also writes their behaviours (the fused closed-loop kernel, or a host-stepped source's episodes)."""
         if self.fitness is None or self.fitness.numel() != ga.N:
             self.fitness = torch.zeros(ga.N, dtype=torch.float32, device=self.device)
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
         if self.fused:
-            self.source.ga_members(ga.parents, ga.n_elites, ga.gen, 0, ga.N, self.fitness)
+            self.source.ga_members(ga.parents, ga.n_elites, ga.gen, 0, ga.N, self.fitness, **bc)
         else:
             self.rows = ga.ask(out=self.rows)
-            self.source.solutions(self.rows, offset=0, generation=ga.gen, out=self.fitness)
+            self.source.solutions(self.rows, offset=0, generation=ga.gen, out=self.fitness, **bc)
         return self.fitness
 
     def steps(self, N):
         """Environment steps of the last run()."""
         return self.source.steps(N, self.group)
 
-    def test_returns(self, solution, repetitions):
+    def test_returns(self, solution, repetitions, bc_out=None):
         """Returns of `repetitions` noiseless episodes of one solution with the current statistics; the k-th call
-        (k = 0 first) resets its episodes from the test stream with generation word k."""
-        ret = self.source.test_returns(solution, int(repetitions), self.tests_run)
+        (k = 0 first) resets its episodes from the test stream with generation word k.  With bc_out [1, d0], the same
+        episodes also write the solution's behaviour."""
+        bc = {} if bc_out is None else dict(bc_out=bc_out)
+        ret = self.source.test_returns(solution, int(repetitions), self.tests_run, **bc)
         self.tests_run += 1
         return ret
 

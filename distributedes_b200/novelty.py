@@ -20,7 +20,14 @@ host-stepped configs only (a tape has no episodes), plain sampling, one process.
 
 train_sweep(configs) trains R one-agent configs as one batch on one GPU (NoveltySweep): run r is train(configs[r]), bit
 for bit, and each run has its own seed, hyper-parameters, start point, archive and reward weight.  multi_runs is the
-reference's driver of ten runs, sequential or batched."""
+reference's driver of ten runs, sequential or batched.
+
+train_ga(config) is novelty search for the genetic algorithm (Such et al. 2017: GA-NS, and GA-NSR / GA-NSRA with the
+reward weights above), with genetic.train's loop (NoveltyGA).  The members' behaviours come from the generation's own
+evaluation, and truncation selection orders fmaf(w, rank(-fitness), (1 - w) * rank(-novelty)) ascending
+(des_ns_ga_order): w = 1 is genetic.train, bit for bit.  The archive takes one behaviour per generation, that of the
+tested best row, and novelty is measured against the archive alone; this is this project's rule, the one train() uses,
+not necessarily the paper's."""
 from __future__ import annotations
 
 import copy
@@ -33,7 +40,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import natural_es
+from . import genetic, natural_es
 from .engine import kernels_and_device
 from .model import StandardFCNet
 from .utils import logger
@@ -93,6 +100,27 @@ def _adapted(w, stall, improved):
     return w, stall
 
 
+class Archive:
+    """Behaviours in the order they were added: `rows` [A, d] is a view of the device buffer, whose capacity doubles
+    when full."""
+
+    def __init__(self, d, device):
+        self.buffer = torch.zeros((_INITIAL_CAPACITY, int(d)), dtype=torch.float32, device=device)
+        self.size = 0
+
+    @property
+    def rows(self):
+        return self.buffer[:self.size]
+
+    def add(self, row):
+        if self.size == self.buffer.shape[0]:
+            grown = torch.zeros((2 * self.size, self.buffer.shape[1]), dtype=torch.float32, device=self.buffer.device)
+            grown[:self.size].copy_(self.buffer)
+            self.buffer = grown
+        self.buffer[self.size].copy_(row.reshape(-1))
+        self.size += 1
+
+
 class NoveltySearch:
     """The meta-population and its archive.  `agents` are the M engines, `archive` the [A, d] view of the device archive
     (capacity doubled when full), `reward_weight` the current w, `weights` the w each generation shaped with, `selected`
@@ -115,8 +143,7 @@ class NoveltySearch:
             self.agents.append(natural_es.build_engine(c, theta0, kernels=self.kn, device=self.device))
         e = self.agents[0]
         self.d, self.N, dev = e.d0, e.N, self.device
-        self._archive = torch.zeros((_INITIAL_CAPACITY, self.d), dtype=torch.float32, device=dev)
-        self.size = 0
+        self.store = Archive(self.d, dev)
         self.agent_bc = torch.zeros((M, self.d), dtype=torch.float32, device=dev)     # each agent's latest behaviour
         self.bc = torch.zeros((self.N, self.d), dtype=torch.float32, device=dev)      # the members' behaviours
         self.novelty = torch.zeros(self.N, dtype=torch.float32, device=dev)
@@ -128,15 +155,18 @@ class NoveltySearch:
 
     @property
     def archive(self):
-        return self._archive[:self.size]
+        return self.store.rows
+
+    @property
+    def size(self):
+        return self.store.size
+
+    @property
+    def _archive(self):
+        return self.store.buffer
 
     def _archive_add(self, row):
-        if self.size == self._archive.shape[0]:
-            grown = torch.zeros((2 * self.size, self.d), dtype=torch.float32, device=self.device)
-            grown[:self.size].copy_(self._archive)
-            self._archive = grown
-        self._archive[self.size].copy_(row.reshape(-1))
-        self.size += 1
+        self.store.add(row)
 
     def test_agent(self, m, repetitions):
         """natural_es.test of agent m's theta (mean, std / repetitions); the same launch writes its behaviour, which joins
@@ -231,6 +261,128 @@ def test(config, solution, stats, ns=None, agent=0):
     """natural_es.test: the mean and std / test_repetitions of noiseless episodes of `solution` (None = the agent's
     current weights) with agent `agent`'s statistics; without `ns`, natural_es.test's host evaluation with `stats`."""
     return natural_es.test(config, solution, stats, engine=None if ns is None else ns.agents[agent])
+
+
+# ---- the genetic algorithm's novelty search: GA-NS, GA-NSR and GA-NSRA (Such et al. 2017) --------------------------------
+def check_ga_config(config):
+    """Raises ValueError unless train_ga can train `config`: what check_config and genetic.check_config accept, with one
+    agent."""
+    check_config(config)
+    M = settings(config)[3]
+    if M != 1:
+        raise ValueError('novelty.train_ga: ns_agents = %d; the genetic algorithm evolves one population (the '
+                         'meta-population of agents is an NES construction), so ns_agents must be 1' % M)
+    genetic.check_config(config)
+
+
+class NoveltyGA:
+    """The genetic algorithm's novelty search: genetic's (Worker, GeneticAlgorithm) pair `worker`, `ga`, and an archive
+    of behaviours.  Each generation's members write their behaviours from the evaluation's own launch (closed-loop:
+    des_rollout_eval_ga_bc; host-stepped: the final observations of their episodes).  Their novelty against the archive
+    (des_novelty) and their fitness select the next parents (des_ns_ga_order, reward weight w), and the test of the new
+    best row writes the behaviour that joins the archive: one row per generation, after the start point's.  Novelty is
+    measured against the archive alone, not against the current population.
+
+    `reward_weight` is the current w, `weights` the w of each selection, `best` the best test mean so far and
+    `best_theta` the weights that scored it.  `kernels` (default: distributedes_b200.ops) exists so the host logic can run
+    on CPU with an oracle-backed stand-in."""
+
+    def __init__(self, config, *, kernels=None, device=None):
+        check_ga_config(config)
+        self.config = config
+        self.worker, self.ga = genetic.build(config, kernels=kernels, device=device)
+        self.kn, self.device = self.worker.kn, self.worker.device
+        self.k, w, self.adaptive, _ = settings(config)
+        self.reward_weight = 1.0 if self.adaptive else w
+        self.d, self.N, dev = self.worker.source.d0, self.ga.N, self.device
+        self.store = Archive(self.d, dev)
+        self.bc = torch.zeros((self.N, self.d), dtype=torch.float32, device=dev)       # the members' behaviours
+        self.test_bc = torch.zeros((1, self.d), dtype=torch.float32, device=dev)
+        self.novelty = torch.zeros(self.N, dtype=torch.float32, device=dev)
+        self.weights = []
+        self.best, self.best_theta, self.stall = -np.inf, None, 0
+
+    @property
+    def archive(self):
+        return self.store.rows
+
+    def test(self, solution):
+        """genetic.test of one solution with the worker's statistics (mean, std / repetitions, improved); the same
+        episodes write its behaviour, which joins the archive.  Keeps the best test mean and its weights."""
+        c = self.config
+        row = genetic._row(solution, self.device)
+        rewards = self.worker.test_returns(row, c.test_repetitions, bc_out=self.test_bc)
+        self.store.add(self.test_bc[0])
+        mean, ste = np.mean(rewards), np.std(rewards) / c.repetitions
+        improved = bool(mean > self.best)
+        if improved:
+            self.best, self.best_theta = mean, row.reshape(-1).cpu().numpy().copy()
+        return mean, ste, improved
+
+    def adapt(self, improved):
+        """GA-NSRA's schedule of w after a generation's test (NSRA-ES's); a fixed weight stays as it is."""
+        if self.adaptive:
+            self.reward_weight, self.stall = _adapted(self.reward_weight, self.stall, improved)
+
+    def evaluate(self):
+        """The generation's fitness [N] (worker.run) and the members' behaviours (self.bc) from one evaluation."""
+        return self.worker.run(self.ga, bc_out=self.bc)
+
+    def select(self, fitness):
+        """The members' novelty against the archive and the selection of the next parents with weight w."""
+        self.kn.novelty(self.bc, self.archive, self.k, out=self.novelty)
+        self.weights.append(self.reward_weight)
+        return self.ga.tell(fitness, self.novelty, self.reward_weight)
+
+
+def build_ga(config, *, kernels=None, device=None):
+    """The NoveltyGA of train_ga(config)."""
+    return NoveltyGA(config, kernels=kernels, device=device)
+
+
+def train_ga(config, nsga=None):
+    """The genetic algorithm's novelty search on `config`; returns [training_rewards, training_steps,
+    training_timestamps] with genetic.train's loop, stopping rules, steps accounting and log lines.  ns_reward_weight 0
+    is GA-NS, 0.5 (the default) GA-NSR and 'adaptive' GA-NSRA (w from 1, NSRA-ES's schedule); truncation and elites are
+    genetic's.  At ns_reward_weight = 1 it is genetic.train(config), bit for bit."""
+    check_ga_config(config)
+    nsga = nsga if nsga is not None else build_ga(config)
+    worker, ga = nsga.worker, nsga.ga
+    total_steps = 0
+    initial_time = time.time()
+    training_rewards, training_steps, training_timestamps = [], [], []
+    test_mean, test_ste, _ = nsga.test(config.initial_weight)
+    logger.info('total steps %d, %f(%f)' % (total_steps, test_mean, test_ste))
+    training_rewards.append(test_mean)
+    training_steps.append(0)
+    training_timestamps.append(0)
+    generation = 0
+    while True:
+        f = nsga.evaluate()
+        total_steps += worker.steps(ga.N)
+        best = float(f.max())
+        nsga.select(f)
+        elapsed_time = time.time() - initial_time
+        test_mean, test_ste, improved = nsga.test(ga.best)
+        nsga.adapt(improved)
+        logger.info('total steps %d, test %f(%f), best %f, elapsed time %f'
+                    % (total_steps, test_mean, test_ste, best, elapsed_time))
+        training_rewards.append(test_mean)
+        training_steps.append(total_steps)
+        training_timestamps.append(elapsed_time)
+        worker.merge_obs_stats(ga.N)
+        generation += 1
+        if config.max_steps and total_steps > config.max_steps:
+            break
+        if getattr(config, 'max_generations', 0) and generation >= config.max_generations:
+            break
+    return [training_rewards, training_steps, training_timestamps]
+
+
+def test_ga(config, solution, stats, nsga=None):
+    """genetic.test: the mean and std / repetitions of test_repetitions noiseless episodes of `solution` with the
+    worker's statistics (`stats`, if given, replaces them first); without `nsga`, with a new genetic.Worker."""
+    return genetic.test(config, solution, stats, worker=None if nsga is None else nsga.worker)
 
 
 # ---- sweeps: R one-agent novelty searches of different configs trained together on one GPU ------------------------------

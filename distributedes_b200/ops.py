@@ -448,3 +448,5 @@ from .ops_record import rollout_record, rollout_record_solutions  # noqa: E402,F
 from .ops_ga import ga_order, ga_order_workspace, ga_rows, rollout_eval_ga  # noqa: E402,F401
 # Novelty search's ops (novelty.py): defined in ops_novelty on this module's checks.
 from .ops_novelty import novelty, ns_shape, ns_shape_workspace, rollout_eval_bc  # noqa: E402,F401
+# The genetic algorithm's novelty search's ops (novelty.NoveltyGA): defined in ops_ga_novelty on this module's checks.
+from .ops_ga_novelty import ns_ga_order, ns_ga_order_workspace, rollout_eval_ga_bc  # noqa: E402,F401

@@ -38,6 +38,15 @@ def rollout_eval_ga(parents, n_elites, *, env=0, hidden, horizon=200, repetition
     """Closed-loop fitness of members [member_offset, member_offset + n_local) of the generation whose table is
     parents[n_parents, P] (des_rollout_eval_ga): rollout_eval_solutions of ga_rows' rows, bit for bit, with no rows in
     memory."""
+    return _rollout_ga('des_rollout_eval_ga', parents, n_elites, env, hidden, horizon, repetitions, sigma, clip,
+                       action_noise_std, seed, generation, state, member_offset, n_local, obs_stats, totals_out,
+                       workspace, out, episodes_out)
+
+
+def _rollout_ga(fn, parents, n_elites, env, hidden, horizon, repetitions, sigma, clip, action_noise_std, seed,
+                generation, state, member_offset, n_local, obs_stats, totals_out, workspace, out, episodes_out,
+                bc_out=None):
+    """The launch of rollout_eval_ga, and with `bc_out` [n_local, d0] that of rollout_eval_ga_bc (ops_ga_novelty)."""
     d0, A = _env_dims(env)
     P, mlp = _mlp(d0, int(hidden), A)
     n_parents, _, n_elites = _table(parents, n_elites)
@@ -46,13 +55,14 @@ def rollout_eval_ga(parents, n_elites, *, env=0, hidden, horizon=200, repetition
         out = torch.empty(n_local, dtype=F32, device=dev)
     if totals_out is not None and workspace is None:
         workspace = torch.empty(max(n_local, 1) * w, dtype=F64, device=dev)
-    _launch('des_rollout_eval_ga', parents, 'parents', _ptr(out, 'out', F32, n_local, dev),
+    bc = () if bc_out is None else (_ptr(bc_out, 'bc_out', F32, n_local * d0, dev),)
+    _launch(fn, parents, 'parents', _ptr(out, 'out', F32, n_local, dev),
             _ptr(episodes_out, 'episodes_out', F32, n_local * reps, dev, True),
             _ptr(totals_out, 'totals_out', F64, w, dev, True),
             _ptr(parents, 'parents', F32, n_parents * P, need=mlp + ' n_parents x P ='), n_parents, n_elites,
             _ptr(obs_stats, 'obs_stats', F32, w, dev, True), int(env), Dims(d0, hidden, A, horizon), reps, float(sigma),
             float(clip), float(action_noise_std), int(seed), int(generation),
-            _ptr(state, 'state', U8, STATE_BYTES, dev, True), int(member_offset), n_local, 0, *_ws(workspace, dev))
+            _ptr(state, 'state', U8, STATE_BYTES, dev, True), int(member_offset), n_local, 0, *bc, *_ws(workspace, dev))
     return out
 
 

@@ -290,6 +290,35 @@ DES_API size_t des_ns_shape_workspace_bytes(int64_t N);
 DES_API int des_ns_shape(float *shaped_out_dev, const float *fitness_dev, const float *novelty_dev, int64_t N,
                          double reward_weight, void *workspace_dev, size_t workspace_bytes, void *stream);
 
+/* ---- novelty search for the genetic algorithm: GA-NS, GA-NSR and GA-NSRA (Such et al. 2017) ----------------------------
+ *
+ * The genetic algorithm above, its truncation selection ordering a blend of fitness and novelty ranks.  The behaviour and
+ * the novelty are those of "novelty search" above.
+ *   Key        key_i = fmaf(w, c_f[i], fp32(1 - w) * c_n[i]) in fp32, with c_f = des_centered_rank(-fitness) and
+ *              c_n = des_centered_rank(-novelty), w and 1 - w converted as des_ns_shape converts them.  A NaN fitness and a
+ *              NaN novelty each rank worst in their own term; -0 == +0.
+ *   Selection  the members in ascending order of key, ties to the lower index.  At w = 1 the key is c_f, whose entries
+ *              are distinct and finite, so the order is des_ga_order's bit for bit (ties and NaN included); at w = 0 it
+ *              is by novelty, descending.
+ *
+ * des_rollout_eval_ga_bc   des_rollout_eval_ga that also writes bc_out_dev[n_local][3], each member's behaviour.  Fitness,
+ *                          episode returns and observation totals are des_rollout_eval_ga's, bit for bit; its checks are
+ *                          des_rollout_eval_ga's, and bc_out_dev may be NULL only when n_local == 0.
+ * des_ns_ga_order          order_out[T] int32: the members in positions 0 .. T-1 of the selection order of fitness_dev[N]
+ *                          and novelty_dev[N].  2 <= N <= 2^24 (above, the fp32 rounding of r / (N - 1) - 0.5 can give two
+ *                          ranks one key), 1 <= T <= N, 0 <= reward_weight <= 1.  workspace:
+ *                          des_ns_ga_order_workspace_bytes(N) bytes, or DES_ERR_WORKSPACE.  The ranks take
+ *                          des_centered_rank's counting path up to N = 2048 and its bucketed path above. */
+DES_API int des_rollout_eval_ga_bc(float *fitness_out_dev, float *episode_returns_out_dev, double *obs_totals_out_dev,
+                                   const float *parents_dev, int64_t n_parents, int64_t n_elites, const float *obs_stats_dev,
+                                   int env, des_dims dims, int32_t repetitions, double sigma, double clip,
+                                   double action_noise_std, uint64_t seed, uint64_t generation, const des_state *state_dev,
+                                   int64_t member_offset, int64_t n_local, int noiseless, float *bc_out_dev,
+                                   void *workspace_dev, size_t workspace_bytes, void *stream);
+DES_API size_t des_ns_ga_order_workspace_bytes(int64_t N);
+DES_API int des_ns_ga_order(int32_t *order_out_dev, const float *fitness_dev, const float *novelty_dev, int64_t N,
+                            int64_t T, double reward_weight, void *workspace_dev, size_t workspace_bytes, void *stream);
+
 /* Chan merge (utils.py:85-96) of a batch given by obs_totals_dev = [sum (d0) | sum of squares (d0) | count] into
  * stats_dev [m|v|n]  (natural_es.py:85-89 after the cross-rank sum of the totals). */
 DES_API int des_obs_stats_merge_totals(float *stats_dev, const double *obs_totals_dev, int32_t state_dim, void *stream);
