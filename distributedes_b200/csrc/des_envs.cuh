@@ -1,13 +1,15 @@
-// The closed-loop Pendulum rollout kernel (des_envs.cu), in a header for the translation units that instantiate it.
-// des_envs.cu instantiates every kernel of des_rollout_eval[_mirrored|_solutions|_runs|_sweep], and des_envs_sweep.cu the
-// row-mode sweep kernels of des_rollout_eval_solutions_sweep: one unit of their own keeps ptxas's code for the others
-// exactly what it was before CMA-ES sweeps existed (instantiated together, rollout_pendulum_kernel<8, true, RollArgs>
-// came out scheduled differently).  des_envs_record.cu instantiates the recording kernels of des_rollout_record[_solutions]
-// (RecordArgs) in a unit of their own for the same reason, des_envs_ga.cu the genetic algorithm's kernels of
-// des_rollout_eval_ga (GaArgs) and des_envs_ga_sweep.cu those of its sweeps, des_rollout_eval_ga_sweep (GaSweepArgs).
-// des_envs_bc.cu instantiates the behaviour-writing kernels of des_rollout_eval_bc (BcArgs) for novelty search, and
-// des_envs_bc_sweep.cu those of its sweeps, des_rollout_eval_bc_sweep (BcSweepArgs).  des_envs_ga_bc.cu instantiates the
-// genetic algorithm's behaviour-writing kernels of des_rollout_eval_ga_bc (GaBcArgs) for its novelty search.
+// The closed-loop Pendulum rollout kernel and its launcher rollout_kernels (des_envs.cu), in a header for the units that
+// instantiate them.  Each unit compiles the kernels of its own entry points:
+//   des_envs.cu            RollArgs, RunArgs, SweepArgs   des_rollout_eval[_mirrored|_solutions|_runs|_sweep]
+//   des_envs_sweep.cu      SweepArgs in row mode          des_rollout_eval_solutions_sweep
+//   des_envs_record.cu     RecordArgs                     des_rollout_record[_solutions]
+//   des_envs_ga.cu         GaArgs                         des_rollout_eval_ga
+//   des_envs_ga_sweep.cu   GaSweepArgs                    des_rollout_eval_ga_sweep
+//   des_envs_bc.cu         BcArgs                         des_rollout_eval_bc
+//   des_envs_bc_sweep.cu   BcSweepArgs                    des_rollout_eval_bc_sweep
+//   des_envs_ga_bc.cu      GaBcArgs                       des_rollout_eval_ga_bc
+// The split keeps ptxas's code for des_envs.cu's kernels what it was before the others existed: instantiated together
+// with the row-mode sweep kernels, rollout_pendulum_kernel<8, true, RollArgs> came out scheduled differently.
 #pragma once
 #include <type_traits>
 #include "des_common.cuh"
@@ -428,23 +430,29 @@ __global__ void __launch_bounds__(32) rollout_pendulum_kernel(Args a) {
     }
 }
 
-// rollout_pendulum_kernel<H / 16, true, SweepArgs> over `blocks` CTAs (des_rollout_eval_solutions_sweep), defined in
-// des_envs_sweep.cu
-int rollout_rows_sweep_launch(const SweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, rows_mode, RecordArgs> over `blocks` CTAs (des_rollout_record[_solutions]), defined in
-// des_envs_record.cu
-int rollout_record_launch(const RecordArgs &a, int H, bool rows_mode, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, false, GaArgs> over `blocks` CTAs (des_rollout_eval_ga), defined in des_envs_ga.cu
-int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, false, GaSweepArgs> over `blocks` CTAs (des_rollout_eval_ga_sweep), defined in
-// des_envs_ga_sweep.cu
-int rollout_ga_sweep_launch(const GaSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, false, BcArgs> over `blocks` CTAs (des_rollout_eval_bc), defined in des_envs_bc.cu
-int rollout_bc_launch(const BcArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, false, BcSweepArgs> over `blocks` CTAs (des_rollout_eval_bc_sweep), defined in
-// des_envs_bc_sweep.cu
-int rollout_bc_sweep_launch(const BcSweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
-// rollout_pendulum_kernel<H / 16, false, GaBcArgs> over `blocks` CTAs (des_rollout_eval_ga_bc), defined in des_envs_ga_bc.cu
-int rollout_ga_bc_launch(const GaBcArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st);
+// Launches rollout_pendulum_kernel<H / 16, kRows, Args> over `blocks` CTAs of one warp.  Not inline, so that the
+// extern template declarations below keep des_envs.cu from compiling the kernels another unit instantiates.
+template <bool kRows, typename Args>
+int rollout_kernels(const Args &a, int H, unsigned blocks, size_t smem, cudaStream_t st) {
+    void (*kernel)(Args);
+    switch (H / 16) {                    // R = H/16 hidden units per lane
+        case 1: kernel = rollout_pendulum_kernel<1, kRows, Args>; break;
+        case 2: kernel = rollout_pendulum_kernel<2, kRows, Args>; break;
+        case 4: kernel = rollout_pendulum_kernel<4, kRows, Args>; break;
+        case 6: kernel = rollout_pendulum_kernel<6, kRows, Args>; break;
+        default: kernel = rollout_pendulum_kernel<8, kRows, Args>; break;
+    }
+    return launch_smem("rollout_pendulum_kernel", kernel, blocks, 32, smem, st, a);
+}
+
+// The instantiations of the other units (see the top of this file); des_envs.cu instantiates the rest.
+extern template int rollout_kernels<true, SweepArgs>(const SweepArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, RecordArgs>(const RecordArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<true, RecordArgs>(const RecordArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, GaArgs>(const GaArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, GaSweepArgs>(const GaSweepArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, BcArgs>(const BcArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, BcSweepArgs>(const BcSweepArgs &, int, unsigned, size_t, cudaStream_t);
+extern template int rollout_kernels<false, GaBcArgs>(const GaBcArgs &, int, unsigned, size_t, cudaStream_t);
 
 }  // namespace des

@@ -4,16 +4,6 @@
 
 namespace des {
 
-int rollout_ga_launch(const GaArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st) {
-    void (*kernel)(GaArgs);
-    switch (H / 16) {                    // R = H/16 hidden units per lane
-        case 1: kernel = rollout_pendulum_kernel<1, false, GaArgs>; break;
-        case 2: kernel = rollout_pendulum_kernel<2, false, GaArgs>; break;
-        case 4: kernel = rollout_pendulum_kernel<4, false, GaArgs>; break;
-        case 6: kernel = rollout_pendulum_kernel<6, false, GaArgs>; break;
-        default: kernel = rollout_pendulum_kernel<8, false, GaArgs>; break;
-    }
-    return launch_smem("rollout_pendulum_kernel", kernel, blocks, 32, smem, st, a);
-}
+template int rollout_kernels<false, GaArgs>(const GaArgs &, int, unsigned, size_t, cudaStream_t);
 
 }  // namespace des

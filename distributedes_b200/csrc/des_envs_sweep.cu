@@ -4,16 +4,6 @@
 
 namespace des {
 
-int rollout_rows_sweep_launch(const SweepArgs &a, int H, unsigned blocks, size_t smem, cudaStream_t st) {
-    void (*kernel)(SweepArgs);
-    switch (H / 16) {                    // R = H/16 hidden units per lane
-        case 1: kernel = rollout_pendulum_kernel<1, true, SweepArgs>; break;
-        case 2: kernel = rollout_pendulum_kernel<2, true, SweepArgs>; break;
-        case 4: kernel = rollout_pendulum_kernel<4, true, SweepArgs>; break;
-        case 6: kernel = rollout_pendulum_kernel<6, true, SweepArgs>; break;
-        default: kernel = rollout_pendulum_kernel<8, true, SweepArgs>; break;
-    }
-    return launch_smem("rollout_pendulum_kernel", kernel, blocks, 32, smem, st, a);
-}
+template int rollout_kernels<true, SweepArgs>(const SweepArgs &, int, unsigned, size_t, cudaStream_t);
 
 }  // namespace des
